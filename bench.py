@@ -10,6 +10,7 @@ step   : one pass of the hot path over the whole 4000-step sequence.
 
     python bench.py --gpus N --steps K --warmup W          # this repo
     python bench.py --impl reference ...                   # CPU arm (oracle port)
+    python bench.py ... --dump-outputs DIR                 # also write the last timed step's outputs as .npy
 
 N > 1: one process per GPU (torchrun).  `value` stays C2: the single-state path
 does not shard ("replicas only", DESIGN.md), every GPU evolves the same Sequence,
@@ -117,17 +118,15 @@ def measured_peak() -> tuple[float, str]:
             return float(json.load(open(p))["hbm_gbs"]), "measured (MEASURED_PEAKS.json hbm_gbs)"
         except Exception:
             pass
-    return 6650.0, "fallback (B200_PROFILING.md 6.65 TB/s)"
+    return 3350.0, "data sheet (H100 SXM HBM3, 3.35 TB/s; not a measured figure)"
 
 
-def ncu_traffic_per_launch() -> float | None:
-    """dram bytes per launch of the dominant kernel from the committed ncu summary."""
-    for name in ("r02_taylor_stage_kernel_summary.json", "r02_stage_kernel_summary.json", "r01_stage_kernel_summary.json"):
-        try:
-            return float(json.load(open(os.path.join(ROOT, "profiles", name)))["dram_bytes_per_launch"])
-        except Exception:
-            continue
-    return None
+def dump_outputs(out_dir: str, state: np.ndarray, dens: np.ndarray) -> None:
+    """What the timed path hands its caller after the last timed step: the final state vector (real and imaginary
+    parts, float64 [D, 2], 16 MiB at the default 20 atoms) and the per-atom Rydberg densities computed from it."""
+    os.makedirs(out_dir, exist_ok=True)
+    np.save(os.path.join(out_dir, "final_state.npy"), np.ascontiguousarray(np.stack([state.real, state.imag], axis=-1)))
+    np.save(os.path.join(out_dir, "rydberg_density.npy"), np.asarray(dens, dtype=np.float64))
 
 
 # --------------------------------------------------------------------------
@@ -368,9 +367,7 @@ def c5_leg(local: int, stream, peak: float) -> dict:
 def run_gpu(args) -> None:
     import torch
 
-    from pulser_b200 import build
-    build.build()
-    from pulser_b200 import engine
+    from pulser_b200 import engine   # the library build() left in the tree; nothing is compiled here
 
     world = int(os.environ.get("WORLD_SIZE", "1"))
     rank = int(os.environ.get("RANK", "0"))
@@ -424,6 +421,8 @@ def run_gpu(args) -> None:
     probs = plan.probabilities()[0]
     idx = np.arange(D)
     dens = np.array([probs[((idx >> (N_ATOMS - 1 - k)) & 1) == 0].sum() for k in range(N_ATOMS)])
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, plan.get_state()[0], dens)
     total_ms = float(np.sum(times_ms))
     t_all = torch.tensor([total_ms], dtype=torch.float64, device="cuda")
     obs = torch.tensor(dens, dtype=torch.float64, device="cuda")
@@ -489,15 +488,14 @@ def run_gpu(args) -> None:
                     "api": "pulser_b200.engine.DevicePlan(spec).set_state/propagate/get_state (C-ABI, host buffers)"},
             "gpu_launches": int(launches),
             "roofline": {"bound": "hbm", "achieved": achieved, "peak": peak, "unit": "GB/s", "frac": achieved / peak,
-                         "traffic": ncu_traffic_per_launch(), "peak_source": peak_src,
+                         "peak_source": peak_src,
                          "kernel": "stage_d2_taylor_kernel (fused H-apply + Taylor-order update + accumulation; one order per launch)",
                          "algorithmic_bytes_per_launch": alg_bytes,
                          "h_applies_per_launch": applies_per_launch,
                          "avg_launch_us": per_launch_s * 1e6,
                          "note": "achieved = algorithmic bytes / (CUDA-event time of the propagation / launches), launch "
-                                 "gaps included; traffic = dram read+write per launch from the committed ncu --set full "
-                                 "capture (profiles/r02_taylor_stage_kernel_summary.json), cold L2 at every ncu replay; in the "
-                                 "timed run the 16 MiB state and its ring buffers stay L2-resident"},
+                                 "gaps included; in the timed run the 16 MiB state fits the H100's 50 MB L2, its Taylor ring "
+                                 "buffers only partly"},
         }
         if c4 is not None:
             line["c4"] = c4
@@ -519,6 +517,8 @@ def main() -> None:
     ap.add_argument("--steps", type=int, default=5)
     ap.add_argument("--warmup", type=int, default=3)
     ap.add_argument("--impl", default="b200", choices=["b200", "reference"])
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="after the timed steps, write the last step's final state and Rydberg densities as DIR/<name>.npy")
     args = ap.parse_args()
     if args.impl == "reference":
         run_reference(args)

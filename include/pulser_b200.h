@@ -1,5 +1,5 @@
 /*
- * pulser_b200 -- C ABI of the B200-native time-evolution hot path.
+ * pulser_b200 -- C ABI of the H100-native (sm_90a) time-evolution hot path.
  *
  * The reference (pasqal-io/Pulser) is pure Python and has no FFI: its "plugin
  * boundary" for this path is the pair

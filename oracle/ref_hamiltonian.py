@@ -16,7 +16,7 @@ Only ``tests/``, ``__graft_entry__.smoke()`` and ``bench.py``'s CPU-baseline
 legs may import this package.
 
 Every function cites the reference lines it follows; paths are relative to
-``/root/reference/pulser-simulation/pulser_simulation/``.
+``pulser-simulation/pulser_simulation/`` of the Pulser repository.
 """
 from __future__ import annotations
 

@@ -1,4 +1,4 @@
-"""pulser_b200: B200-native time-evolution emulator for Pulser sequences.
+"""pulser_b200: H100-native (sm_90a) time-evolution emulator for Pulser sequences.
 
 Public names mirror ``pulser_simulation/__init__.py`` (``QutipEmulator`` -> ``B200Emulator``, ``QutipBackendV2`` ->
 ``B200Backend``, ``QutipBackend`` -> ``B200LegacyBackend``, ``QutipConfig / QutipState / QutipOperator`` ->

@@ -77,7 +77,7 @@ def _load() -> C.CDLL:
     if not os.path.exists(LIB_PATH):
         raise LibraryMissing(
             f"{LIB_PATH} not found: build it with "
-            "`python -m pulser_b200.build` (nvcc, sm_100a). "
+            "`python -m pulser_b200.build` (nvcc, sm_90a). "
             "pulser_b200 has no CPU fallback."
         )
     lib = C.CDLL(LIB_PATH)

@@ -591,7 +591,7 @@ def _state_aggregators(results: list) -> dict:
 
 
 class B200Backend(EmulatorBackend):
-    """Emulate a sequence on a B200 through the generic ``pulser.backend`` API."""
+    """Emulate a sequence on an H100 through the generic ``pulser.backend`` API."""
 
     default_config = B200Config(observables=[BitStrings(evaluation_times=[1.0]), StateResult()])
     _config: B200Config
@@ -815,7 +815,7 @@ class B200LegacyBackend(pulser.backend.abc.Backend):
         self._sim_obj.set_initial_state(self._config.initial_state)
 
     def run(self, progress_bar: bool = False, **options: Any) -> Any:
-        """Emulates the sequence on the B200 (``QutipBackend.run``, ``qutip_backend.py:89-118``); QuTiP solver
+        """Emulates the sequence on the GPU (``QutipBackend.run``, ``qutip_backend.py:89-118``); QuTiP solver
         options are accepted and ignored like in ``B200Emulator.run``."""
         with warnings.catch_warnings():
             warnings.simplefilter("ignore", DeprecationWarning)

@@ -1,4 +1,4 @@
-"""Build the C-ABI shared library in-tree with nvcc for sm_100a."""
+"""Build the C-ABI shared library in-tree with nvcc for sm_90a (H100)."""
 from __future__ import annotations
 
 import os
@@ -36,7 +36,7 @@ def build(force: bool = False, verbose: bool = False) -> str:
         return LIB
     cmd = [
         _nvcc(),
-        "-gencode", "arch=compute_100a,code=sm_100a",
+        "-gencode", "arch=compute_90a,code=sm_90a",
         "-lineinfo", "-O3", "-std=c++17",
         "-Xcompiler", "-fPIC,-O2,-Wall",
         "-Xptxas", "-v" if verbose else "-O3",

@@ -1,4 +1,4 @@
-// sm_100a kernels of the matrix-free propagator.
+// sm_90a (H100) kernels of the matrix-free propagator.
 //
 // Hot op (one Clenshaw stage of the Chebyshev expansion of exp(-iG)):
 //     out[s] = c_psi*psi[s] + c_b2*b2[s] + c_g * (Gt v)[s]
@@ -612,15 +612,15 @@ stage_d2_rb_kernel(const __grid_constant__ StageArgs2 m) {
 }
 
 // ---- d = 2 stage kernel with partner-sum forwarding (uniform drives) ---------------------------------------------
-// The single-pass kernel above sits at the L2 throughput cap (~6300 B/clk chip-wide): (N - TBITS) x 16 B of partner
-// loads per amplitude dominate its L2 sectors (profiles/r02_l2_hint_experiment.json).  Here consecutive Clenshaw
+// The single-pass kernel above is bound by L2 throughput: (N - TBITS) x 16 B of partner loads per amplitude dominate
+// its L2 sectors.  Here consecutive Clenshaw
 // stages alternate between two tile geometries with complementary flip sets -- A: the TBITS low bits; B: the
 // hb = min(N - TBITS, TBITS - 2) bits above them, gathered as 2^hb rows of 2^(TBITS - hb) amplitudes -- and a stage
 // receives the partner sums over the OTHER geometry's flips from the stage that produced its input (w_in, 16 B per
 // amplitude) and emits the sums of its own result over ITS flips (w_out): 104 B of L2 traffic per amplitude and stage
 // instead of 72 + 16 (N - TBITS).  Bits above TBITS + hb (N > 20) stay coalesced partner loads in both geometries.
-// Unlike the round-1 attempt (latency-bound: operand loads after the gathers, profiles/r02_forwarding_kernel_ncu_
-// summary.json) every global operand of the stage is requested BEFORE the wait on the tile copy and folded into the
+// Issuing the operand loads after the gathers leaves the kernel latency-bound, so every global operand of the stage
+// is requested BEFORE the wait on the tile copy and folded into the
 // accumulators as it arrives, so a CTA has one exposed memory latency.
 template <bool REAL_G, int TBITS, int RB>
 __global__ void __launch_bounds__(1 << (TBITS - RB), 2) stage_d2_fwd_kernel(const __grid_constant__ StageArgs2 m) {

@@ -206,7 +206,7 @@ struct Plan {
     bool state_set = false;
     int tile_bits = 12;
     int max_extra = 3;
-    int sm_count = 148;
+    int sm_count = 132;
     bool force_v1 = false;
     int reg_bits = 3;
     bool use_dual = true;
@@ -490,10 +490,9 @@ static bool fwd_eligible(const Plan& P, const std::vector<PassGeom>& passes) {
     if (!P.use_fwd || !is_d2path(P) || P.force_v1 || !P.all_uniform() || P.B != 1) return false;
     if (P.tile_bits != 11 || P.reg_bits != 3) return false;
     if (passes.size() != 1 || passes[0].hi_bits != 0 || passes[0].lo_bits != 11) return false;
-    // Measured (profiles/r02_forwarding_ab.jsonl): the second in-tile gather and the 64-byte rows of the high-bit
-    // tile cost as much shared-memory / LSU time as the forwarded sums save in L2 traffic once N >= 20 (N = 20:
-    // 24.0 vs 21.9 us per apply, N = 22: 123 vs 93), while at N = 18 (256-byte rows) forwarding wins 5.55 vs 6.35 us:
-    // it is used for the registers in between only.
+    // The second in-tile gather and the 64-byte rows of the high-bit tile cost as much shared-memory / LSU time as the
+    // forwarded sums save in L2 traffic once N >= 20, while at N = 18 (256-byte rows) forwarding saves L2 traffic
+    // without that penalty: it is used for the registers in between only (tools/fwd_ab.py measures both sides).
     return P.n >= env_int("PB200_FWD_MIN_N", 17) && P.n <= env_int("PB200_FWD_MAX_N", 19);
 }
 
@@ -2111,7 +2110,7 @@ static void propagate_taylor(Plan& P, double t_start, double t_stop, const pb200
     Plan::TaylorCache& C = P.tay;
     taylor_knot_widths(P);
     // Step length: rho = h W <= rho_max, lowered where the fp64 cancellation of the series would eat the tolerance.  The
-    // rounding error of a step grows like e^rho: ~0.05 eps e^rho measured (profiles/r02_taylor_rho_sweep.jsonl: 6e-12 per
+    // rounding error of a step grows like e^rho: ~0.05 eps e^rho measured (tools/taylor_rho_sweep.py: 6e-12 per
     // step at rho = 14, 1.4e-10 at 18), random from step to step, n ~ (int W dt) / rho steps over the whole sequence;
     // it may use a fifth of the tolerance.  At the default 1e-8 this never binds (17 > 14 for C2, C4, C5).
     const double kRoundUnit = 0.05 * 1.1102230246251565e-16;

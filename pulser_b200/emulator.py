@@ -143,7 +143,7 @@ class _NoiseModelConfig:
 
 
 class B200Emulator:
-    r"""Emulator of a pulse sequence on a B200 GPU.
+    r"""Emulator of a pulse sequence on an H100 GPU.
 
     Args: identical to ``QutipEmulator`` (simulation.py:84-141), plus
         ``interp_order`` (QobjEvo coefficient interpolation order, 3 = QuTiP 5

@@ -1,4 +1,4 @@
-"""Result objects of the B200 emulator: qutip-free mirrors of the reference's.
+"""Result objects of the GPU emulator: qutip-free mirrors of the reference's.
 
 * ``StateVector``    -- the minimal ``qutip.Qobj`` surface the reference's
   result classes and its users touch (``full()``, ``isket``, ``shape``,

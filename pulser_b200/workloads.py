@@ -1,6 +1,6 @@
 """Synthetic workloads of BASELINE.json ``configs`` as plain-array specs.
 
-The GPU box has neither ``/root/reference`` nor pulser, so the benchmark and
+pulser is an optional dependency, so the benchmark and
 the GPU parity tests build their inputs here with numpy only, restating what
 ``pulser.sampler.sample`` + ``HamiltonianData`` produce for these sequences
 (waveform formulas: reference ``pulser-core/pulser/waveforms.py:584`` constant,
@@ -8,8 +8,8 @@ the GPU parity tests build their inputs here with numpy only, restating what
 ``pulser-core/pulser/devices/interaction_coefficients/``; interaction matrix
 ``pulser-core/pulser/_hamiltonian_data/hamiltonian_data.py:607-611``; the
 zero-padded extra sample ``pulser-simulation/pulser_simulation/simulation.py:172-173``).
-``tests/test_workloads_vs_pulser.py`` checks every builder against the real
-pulser objects whenever pulser is importable.
+``tests/test_oracle_cpu.py`` checks the builders against what the real
+pulser objects produce (stored in ``tests/golden/pulser_*.npz``).
 
 Definitions follow SURVEY.md section 8(d).
 """

@@ -1,15 +1,17 @@
-"""Generate the committed golden fixtures from the REAL reference (pulser-core
-imported from /root/reference) plus the tight-tolerance oracle.
+"""Generate the committed golden fixtures from the REAL reference (pulser-core,
+staged under oracle/_ref by oracle/build_ref.py) plus the tight-tolerance oracle.
 
-Run in the build container only (the GPU box has no /root/reference):
-    python tests/golden/make_golden.py [--extra | --xy | --slm | --counters]
+Run where the Pulser source is available:
+    python tests/golden/make_golden.py [--extra | --xy | --slm | --counters | --workloads]
 
 Each ``*.npz`` holds a HamiltonianSpec (what the reference's Hamiltonian
 constructor receives, extracted from real pulser objects), an initial state and
 the expected output.  Sources of the expected values:
   * ``ref_*``  : numbers hard-coded in the reference's own tests
                  (tests/pulser_simulation/test_simulation.py etc., cited below);
-  * ``orc_*``  : oracle (oracle/evolve.py, DOP853 rtol 1e-13) on the same spec.
+  * ``orc_*``  : oracle (oracle/evolve.py, DOP853 rtol 1e-13) on the same spec;
+  * ``pulser_*``: the spec pulser-core itself builds for a BASELINE workload
+                 (``--workloads``), which pulser_b200.workloads restates.
 """
 import os
 import sys
@@ -164,7 +166,7 @@ def main():
         save(f"orc_noisy_traj{i}", spec, psi0=psi0, orc_final=oracle_final(spec, psi0), reps=reps)
 
 
-if __name__ == "__main__" and "--extra" not in sys.argv and "--xy" not in sys.argv and "--slm" not in sys.argv and "--counters" not in sys.argv:
+if __name__ == "__main__" and not {"--extra", "--xy", "--slm", "--counters", "--workloads"} & set(sys.argv):
     main()
 
 
@@ -563,3 +565,67 @@ if __name__ == "__main__" and "--counters" in sys.argv:
     if "--expect-only" not in sys.argv:
         eom_counters()
     expect_leakage()
+
+
+def workloads():
+    """What pulser-core builds for the sequences pulser_b200.workloads restates (tests/test_oracle_cpu.py)."""
+    from pulser_b200 import workloads as W
+
+    seq = Sequence(Register.square(2, spacing=6.0, prefix="q"), MockDevice)
+    seq.declare_channel("ch", "rydberg_global")
+    seq.add(Pulse.ConstantPulse(1000, 2 * np.pi, np.pi, 0), "ch")
+    save("pulser_c1", specs_of(seq)[0][0])
+
+    om = 2 * np.pi * 1.5
+    U = om / 2
+
+    def sweep(s):
+        s.add(Pulse.ConstantDetuning(RampWaveform(500, 0, om), -6 * U, 0), "ch")
+        s.add(Pulse.ConstantAmplitude(om, RampWaveform(2500, -6 * U, 2 * U), 0), "ch")
+        s.add(Pulse.ConstantDetuning(RampWaveform(1000, om, 0), 2 * U, 0), "ch")
+
+    n = 9
+    seq = Sequence(Register.from_coordinates(W.disc_register(n, 38.0, 5.0, n), center=False, prefix="q"), AnalogDevice)
+    seq.declare_channel("ch", "rydberg_global")
+    sweep(seq)
+    save("pulser_c2_n9", specs_of(seq)[0][0])
+
+    n = 5
+    seq = Sequence(Register.from_coordinates(W.disc_register(n, 22.0, 6.0, 100 + n), center=False, prefix="q"),
+                   MockDevice)
+    seq.declare_channel("ram", "raman_global")
+    seq.declare_channel("ryd", "rydberg_global")
+    seq.add(Pulse.ConstantDetuning(BlackmanWaveform(500, np.pi / 2), 0, 0), "ram")
+    seq.add(Pulse.ConstantDetuning(BlackmanWaveform(1000, np.pi), 0, 0), "ryd", protocol="wait-for-all")
+    seq.add(Pulse.ConstantDetuning(BlackmanWaveform(500, np.pi / 2), 0, 0), "ram", protocol="wait-for-all")
+    save("pulser_c3_n5", specs_of(seq)[0][0])
+
+    # C4: the first two noise trajectories pulser draws under np.random.seed(3), with the draws themselves.  The
+    # per-qubit tables (16 x 4001 samples) are kept as SHA-256 digests of their bytes plus every 40th sample.
+    import hashlib
+
+    seq = Sequence(Register.square(4, spacing=6.0, prefix="q"), MockDevice)
+    seq.declare_channel("ch", "rydberg_global")
+    sweep(seq)
+    np.random.seed(3)
+    hd, T = hdata(seq, NoiseModel(temperature=50.0, amp_sigma=0.05, laser_waist=175.0), 2)
+    for k, (tr, ns, _) in enumerate(hd.noisy_samples):
+        d = spec_from_pulser(ns, tr, hd.basis_data, hd.lindblad_data, 1.0, T).drives[0]
+        coef, det = np.ascontiguousarray(d.coef, dtype=np.complex128), np.ascontiguousarray(d.det, dtype=np.float64)
+        np.savez_compressed(
+            os.path.join(OUT, f"pulser_c4_traj{k}.npz"),
+            doppler=np.array([tr.doppler_detune[q] for q in seq.register.qubit_ids]),
+            amp=float(tr.amp_fluctuations["ch"]), coef_every40=coef[:, ::40], det_every40=det[:, ::40],
+            coef_sha256=hashlib.sha256(coef.tobytes()).hexdigest(), det_sha256=hashlib.sha256(det.tobytes()).hexdigest())
+        print("wrote", f"pulser_c4_traj{k}")
+
+    n, T, field = 5, 120, (0.3, 1.0, 0.5)
+    seq = Sequence(Register.from_coordinates(W.disc_register(n, 30.0, 8.0, 9), center=False, prefix="q"), MockDevice)
+    seq.declare_channel("mw", "mw_global")
+    seq.set_magnetic_field(*field)
+    seq.add(Pulse.ConstantDetuning(BlackmanWaveform(T, 1.5 * np.pi), 0.8, 0), "mw")
+    save("pulser_xy_n5", specs_of(seq)[0][0])
+
+
+if __name__ == "__main__" and "--workloads" in sys.argv:
+    workloads()

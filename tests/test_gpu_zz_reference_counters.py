@@ -56,7 +56,7 @@ def test_schroedinger_reference_counters(lib, name):
         plan.propagate(0.0, spec.sampling_times[-1])
         psi = plan.get_state()[0]
     # EOM detunings of +-1000 rad/us held for microseconds: the stiffest sequence of the suite; north-star bound,
-    # the measured error is printed (pytest -s) and recorded in profiles/r02_gpu_tests.log
+    # the measured error is printed (pytest -s)
     err = float(np.max(np.abs(psi - extra["orc_final"])))
     print(f"{name}: max |psi_gpu - psi_oracle| = {err:.3e}")
     assert err < 1e-8

@@ -150,7 +150,11 @@ def test_fixtures_present():
     assert len(glob.glob(os.path.join(GOLD, "*.npz"))) >= 11
 
 
-@pytest.mark.skipif(not HAVE_PULSER, reason="pulser-core not importable here")
+def _pulser_spec(name):
+    """The spec pulser-core built for a workload (tests/golden/make_golden.py --workloads)."""
+    return HamiltonianSpec.load(os.path.join(GOLD, name + ".npz"))
+
+
 class TestAgainstPulser:
     def _spec(self, seq, rate=1.0):
         from pulser import NoiseModel
@@ -165,35 +169,20 @@ class TestAgainstPulser:
         return spec_from_pulser(ns, traj, hd.basis_data, hd.lindblad_data, rate, T), (ns, traj, hd)
 
     def test_workload_c1_c2_equal_pulser(self):
-        from pulser import Pulse, Register, Sequence
-        from pulser.devices import AnalogDevice, MockDevice
-        from pulser.waveforms import RampWaveform
-
-        seq = Sequence(Register.square(2, spacing=6.0, prefix="q"), MockDevice)
-        seq.declare_channel("ch", "rydberg_global")
-        seq.add(Pulse.ConstantPulse(1000, 2 * np.pi, np.pi, 0), "ch")
-        a, _ = self._spec(seq)
+        a = _pulser_spec("pulser_c1")
         b = W.config_c1()
         np.testing.assert_array_equal(a.drives[0].coef, b.drives[0].coef)
         np.testing.assert_array_equal(a.drives[0].det, b.drives[0].det)
         np.testing.assert_allclose(a.interaction_matrix, b.interaction_matrix, rtol=1e-15)
 
-        n = 9
-        coords = W.disc_register(n, 38.0, 5.0, n)
-        seq = Sequence(Register.from_coordinates(coords, center=False, prefix="q"), AnalogDevice)
-        seq.declare_channel("ch", "rydberg_global")
-        om = 2 * np.pi * 1.5
-        U = om / 2
-        seq.add(Pulse.ConstantDetuning(RampWaveform(500, 0, om), -6 * U, 0), "ch")
-        seq.add(Pulse.ConstantAmplitude(om, RampWaveform(2500, -6 * U, 2 * U), 0), "ch")
-        seq.add(Pulse.ConstantDetuning(RampWaveform(1000, om, 0), 2 * U, 0), "ch")
-        a, _ = self._spec(seq)
-        b = W.config_c2(n=n)
+        a = _pulser_spec("pulser_c2_n9")
+        b = W.config_c2(n=9)
         np.testing.assert_array_equal(a.drives[0].coef, b.drives[0].coef)
         np.testing.assert_array_equal(a.drives[0].det, b.drives[0].det)
         np.testing.assert_allclose(a.interaction_matrix, b.interaction_matrix, rtol=1e-14)
         np.testing.assert_array_equal(a.sampling_times, b.sampling_times)
 
+    @pytest.mark.skipif(not HAVE_PULSER, reason="pulser-core not importable here")
     def test_spec_extraction_equals_direct_restatement(self):
         """OracleHamiltonian.from_pulser walks the nested dict itself
         (hamiltonian.py:426-431); from_spec goes through the product's spec."""
@@ -229,36 +218,12 @@ def test_fast_terms_equal_kron_terms():
         assert abs(A.matrix_at(t) - B.matrix_at(t)).max() < 1e-13
 
 
-@pytest.mark.skipif(not HAVE_PULSER, reason="pulser-core not importable here")
 def test_workloads_c3_c4_equal_pulser():
-    """The numpy restatements of BASELINE configs C3 / C4 equal what pulser-core produces."""
-    import warnings
+    """The numpy restatements of BASELINE configs C3 / C4 equal what pulser-core produces (tests/golden/pulser_*)."""
+    import hashlib
 
-    from pulser import NoiseModel, Pulse, Register, Sequence
-    from pulser._hamiltonian_data import HamiltonianData
-    from pulser.devices import MockDevice
-    from pulser.sampler import sampler
-    from pulser.waveforms import BlackmanWaveform, RampWaveform
-    from pulser_b200.spec import spec_from_pulser
-
-    def first_specs(seq, nm=None, ntraj=None):
-        samples = sampler.sample(seq, extended_duration=seq.get_duration())
-        T = samples.max_duration
-        with warnings.catch_warnings():
-            warnings.simplefilter("ignore")
-            hd = HamiltonianData(samples.extend_duration(T + 1), seq.register, seq.device, nm or NoiseModel(), ntraj)
-        return [(spec_from_pulser(ns, tr, hd.basis_data, hd.lindblad_data, 1.0, T), tr) for tr, ns, _ in hd.noisy_samples]
-
-    n = 5
-    coords = W.disc_register(n, 22.0, 6.0, 100 + n)
-    seq = Sequence(Register.from_coordinates(coords, center=False, prefix="q"), MockDevice)
-    seq.declare_channel("ram", "raman_global")
-    seq.declare_channel("ryd", "rydberg_global")
-    seq.add(Pulse.ConstantDetuning(BlackmanWaveform(500, np.pi / 2), 0, 0), "ram")
-    seq.add(Pulse.ConstantDetuning(BlackmanWaveform(1000, np.pi), 0, 0), "ryd", protocol="wait-for-all")
-    seq.add(Pulse.ConstantDetuning(BlackmanWaveform(500, np.pi / 2), 0, 0), "ram", protocol="wait-for-all")
-    ref = first_specs(seq)[0][0]
-    mine = W.config_c3(n)
+    ref = _pulser_spec("pulser_c3_n5")
+    mine = W.config_c3(5)
     assert ref.eigenbasis == mine.eigenbasis == ["r", "g", "h"] and ref.basis_name == "all"
     for a in mine.drives:
         b = [d for d in ref.drives if d.basis == a.basis][0]
@@ -266,50 +231,26 @@ def test_workloads_c3_c4_equal_pulser():
         np.testing.assert_array_equal(a.det, b.det)
     np.testing.assert_allclose(mine.interaction_matrix, ref.interaction_matrix, rtol=1e-14)
 
-    seq = Sequence(Register.square(4, spacing=6.0, prefix="q"), MockDevice)
-    seq.declare_channel("ch", "rydberg_global")
-    om = 2 * np.pi * 1.5
-    U = om / 2
-    seq.add(Pulse.ConstantDetuning(RampWaveform(500, 0, om), -6 * U, 0), "ch")
-    seq.add(Pulse.ConstantAmplitude(om, RampWaveform(2500, -6 * U, 2 * U), 0), "ch")
-    seq.add(Pulse.ConstantDetuning(RampWaveform(1000, om, 0), 2 * U, 0), "ch")
-    np.random.seed(3)
-    nm = NoiseModel(temperature=50.0, amp_sigma=0.05, laser_waist=175.0)
+    # the first two trajectories pulser draws under np.random.seed(3) for NoiseModel(temperature=50, amp_sigma=0.05,
+    # laser_waist=175) on the 4x4 blockade sweep
     coords = W.square_register(4, 6.0)
     base = W.ising_global_spec(coords, W.C6_LEVEL_70, *W.blockade_sweep_waveforms())
-    for ref, tr in first_specs(seq, nm, 2):
-        dop = np.array([tr.doppler_detune[q] for q in seq.register.qubit_ids])
-        mine = W.noisy_trajectory_spec(base, coords, dop, tr.amp_fluctuations["ch"], 175.0)
-        np.testing.assert_array_equal(mine.drives[0].coef, ref.drives[0].coef)
-        np.testing.assert_array_equal(mine.drives[0].det, ref.drives[0].det)
+    for k in range(2):
+        with np.load(os.path.join(GOLD, f"pulser_c4_traj{k}.npz")) as g:
+            mine = W.noisy_trajectory_spec(base, coords, g["doppler"], float(g["amp"]), 175.0).drives[0]
+            coef = np.ascontiguousarray(mine.coef, dtype=np.complex128)
+            det = np.ascontiguousarray(mine.det, dtype=np.float64)
+            np.testing.assert_array_equal(coef[:, ::40], g["coef_every40"])
+            np.testing.assert_array_equal(det[:, ::40], g["det_every40"])
+            assert hashlib.sha256(coef.tobytes()).hexdigest() == str(g["coef_sha256"])
+            assert hashlib.sha256(det.tobytes()).hexdigest() == str(g["det_sha256"])
     assert abs(W.doppler_sigma(50.0) - 0.600149981254686) < 1e-15
 
 
-@pytest.mark.skipif(not HAVE_PULSER, reason="pulser-core not importable here")
 def test_xy_workload_equals_pulser():
     """workloads.config_xy restates what pulser-core produces for a global microwave pulse under a tilted field."""
-    import warnings
-
-    from pulser import NoiseModel, Pulse, Register, Sequence
-    from pulser._hamiltonian_data import HamiltonianData
-    from pulser.devices import MockDevice
-    from pulser.sampler import sampler
-    from pulser.waveforms import BlackmanWaveform
-    from pulser_b200.spec import spec_from_pulser
-
-    n, T, field = 5, 120, (0.3, 1.0, 0.5)
-    mine = W.config_xy(n=n, seed=9, t_total=T, magnetic_field=field)
-    coords = W.disc_register(n, 30.0, 8.0, 9)
-    seq = Sequence(Register.from_coordinates(coords, center=False, prefix="q"), MockDevice)
-    seq.declare_channel("mw", "mw_global")
-    seq.set_magnetic_field(*field)
-    seq.add(Pulse.ConstantDetuning(BlackmanWaveform(T, 1.5 * np.pi), 0.8, 0), "mw")
-    samples = sampler.sample(seq, extended_duration=seq.get_duration())
-    with warnings.catch_warnings():
-        warnings.simplefilter("ignore")
-        hd = HamiltonianData(samples.extend_duration(T + 1), seq.register, seq.device, NoiseModel(), None)
-    tr, ns, _ = next(iter(hd.noisy_samples))
-    ref = spec_from_pulser(ns, tr, hd.basis_data, hd.lindblad_data, 1.0, T)
+    mine = W.config_xy(n=5, seed=9, t_total=120, magnetic_field=(0.3, 1.0, 0.5))
+    ref = _pulser_spec("pulser_xy_n5")
     assert ref.eigenbasis == mine.eigenbasis and ref.interaction_type == "XY"
     assert np.allclose(ref.interaction_matrix, mine.interaction_matrix, rtol=1e-12, atol=0)
     assert np.allclose(ref.drives[0].coef, mine.drives[0].coef, rtol=1e-12, atol=1e-15)

@@ -4,7 +4,7 @@ For every (PB200_RHO_CAP_MILLI, max_step_samples):
   (i)   error against the DOP853 oracle at N = 10 / 12 on the C2 shape,
   (ii)  self-convergence against a tol = 1e-11 run at N = 20,
   (iii) H-applies per ns and time-steps/s at N = 20.
-Writes one JSON line per case to stdout (collected under profiles/r02_rho_cap_sweep.json).
+Writes one JSON line per case to stdout.
 """
 import json
 import os
