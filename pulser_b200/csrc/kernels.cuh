@@ -96,6 +96,13 @@ __device__ __forceinline__ c2 ld_stream(const c2* p) {
 __device__ __forceinline__ void st_c2(c2* p, c2 v) {
     *reinterpret_cast<double2*>(p) = make_double2(v.x, v.y);
 }
+// 16-byte store whose L2 lines are evicted after the evict-normal / evict-first ones: for a result the next launch
+// gathers from, while the launch streams more than the L2 holds
+__device__ __forceinline__ void st_c2_evict_last(c2* p, c2 v) {
+    uint64_t pol;
+    asm("createpolicy.fractional.L2::evict_last.b64 %0, 1.0;" : "=l"(pol));
+    asm volatile("st.global.L2::cache_hint.v2.f64 [%0], {%1, %2}, %3;" ::"l"(p), "d"(v.x), "d"(v.y), "l"(pol) : "memory");
+}
 
 // Fused Lanczos step (StageArgs::lz set).  The gather source `v` holds the RAW vector r_j = G v_j - beta_{j-1} v_{j-1}
 // of the previous stage; alpha_j = Re<v_j, r_j> and |r_j|^2 were reduced by that stage into lz.acc_prev.  This stage
@@ -777,11 +784,11 @@ struct TaylorArgs {
 
 // epilogue of one amplitude block: everything after the partner sums.  `off[r]` = sum_k c_k [digit_k == from] of the
 // amplitude (0 for uniform drives); idx is the index inside the trajectory, voff the trajectory's offset.
-template <int R>
+// The own-element operands are loaded H amplitudes at a time.
+template <int R, int H = (R >= 4) ? R / 2 : R>
 __device__ __forceinline__ void taylor_epilogue(const TaylorArgs& a, const long long (&idx)[R], const c2 (&v)[R],
                                                 const double (&gx)[R], const double (&gy)[R], const double (&off)[R],
                                                 long long voff, const double* __restrict__ dsrc) {
-    constexpr int H = (R >= 4) ? R / 2 : R;
     const int nb = a.geo.n_bits;
 #pragma unroll
     for (int h0 = 0; h0 < R; h0 += H) {
@@ -822,7 +829,9 @@ __device__ __forceinline__ void taylor_epilogue(const TaylorArgs& a, const long 
 #pragma unroll
         for (int r = 0; r < H; ++r) {
             res[r] = {a.scale.x * sx[r] - a.scale.y * sy[r], a.scale.x * sy[r] + a.scale.y * sx[r]};
-            st_c2(a.out + voff + idx[h0 + r], res[r]);
+            // chi_{k+1} is the next order's gather source: kept in L2 ahead of the ring buffers read once per order
+            // (C2 on H100: the ring is twice the 50 MB L2; 42.9 against 44.1 us per order, DESIGN.md section 8)
+            st_c2_evict_last(a.out + voff + idx[h0 + r], res[r]);
             if (a.g_out) st_c2(a.g_out + voff + idx[h0 + r], c2{gx[h0 + r], gy[h0 + r]});
         }
         if (a.acc_on) {
@@ -841,12 +850,24 @@ __device__ __forceinline__ void taylor_epilogue(const TaylorArgs& a, const long 
 
 // UNIFORM: one drive coefficient for every qubit and a single state (C2, C5); otherwise per-(trajectory, qubit) static
 // factors from `table`, blockIdx.y = trajectory (C4: doppler + amplitude noise batches).
+// The tile is the TBITS low bits of the index (taylor_geometry), the bits above it are coalesced partner loads.  A thread
+// owns R = 2^RB amplitudes (tile index t = tid + r*NT) and works through them in chunks of 8: chunk c is the sub-tile
+// whose top RB - 3 tile bits equal c, where the register-blocked gather of rb_tile_gather applies, and a flip of a chunk
+// bit is one more LDS.128 from the other chunk's sub-tile.  Only one chunk's partner sums are live at a time, which is
+// what lets 16 amplitudes per thread fit in 128 registers; the first chunk's partner loads overlap the tile copy.
 template <bool UNIFORM, bool REAL_G, int TBITS, int RB>
 __global__ void __launch_bounds__(1 << (TBITS - RB), (65536 / ((1 << (TBITS - RB)) * (RB >= 3 ? 128 : 64))))
 stage_d2_taylor_kernel(const __grid_constant__ TaylorArgs a) {
-    constexpr int R = 1 << RB;
+    static_assert(RB >= 3, "chunks of 8 amplitudes per thread");
     constexpr int NT = 1 << (TBITS - RB);
     constexpr int TSIZE = 1 << TBITS;
+    constexpr int RC = 8;                   // amplitudes per chunk
+    constexpr int CB = RB - 3;              // chunk bits: the top CB tile bits
+    constexpr int STB = TBITS - CB;         // bits of a chunk's sub-tile
+    // complex per-bit drive factors from the shared-memory table: the per-qubit factors, or the unit of a uniform
+    // drive of non-zero phase (G = sum_k (unit |to><from|_k + h.c.): one complex factor per partner and two
+    // accumulators per amplitude instead of the P and Q sums)
+    constexpr bool TAB = !(UNIFORM && REAL_G);
     extern __shared__ __align__(128) unsigned char smem_raw[];
     c2* tile = reinterpret_cast<c2*>(smem_raw);
     __shared__ __align__(8) uint64_t mbar;
@@ -854,100 +875,113 @@ stage_d2_taylor_kernel(const __grid_constant__ TaylorArgs a) {
     const int tid = threadIdx.x;
     const long long traj = UNIFORM ? 0 : (long long)blockIdx.y;
     const long long voff = traj * a.D;
-    const long long base = tile_base_of(g, blockIdx.x);
+    const long long base = (long long)blockIdx.x << TBITS;
     const c2* vsrc = a.v + voff;
 
     if (tid == 0) mbar_init(&mbar, 1);
     __syncthreads();
     pdl_wait();
     pdl_launch_dependents();
-    if (tid == 0) mbar_arrive_expect_tx(&mbar, (uint32_t)TSIZE * 16u);
-    {
-        const int rows = 1 << g.hi_bits;
-        const uint32_t row_bytes = (uint32_t)(16u << g.lo_bits);
-        for (int r = tid; r < rows; r += NT)
-            tma_load_1d(tile + ((size_t)r << g.lo_bits), vsrc + base + ((long long)r << g.hi_shift), row_bytes, &mbar);
+    if (tid == 0) {
+        mbar_arrive_expect_tx(&mbar, (uint32_t)TSIZE * 16u);
+        tma_load_1d(tile, vsrc + base, (uint32_t)TSIZE * 16u, &mbar);
     }
     double* tab = reinterpret_cast<double*>(tile + TSIZE);
-    if (!UNIFORM) {   // the per-trajectory table is read behind the tile copy
-        const int stride = d2_table_stride(g.n_bits);
-        const double* src = a.table + traj * stride;
-        for (int i = tid; i < stride; i += NT) tab[i] = src[i];
+    if (TAB) {   // the table is written behind the tile copy
+        if (UNIFORM) {
+            for (int i = tid; i < 2 * g.n_bits; i += NT) tab[i] = (i & 1) ? a.unit.y : a.unit.x;
+        } else {
+            const int stride = d2_table_stride(g.n_bits);
+            const double* src = a.table + traj * stride;
+            for (int i = tid; i < stride; i += NT) tab[i] = src[i];
+        }
         __syncthreads();
     }
-    const long long lomask = (1LL << g.lo_bits) - 1;
     const int to_bit = a.to_bit;
-    c2 v[R];
-    double pr[R], pi[R], qr[R], qi[R];
-    long long idx[R];
-#pragma unroll
-    for (int r = 0; r < R; ++r) {
-        const int t = tid + r * NT;
-        idx[r] = base | (t & lomask) | ((long long)(t >> g.lo_bits) << g.hi_shift);
-        pr[r] = 0.0; pi[r] = 0.0; qr[r] = 0.0; qi[r] = 0.0;
-    }
-    // partners across the bits outside the tile: coalesced loads issued while the bulk copy of the tile is in flight
-    for (unsigned long long m = g.extra_mask; m; m &= m - 1) {
-        const int p = __ffsll((long long)m) - 1;
-        const int bit = (int)((base >> p) & 1);
-        const double sg = (bit == to_bit) ? 1.0 : -1.0;
-        double gx = 0.0, gy = 0.0;
-        if (!UNIFORM) { gx = tab[2 * p]; gy = (bit == to_bit) ? tab[2 * p + 1] : -tab[2 * p + 1]; }
-        double2 raw[R];
-#pragma unroll
-        for (int r = 0; r < R; ++r) raw[r] = __ldg(reinterpret_cast<const double2*>(vsrc + (idx[r] ^ (1LL << p))));
-#pragma unroll
-        for (int r = 0; r < R; ++r) {
-            if (UNIFORM) {
-                pr[r] += raw[r].x; pi[r] += raw[r].y;
-                if (!REAL_G) { qr[r] = fma(sg, raw[r].x, qr[r]); qi[r] = fma(sg, raw[r].y, qi[r]); }
-            } else {
-                pr[r] = fma(gx, raw[r].x, pr[r]); pr[r] = fma(-gy, raw[r].y, pr[r]);
-                pi[r] = fma(gx, raw[r].y, pi[r]); pi[r] = fma(gy, raw[r].x, pi[r]);
-            }
-        }
-    }
-    mbar_wait(&mbar, 0);
-#pragma unroll
-    for (int r = 0; r < R; ++r) v[r] = tile[tid + r * NT];
-    rb_tile_gather<UNIFORM, REAL_G, TBITS, RB>(g, tile, tab, tid, to_bit, 0, false, v, pr, pi, qr, qi);
-    double off[R];
-    if (UNIFORM) {
-        // G = unit S_to + conj(unit) S_from = ux P + i uy Q
-#pragma unroll
-        for (int r = 0; r < R; ++r) {
-            const double dx = a.unit.x * pr[r], dy = a.unit.x * pi[r];
-            if (!REAL_G) { pr[r] = fma(-a.unit.y, qi[r], dx); pi[r] = fma(a.unit.y, qr[r], dy); }
-            else { pr[r] = dx; pi[r] = dy; }
-            off[r] = 0.0;
-        }
-    } else {
-        // static per-qubit detuning weights: sum over (bits of base) + (bits of tid) + (register bits)
-        const int nb = g.n_bits;
-        const long long fixed = base | (tid & lomask) | ((long long)(tid >> g.lo_bits) << g.hi_shift);
-        double common = 0.0;
+    const int nb = g.n_bits;
+    // static per-qubit detuning weights: sum over (bits of base) + (bits of tid) + (register bits)
+    double common = 0.0;
+    if (!UNIFORM) {
         for (int p = 0; p < nb; ++p) {
-            const int bit = (int)((fixed >> p) & 1);
+            const int bit = (int)(((base + tid) >> p) & 1);
             common += (bit == a.from_is_one) ? tab[2 * nb + p] : 0.0;
         }
+    }
+    const double* dsrc = a.dint ? a.dint + traj * a.dint_stride : nullptr;
+#pragma unroll 1
+    for (int c = 0; c < (1 << CB); ++c) {
+        const long long i0 = base + tid + c * RC * NT;   // index of the chunk's first amplitude; the r-th is i0 + r*NT
+        double pr[RC], pi[RC];
 #pragma unroll
-        for (int r = 0; r < R; ++r) {
+        for (int r = 0; r < RC; ++r) { pr[r] = 0.0; pi[r] = 0.0; }
+        // partners across the bits outside the tile: coalesced loads (for the first chunk, while the tile is in flight)
+        for (unsigned long long m = g.extra_mask; m; m &= m - 1) {
+            const int p = __ffsll((long long)m) - 1;
+            const int bit = (int)((base >> p) & 1);
+            double gx = 0.0, gy = 0.0;
+            if (TAB) { gx = tab[2 * p]; gy = (bit == to_bit) ? tab[2 * p + 1] : -tab[2 * p + 1]; }
+            const c2* src = vsrc + (i0 ^ (1LL << p));
+            double2 raw[RC];
+#pragma unroll
+            for (int r = 0; r < RC; ++r) raw[r] = __ldg(reinterpret_cast<const double2*>(src + r * NT));
+#pragma unroll
+            for (int r = 0; r < RC; ++r) {
+                if (!TAB) {
+                    pr[r] += raw[r].x; pi[r] += raw[r].y;
+                } else {
+                    pr[r] = fma(gx, raw[r].x, pr[r]); pr[r] = fma(-gy, raw[r].y, pr[r]);
+                    pi[r] = fma(gx, raw[r].y, pi[r]); pi[r] = fma(gy, raw[r].x, pi[r]);
+                }
+            }
+        }
+        if (c == 0) mbar_wait(&mbar, 0);
+        const c2* sub = tile + (c << STB);
+        c2 v[RC];
+        double qd[RC];   // the Q sums of rb_tile_gather: not used by the two instantiations below
+#pragma unroll
+        for (int r = 0; r < RC; ++r) v[r] = sub[tid + r * NT];
+        rb_tile_gather<!TAB, !TAB, STB, 3>(g, sub, tab, tid, to_bit, 0, false, v, pr, pi, qd, qd);
+#pragma unroll
+        for (int q = 0; q < CB; ++q) {   // flips of the chunk bits
+            const int p = STB + q;
+            const int bit = (c >> q) & 1;
+            double gx = 0.0, gy = 0.0;
+            if (TAB) { gx = tab[2 * p]; gy = (bit == to_bit) ? tab[2 * p + 1] : -tab[2 * p + 1]; }
+            const c2* other = tile + ((c ^ (1 << q)) << STB);
+#pragma unroll
+            for (int r = 0; r < RC; ++r) {
+                const c2 pv = other[tid + r * NT];
+                if (!TAB) {
+                    pr[r] += pv.x; pi[r] += pv.y;
+                } else {
+                    pr[r] = fma(gx, pv.x, pr[r]); pr[r] = fma(-gy, pv.y, pr[r]);
+                    pi[r] = fma(gx, pv.y, pi[r]); pi[r] = fma(gy, pv.x, pi[r]);
+                }
+            }
+        }
+        double off[RC];
+        long long idx[RC];
+#pragma unroll
+        for (int r = 0; r < RC; ++r) {
+            idx[r] = i0 + r * NT;
+            if (!TAB) { pr[r] *= a.unit.x; pi[r] *= a.unit.x; }   // G = ux P for a real unit
             double acc = common;
+            if (!UNIFORM) {
 #pragma unroll
-            for (int q = 0; q < RB; ++q) {
-                const int j = TBITS - RB + q;
-                const int p = (j < g.lo_bits) ? j : (j - g.lo_bits + g.hi_shift);
-                const double th = tab[2 * nb + p];
-                const int bit = (r >> q) & 1;   // `fixed` has these bits at 0
-                acc += ((bit == a.from_is_one) ? th : 0.0) - ((0 == a.from_is_one) ? th : 0.0);
+                for (int q = 0; q < RB; ++q) {
+                    const double th = tab[2 * nb + TBITS - RB + q];
+                    const int bit = ((c * RC + r) >> q) & 1;   // `base + tid` has these bits at 0
+                    acc += ((bit == a.from_is_one) ? th : 0.0) - ((0 == a.from_is_one) ? th : 0.0);
+                }
             }
             off[r] = acc;
         }
+        // per-qubit factors (off != 0) leave the registers for 2 amplitudes' operands at a time, not 4
+        taylor_epilogue<RC, UNIFORM ? RC / 2 : RC / 4>(a, idx, v, pr, pi, off, voff, dsrc);
     }
-    taylor_epilogue<R>(a, idx, v, pr, pi, off, voff, a.dint ? a.dint + traj * a.dint_stride : nullptr);
 }
 
-// any register size (N < 11 in particular): one thread per amplitude, partners through global loads
+// any register size (N < 13 in particular): one thread per amplitude, partners through global loads
 __global__ void __launch_bounds__(256) stage_d2_taylor_small_kernel(const __grid_constant__ TaylorArgs a) {
     const long long s = (long long)blockIdx.x * blockDim.x + threadIdx.x;
     if (s >= a.D) return;

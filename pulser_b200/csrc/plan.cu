@@ -146,6 +146,12 @@ static void pool_free(int dev, void* p) {
     cudaFree(p);
 }
 
+// tile of the Taylor stage kernel: 2^13 amplitudes (128 KiB), one CTA of 512 threads per SM, 16 amplitudes per thread.
+// Measured on C2 (N = 20, H100): 44.1 us per order against 45.1 at 2^12 and 48.9 at 2^11, 42.9 with the evict-last
+// store of chi_{k+1} (DESIGN.md section 8).
+constexpr int kTaylorTileBits = 13;
+constexpr int kTaylorRegBits = 4;
+
 // once per device and process: SM count, > 48 KB of dynamic shared memory for the tile kernels
 static int device_setup(int dev) {
     static std::mutex mu;
@@ -164,9 +170,10 @@ static int device_setup(int dev) {
     CUDA_CHECK(cudaFuncSetAttribute(stage_d2_rb_kernel<false, false, TB, RB>, cudaFuncAttributeMaxDynamicSharedMemorySize, max_smem));
     PB200_RB_ATTR(11, 2) PB200_RB_ATTR(11, 3) PB200_RB_ATTR(12, 2) PB200_RB_ATTR(12, 3)
 #undef PB200_RB_ATTR
-    CUDA_CHECK(cudaFuncSetAttribute(stage_d2_taylor_kernel<true, true, 11, 3>, cudaFuncAttributeMaxDynamicSharedMemorySize, 2048 * 16 + 256));
-    CUDA_CHECK(cudaFuncSetAttribute(stage_d2_taylor_kernel<true, false, 11, 3>, cudaFuncAttributeMaxDynamicSharedMemorySize, 2048 * 16 + 256));
-    CUDA_CHECK(cudaFuncSetAttribute(stage_d2_taylor_kernel<false, false, 11, 3>, cudaFuncAttributeMaxDynamicSharedMemorySize, 2048 * 16 + 2048));
+    const int taylor_smem = (1 << kTaylorTileBits) * 16 + 2048;   // tile + per-bit table
+    CUDA_CHECK(cudaFuncSetAttribute(stage_d2_taylor_kernel<true, true, kTaylorTileBits, kTaylorRegBits>, cudaFuncAttributeMaxDynamicSharedMemorySize, taylor_smem));
+    CUDA_CHECK(cudaFuncSetAttribute(stage_d2_taylor_kernel<true, false, kTaylorTileBits, kTaylorRegBits>, cudaFuncAttributeMaxDynamicSharedMemorySize, taylor_smem));
+    CUDA_CHECK(cudaFuncSetAttribute(stage_d2_taylor_kernel<false, false, kTaylorTileBits, kTaylorRegBits>, cudaFuncAttributeMaxDynamicSharedMemorySize, taylor_smem));
     CUDA_CHECK(cudaFuncSetAttribute(stage_d2_fwd_kernel<true, 11, 3>, cudaFuncAttributeMaxDynamicSharedMemorySize, 2 * 2048 * 16 + 256));
     CUDA_CHECK(cudaFuncSetAttribute(stage_d2_fwd_kernel<false, 11, 3>, cudaFuncAttributeMaxDynamicSharedMemorySize, 2 * 2048 * 16 + 256));
     if (dev >= 0 && dev < PB200_MAX_DEVICES) sm_count[dev] = sms;
@@ -1402,7 +1409,7 @@ static void propagate_mcwf(Plan& P, double t_start, double t_stop, const pb200_r
 static thread_local const char* g_taylor_why = "";   // why the Taylor propagator was not taken (PB200_TAYLOR_LOG)
 static bool taylor_prepare(Plan& P);
 static bool taylor_worthwhile(Plan& P, double gtol);
-static bool taylor_geometry(const Plan& P, const std::vector<PassGeom>& passes, bool& use_rb);
+static bool taylor_geometry(const Plan& P, std::vector<PassGeom>& passes, bool& use_rb);
 static void propagate_taylor(Plan& P, double t_start, double t_stop, const pb200_run_opts* o, pb200_run_stats* stats);
 
 static void propagate(Plan& P, double t_start, double t_stop, const pb200_run_opts* o, pb200_run_stats* stats) {
@@ -1430,7 +1437,8 @@ static void propagate(Plan& P, double t_start, double t_stop, const pb200_run_op
         }
         if (want) {
             bool use_rb = false;
-            const bool ok = taylor_prepare(P) && taylor_geometry(P, plan_passes(P.n, P.tile_bits, P.max_extra), use_rb) &&
+            std::vector<PassGeom> passes;
+            const bool ok = taylor_prepare(P) && taylor_geometry(P, passes, use_rb) &&
                             (req == 3 || taylor_worthwhile(P, (o && o->tol > 0.0) ? o->tol : 1e-8));
             if (ok) { propagate_taylor(P, t_start, t_stop, o, stats); return; }
             if (env_int("PB200_TAYLOR_LOG", 0)) fprintf(stderr, "taylor not taken: %s\n", g_taylor_why);
@@ -2072,12 +2080,14 @@ static int taylor_order(double h, const std::vector<double>& mj, double tol, dou
 static void launch_taylor_stage(Plan& P, const PassGeom* geo, const TaylorArgs& a, long long& launches) {
     const bool uniform = a.table == nullptr;
     if (geo) {
-        dim3 grid((unsigned)(P.D >> 11), (unsigned)(uniform ? 1 : P.B)), block(256);
-        const size_t smem = (size_t)2048 * 16 + (uniform ? 0 : (size_t)d2_table_stride(P.n) * 8);
+        constexpr int TB = kTaylorTileBits, RB = kTaylorRegBits;
         const bool real_g = a.unit.y == 0.0;
-        if (!uniform) launch_k(stage_d2_taylor_kernel<false, false, 11, 3>, grid, block, smem, P.stream, P.use_pdl, a);
-        else if (real_g) launch_k(stage_d2_taylor_kernel<true, true, 11, 3>, grid, block, smem, P.stream, P.use_pdl, a);
-        else launch_k(stage_d2_taylor_kernel<true, false, 11, 3>, grid, block, smem, P.stream, P.use_pdl, a);
+        dim3 grid((unsigned)(P.D >> TB), (unsigned)(uniform ? 1 : P.B)), block(1 << (TB - RB));
+        // the kernel keeps a per-bit table behind the tile unless the drive is uniform and real
+        const size_t smem = ((size_t)16 << TB) + (uniform && real_g ? 0 : (size_t)d2_table_stride(P.n) * 8);
+        if (!uniform) launch_k(stage_d2_taylor_kernel<false, false, TB, RB>, grid, block, smem, P.stream, P.use_pdl, a);
+        else if (real_g) launch_k(stage_d2_taylor_kernel<true, true, TB, RB>, grid, block, smem, P.stream, P.use_pdl, a);
+        else launch_k(stage_d2_taylor_kernel<true, false, TB, RB>, grid, block, smem, P.stream, P.use_pdl, a);
     } else {
         dim3 grid((unsigned)((P.D + 255) / 256), (unsigned)P.B);
         stage_d2_taylor_small_kernel<<<grid, 256, 0, P.stream>>>(a);
@@ -2085,10 +2095,11 @@ static void launch_taylor_stage(Plan& P, const PassGeom* geo, const TaylorArgs& 
     ++launches;
 }
 
-// geometry of the Taylor stage: the register-blocked single-pass kernel, or the plain kernel for small registers
-static bool taylor_geometry(const Plan& P, const std::vector<PassGeom>& passes, bool& use_rb) {
-    use_rb = passes.size() == 1 && passes[0].first_pass && passes[0].hi_bits == 0 && passes[0].lo_bits == 11 &&
-             P.tile_bits == 11 && P.reg_bits == 3;
+// geometry of the Taylor stage: the register-blocked single-pass kernel on its own 2^kTaylorTileBits tile (whatever
+// tile the Magnus stages use), or the plain kernel for small registers
+static bool taylor_geometry(const Plan& P, std::vector<PassGeom>& passes, bool& use_rb) {
+    passes = plan_passes(P.n, kTaylorTileBits, P.max_extra);
+    use_rb = passes.size() == 1 && passes[0].first_pass && passes[0].hi_bits == 0 && passes[0].lo_bits == kTaylorTileBits;
     return use_rb || P.n <= 16;
 }
 
@@ -2102,7 +2113,7 @@ static void propagate_taylor(Plan& P, double t_start, double t_stop, const pb200
     const int order = P.desc.interp_order;
     const int N = P.n;
     const int nt = (int)P.times.size();
-    const std::vector<PassGeom> passes = plan_passes(P.n, P.tile_bits, P.max_extra);
+    std::vector<PassGeom> passes;
     bool use_rb = false;
     if (!taylor_geometry(P, passes, use_rb)) fail(PB200_ERR_UNSUPPORTED, "Taylor propagator: unsupported register size");
     const PiecewiseCubic<double>& om_pc = P.tay.om;
