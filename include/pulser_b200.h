@@ -270,6 +270,41 @@ int pb200_coefficients_at(pb200_plan* plan, int32_t traj, int32_t drive,
 int pb200_bench_apply(pb200_plan* plan, double t_us, int32_t reps,
                       double* ms_out, int64_t* launches_out);
 
+/* ---- state-vector shards (registers larger than one GPU) -------------------- */
+/* Shard `shard_index` of G = 2^shard_bits (shard_bits = 1, 2, 3) of ONE state
+ * of desc->n_qudits = N qubits: the plan holds the global indices
+ * [i 2^L, (i+1) 2^L), L = N - shard_bits (13 <= L <= 29), i.e. the top
+ * shard_bits qubits (qudits 0 .. shard_bits-1) select the shard.  d = 2, one
+ * drive, n_traj = 1.  Uploads (interaction, drive) are those of a whole plan;
+ * each shard computes its slice of the interaction diagonal.  A shard answers
+ * pb200_state_set (basis_index: the global index; psi: its slice), _get,
+ * _probabilities, _norm2, _overlap (phi: its slice) and _sample (out: the low L
+ * bits of the bitstring) on its slice, and _occupation / _correlation with its
+ * contributions (global digits); pb200_propagate / _apply_h / _state_energy
+ * fail with PB200_ERR_STATE: use the group calls below.  Argument checks
+ * happen before any device call. */
+int pb200_plan_create_shard(pb200_plan** out, const pb200_plan_desc* desc,
+                            int32_t shard_bits, int32_t shard_index);
+/* Link the G shards plans[i] = shard i (after their uploads): checks N, sampling
+ * times and the Taylor structure (global drive of constant phase), merges the
+ * interaction bounds so that every shard schedules exactly like the unsharded
+ * plan, enables peer access between distinct devices (PB200_ERR_UNSUPPORTED
+ * where it is impossible). */
+int pb200_shards_link(pb200_plan** plans, int32_t count);
+/* pb200_propagate of the whole state with the Taylor propagator (integrator 0
+ * or 3; options steering the Magnus controller are refused): the schedule is
+ * computed once, each order of the series runs on every shard, reading the
+ * peers' slices across the shard bits. */
+int pb200_shards_propagate(pb200_plan** plans, int32_t count, double t_start,
+                           double t_stop, const pb200_run_opts* opts,
+                           pb200_run_stats* stats);
+/* out = H(t) in, host buffers of the FULL 2^N complex amplitudes. */
+int pb200_shards_apply_h(pb200_plan** plans, int32_t count, double t_us,
+                         const double* in, double* out);
+/* <psi|H(t)|psi> and <psi|H(t)^2|psi> of the sharded state (energy[1], h2[1]). */
+int pb200_shards_energy(pb200_plan** plans, int32_t count, double t_us,
+                        double* energy, double* h2);
+
 /* ---- host-side math, usable without a device (exercised by the CPU tests) -- */
 /* Interpolant of complex samples y[n] (re,im) over x[n] at nq query points:
  * out[nq][2].  The QobjEvo array-coefficient rule (order 0 / 1 / 3). */

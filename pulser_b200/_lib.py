@@ -118,6 +118,12 @@ def _load() -> C.CDLL:
             C.c_int, [vp, C.c_int32, C.c_int32, C.c_int32, C.c_double, dp]),
         "pb200_bench_apply": (
             C.c_int, [vp, C.c_double, C.c_int32, dp, C.POINTER(C.c_int64)]),
+        "pb200_plan_create_shard": (C.c_int, [C.POINTER(vp), C.POINTER(PlanDesc), C.c_int32, C.c_int32]),
+        "pb200_shards_link": (C.c_int, [C.POINTER(vp), C.c_int32]),
+        "pb200_shards_propagate": (
+            C.c_int, [C.POINTER(vp), C.c_int32, C.c_double, C.c_double, C.POINTER(RunOpts), C.POINTER(RunStats)]),
+        "pb200_shards_apply_h": (C.c_int, [C.POINTER(vp), C.c_int32, C.c_double, dp, dp]),
+        "pb200_shards_energy": (C.c_int, [C.POINTER(vp), C.c_int32, C.c_double, dp, dp]),
         "pb200_host_interpolate": (
             C.c_int, [dp, dp, C.c_int32, C.c_int32, dp, C.c_int32, dp]),
         "pb200_host_moments": (
@@ -147,6 +153,7 @@ EXPORTED_SYMBOLS = [
     "pb200_state_occupation", "pb200_state_correlation", "pb200_state_energy", "pb200_state_overlap", "pb200_state_sample", "pb200_state_copy", "pb200_state_device_ptr", "pb200_propagate", "pb200_apply_h",
     "pb200_coefficients_at", "pb200_bench_apply", "pb200_host_interpolate",
     "pb200_host_moments", "pb200_host_chebyshev", "pb200_host_taylor_fit", "pb200_host_taylor_order", "pb200_host_taylor_separable",
+    "pb200_plan_create_shard", "pb200_shards_link", "pb200_shards_propagate", "pb200_shards_apply_h", "pb200_shards_energy",
 ]
 
 lib = _load()

@@ -504,7 +504,12 @@ class DeviceHamiltonian(B200Operator):
 
 
 class B200Config(EmulationConfig[B200State]):
-    """``QutipConfig`` mirror (``qutip_config.py:28-192``): same options."""
+    """``QutipConfig`` mirror (``qutip_config.py:28-192``): same options, plus
+
+    ``devices``: CUDA ordinals of the shards of the state vector (2, 4 or 8 entries; the same ordinal may repeat).
+    A noiseless single-state run is then split over ``len(devices)`` plans (``pulser_b200.sharded.ShardedPlan``), so
+    registers larger than one GPU's memory can run.  Default ``None``: one plan on one device.
+    """
 
     _enforce_expected_kwargs = True
     sampling_rate: float
@@ -528,6 +533,11 @@ class B200Config(EmulationConfig[B200State]):
                 "If provided, `initial_state` must be an instance of "
                 f"`B200State`, not {type(initial_state)}."
             )
+        devices = backend_options.setdefault("devices")
+        if devices is not None:
+            from .sharded import validate_devices
+
+            backend_options["devices"] = validate_devices(devices)
         noise_model = backend_options.get("noise_model")
         if noise_model is not None and noise_model.samples_per_run not in [None, 1]:
             warnings.warn(  # qutip_config.py:114-123: the V2 protocol samples through its observables
@@ -544,7 +554,7 @@ class B200Config(EmulationConfig[B200State]):
                          progress_bar=progress_bar, **backend_options)
 
     def _expected_kwargs(self) -> set[str]:
-        return super()._expected_kwargs() | {"sampling_rate", "solver", "print_progress", "progress_bar"}
+        return super()._expected_kwargs() | {"sampling_rate", "solver", "print_progress", "progress_bar", "devices"}
 
     def _get_legacy_evaluation_times(self, total_duration_ns: int):
         """qutip_config.py:169-192: relative observable times -> microseconds."""
@@ -737,10 +747,42 @@ class B200Backend(EmulatorBackend):
                 out.extend(results)
         return out
 
+    def _run_sharded(self, devices: list[int]) -> Results:
+        """Noiseless sequence on a state vector split over ``devices`` (``B200Config(devices=...)``), streamed through
+        the evaluation times like the single-plan run."""
+        from . import engine, sharded
+        from ._lib import PB200Error
+
+        sim = self._sim_obj
+        if sim.noise_model.noise_types:
+            raise NotImplementedError(
+                "a state vector split over `devices` runs noiseless sequences only; this one has the noise types "
+                f"{sorted(sim.noise_model.noise_types)}"
+            )
+        sim._validate_options({})
+        sim._check_supported()
+        n_dev = engine.device_count()
+        missing = sorted({d for d in devices if d >= n_dev})
+        if missing:
+            raise ValueError(f"`devices` names CUDA device(s) {missing}, but {n_dev} are visible")
+        res = Results(atom_order=tuple(sim._register.qubit_ids), total_duration=sim.total_duration_ns)
+        try:
+            plan = sharded.ShardedPlan(sim._noiseless_spec(), devices, sim._interp_order)
+        except PB200Error as e:
+            if e.code == -3:  # PB200_ERR_UNSUPPORTED: outside what the sharded Taylor propagator covers
+                raise NotImplementedError(str(e)) from e
+            raise
+        with plan:
+            self._stream(plan, res)
+        return res
+
     def run(self) -> Results:
         from . import engine
 
         sim = self._sim_obj
+        devices = getattr(self._config, "_backend_options", {}).get("devices")
+        if devices is not None:
+            return self._run_sharded(devices)
         opts = {"print_progress": self._config.print_progress, "progress_bar": self._config.progress_bar}
         atom_order = tuple(sim._register.qubit_ids)
         with engine.DevicePlan(sim._noiseless_spec(sim.noise_model.with_leakage), sim._interp_order, sim._gpu) as hplan:

@@ -755,6 +755,7 @@ __global__ void __launch_bounds__(1 << (TBITS - RB), 2) stage_d2_fwd_kernel(cons
 // order.  Replaces qutip.sesolve (simulation.py:729-735) for global drives of constant phase, and -- with per-qubit
 // static factors from a per-trajectory table (TaylorArgs::table) -- the trajectory loop's solves (simulation.py:885-915).
 #define PB200_TAYLOR_PMAX 8
+#define PB200_MAX_SHARD_BITS 3
 struct TaylorArgs {
     const c2* v;       // chi_k, gather source [B][D]
     c2* out;           // chi_{k+1}
@@ -780,16 +781,23 @@ struct TaylorArgs {
     int acc_add_v;     // 1: chi_k joins the update (even orders), 0: chi_{k+1} alone
     int acc_on;        // 0: this order leaves the accumulator alone
     c2 acc_mul;        // factor of the whole accumulator (phase of the scalar centre on the last order, else 1)
+    // state-vector shards (stage_d2_taylor_kernel<..., SHARD = true>): the top shard_bits qubits of the global index
+    // select the shard, every other operand is this shard's slice of 2^(N - shard_bits) amplitudes.  peer[q] = chi_k
+    // of shard (shard ^ 1 << q): a flip of shard bit q leaves the local index unchanged
+    const c2* peer[PB200_MAX_SHARD_BITS];
+    int shard_bits, shard;
 };
 
 // epilogue of one amplitude block: everything after the partner sums.  `off[r]` = sum_k c_k [digit_k == from] of the
 // amplitude (0 for uniform drives); idx is the index inside the trajectory, voff the trajectory's offset.
-// The own-element operands are loaded H amplitudes at a time.
-template <int R, int H = (R >= 4) ? R / 2 : R>
+// The own-element operands are loaded H amplitudes at a time.  SHARD: idx is local, the excitation count is that of the
+// global index (the shard index holds its top bits).
+template <int R, int H = (R >= 4) ? R / 2 : R, bool SHARD = false>
 __device__ __forceinline__ void taylor_epilogue(const TaylorArgs& a, const long long (&idx)[R], const c2 (&v)[R],
                                                 const double (&gx)[R], const double (&gy)[R], const double (&off)[R],
                                                 long long voff, const double* __restrict__ dsrc) {
     const int nb = a.geo.n_bits;
+    const int ones_hi = SHARD ? __popc(a.shard) : 0;
 #pragma unroll
     for (int h0 = 0; h0 < R; h0 += H) {
         double sx[H], sy[H], cn[H];
@@ -799,7 +807,7 @@ __device__ __forceinline__ void taylor_epilogue(const TaylorArgs& a, const long 
             for (int r = 0; r < H; ++r) dv[r] = dsrc ? __ldcs(dsrc + idx[h0 + r]) : 0.0;
 #pragma unroll
             for (int r = 0; r < H; ++r) {
-                const int ones = __popcll((unsigned long long)idx[h0 + r]);
+                const int ones = __popcll((unsigned long long)idx[h0 + r]) + ones_hi;
                 cn[r] = (double)(a.from_is_one ? ones : (nb - ones));
                 const double diag = fma(-a.th0, cn[r], fma(-a.m0, off[h0 + r], dv[r] - a.gam0));
                 sx[r] = fma(diag, v[h0 + r].x, a.om0 * gx[h0 + r]);
@@ -855,10 +863,13 @@ __device__ __forceinline__ void taylor_epilogue(const TaylorArgs& a, const long 
 // whose top RB - 3 tile bits equal c, where the register-blocked gather of rb_tile_gather applies, and a flip of a chunk
 // bit is one more LDS.128 from the other chunk's sub-tile.  Only one chunk's partner sums are live at a time, which is
 // what lets 16 amplitudes per thread fit in 128 registers; the first chunk's partner loads overlap the tile copy.
-template <bool UNIFORM, bool REAL_G, int TBITS, int RB>
+// SHARD (uniform drives): the launch works on one shard of the state (TaylorArgs::peer); a flip of shard bit q is one
+// more coalesced load from the peer's chi_k at the same local index, issued with the other out-of-tile partners.
+template <bool UNIFORM, bool REAL_G, int TBITS, int RB, bool SHARD = false>
 __global__ void __launch_bounds__(1 << (TBITS - RB), (65536 / ((1 << (TBITS - RB)) * (RB >= 3 ? 128 : 64))))
 stage_d2_taylor_kernel(const __grid_constant__ TaylorArgs a) {
     static_assert(RB >= 3, "chunks of 8 amplitudes per thread");
+    static_assert(UNIFORM || !SHARD, "shards carry one state with a uniform drive");
     constexpr int NT = 1 << (TBITS - RB);
     constexpr int TSIZE = 1 << TBITS;
     constexpr int RC = 8;                   // amplitudes per chunk
@@ -934,6 +945,31 @@ stage_d2_taylor_kernel(const __grid_constant__ TaylorArgs a) {
                 }
             }
         }
+        if (SHARD) {
+            // partners across the shard bits (global bits N - shard_bits + q): same local index in the peer's slice,
+            // the sign of the drive term from the global bit value, i.e. the shard index
+            for (int q = 0; q < a.shard_bits; ++q) {
+                const int bit = (a.shard >> q) & 1;
+                double gx = 0.0, gy = 0.0;
+                if (TAB) {
+                    const int p = nb - a.shard_bits + q;
+                    gx = tab[2 * p]; gy = (bit == to_bit) ? tab[2 * p + 1] : -tab[2 * p + 1];
+                }
+                const c2* src = a.peer[q] + i0;
+                double2 raw[RC];
+#pragma unroll
+                for (int r = 0; r < RC; ++r) raw[r] = *reinterpret_cast<const double2*>(src + r * NT);
+#pragma unroll
+                for (int r = 0; r < RC; ++r) {
+                    if (!TAB) {
+                        pr[r] += raw[r].x; pi[r] += raw[r].y;
+                    } else {
+                        pr[r] = fma(gx, raw[r].x, pr[r]); pr[r] = fma(-gy, raw[r].y, pr[r]);
+                        pi[r] = fma(gx, raw[r].y, pi[r]); pi[r] = fma(gy, raw[r].x, pi[r]);
+                    }
+                }
+            }
+        }
         if (c == 0) mbar_wait(&mbar, 0);
         const c2* sub = tile + (c << STB);
         c2 v[RC];
@@ -977,7 +1013,7 @@ stage_d2_taylor_kernel(const __grid_constant__ TaylorArgs a) {
             off[r] = acc;
         }
         // per-qubit factors (off != 0) leave the registers for 2 amplitudes' operands at a time, not 4
-        taylor_epilogue<RC, UNIFORM ? RC / 2 : RC / 4>(a, idx, v, pr, pi, off, voff, dsrc);
+        taylor_epilogue<RC, UNIFORM ? RC / 2 : RC / 4, SHARD>(a, idx, v, pr, pi, off, voff, dsrc);
     }
 }
 
@@ -1347,7 +1383,9 @@ __global__ void __launch_bounds__(256, 2) stage_multilevel_rb_kernel(GenArgs a) 
 // ---- interaction diagonal ---------------------------------------------------
 // Dint[s] = sum_{i<j} U_ij [digit_i == r][digit_j == r]
 // (make_vdw_term, hamiltonian.py:260-274, after the + dag doubling of 0.5*U)
-__global__ void dint_kernel(double* dint, const double* U, int n, int dim, int rstate, long long D) {
+// Here and in the reductions below, `off` is the global index of element 0 (the first amplitude of a state-vector
+// shard, 0 for a whole state): the digits are those of off + idx.
+__global__ void dint_kernel(double* dint, const double* U, int n, int dim, int rstate, long long D, long long off) {
     extern __shared__ double Us[];
     for (int i = threadIdx.x; i < n * n; i += blockDim.x) Us[i] = U[i];
     __syncthreads();
@@ -1355,7 +1393,7 @@ __global__ void dint_kernel(double* dint, const double* U, int n, int dim, int r
          idx += (long long)gridDim.x * blockDim.x) {
         int pos[64];
         int cnt = 0;
-        long long rem = idx;
+        long long rem = off + idx;
         for (int k = n - 1; k >= 0; --k) {
             if ((int)(rem % dim) == rstate) pos[cnt++] = k;
             rem /= dim;
@@ -1370,12 +1408,12 @@ __global__ void dint_kernel(double* dint, const double* U, int n, int dim, int r
 
 // min / max of Dint grouped by the number of |r> digits (spectral bounds)
 __global__ void dint_bounds_kernel(const double* dint, int n, int dim, int rstate, long long D, double* mins,
-                                   double* maxs) {
+                                   double* maxs, long long off) {
     // one thread per amplitude, atomics on (n+1) bins via ordered-int trick
     for (long long idx = blockIdx.x * (long long)blockDim.x + threadIdx.x; idx < D;
          idx += (long long)gridDim.x * blockDim.x) {
         int cnt = 0;
-        long long rem = idx;
+        long long rem = off + idx;
         for (int k = 0; k < n; ++k) { cnt += ((int)(rem % dim) == rstate); rem /= dim; }
         const double v = dint[idx];
         // Dint >= 0 is not guaranteed (negative C6 never occurs, but be safe): use CAS loops
@@ -1399,24 +1437,25 @@ __global__ void dint_bounds_kernel(const double* dint, int n, int dim, int rstat
 // ---- measurement: bitstring weights, occupations, sampling ---------------------------------------------------
 // weights[b(s)] += |psi_s|^2 with bit k of b = [digit_k(s) == one_digit], qudit 0 = most significant bit
 // (QutipResult._weights, qutip_result.py:101-158: reversal for ground-rydberg and the 3/4-level
-// marginalisation are both this rule)
-__global__ void bitstring_weights_kernel(const c2* psi, double* weights, long long D, int n, int dim, int one_digit) {
+// marginalisation are both this rule).  A shard (d = 2) covers an aligned block of 2^L = D bitstrings: weights[b mod D].
+__global__ void bitstring_weights_kernel(const c2* psi, double* weights, long long D, int n, int dim, int one_digit,
+                                         long long off) {
     for (long long s = blockIdx.x * (long long)blockDim.x + threadIdx.x; s < D;
          s += (long long)gridDim.x * blockDim.x) {
         const c2 v = psi[s];
         const double p = v.x * v.x + v.y * v.y;
-        long long rem = s, b = 0;
+        long long rem = off + s, b = 0;
         for (int k = n - 1; k >= 0; --k) {  // qudit k <-> bit n-1-k
             if ((int)(rem % dim) == one_digit) b |= 1LL << (n - 1 - k);
             rem /= dim;
         }
-        if (dim == 2) weights[b] = p;  // a permutation: no atomics needed
+        if (dim == 2) weights[b & (D - 1)] = p;  // a permutation: no atomics needed
         else atomicAdd(weights + b, p);
     }
 }
 
 // occ[k] += sum_s |psi_s|^2 [digit_k(s) == digit]   (Occupation observable / <n_k>)
-__global__ void occupation_kernel(const c2* psi, double* occ, long long D, int n, int dim, int digit) {
+__global__ void occupation_kernel(const c2* psi, double* occ, long long D, int n, int dim, int digit, long long off) {
     extern __shared__ double socc[];
     for (int i = threadIdx.x; i < n; i += blockDim.x) socc[i] = 0.0;
     __syncthreads();
@@ -1426,7 +1465,7 @@ __global__ void occupation_kernel(const c2* psi, double* occ, long long D, int n
         const c2 v = psi[traj * D + s];
         const double p = v.x * v.x + v.y * v.y;
         if (p == 0.0) continue;
-        long long rem = s;
+        long long rem = off + s;
         for (int k = n - 1; k >= 0; --k) {
             if ((int)(rem % dim) == digit) atomicAdd(&socc[k], p);
             rem /= dim;
@@ -1439,7 +1478,8 @@ __global__ void occupation_kernel(const c2* psi, double* occ, long long D, int n
 // corr[traj][i*n+j] (i <= j) += sum_s |psi_s|^2 [digit_i(s) == digit][digit_j(s) == digit]
 // (CorrelationMatrix observable <n_i n_j>; the diagonal is the occupation).  A block stages 2048 probabilities and
 // their per-qudit match masks in shared memory; each warp then reduces a subset of the n(n+1)/2 pairs over them.
-__global__ void __launch_bounds__(256) correlation_kernel(const c2* psi, double* corr, long long D, int n, int dim, int digit) {
+__global__ void __launch_bounds__(256) correlation_kernel(const c2* psi, double* corr, long long D, int n, int dim, int digit,
+                                                          long long off) {
     constexpr int CH = 2048;
     __shared__ double sp[CH];
     __shared__ unsigned long long sm[CH];
@@ -1454,7 +1494,7 @@ __global__ void __launch_bounds__(256) correlation_kernel(const c2* psi, double*
             if (s < D) {
                 const c2 v = psi[traj * D + s];
                 p = v.x * v.x + v.y * v.y;
-                long long rem = s;
+                long long rem = off + s;
                 for (int k = n - 1; k >= 0; --k) {
                     if ((int)(rem % dim) == digit) m |= 1ull << k;
                     rem /= dim;

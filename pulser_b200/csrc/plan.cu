@@ -151,6 +151,9 @@ static void pool_free(int dev, void* p) {
 // store of chi_{k+1} (DESIGN.md section 8).
 constexpr int kTaylorTileBits = 13;
 constexpr int kTaylorRegBits = 4;
+// a state-vector shard holds 2^L amplitudes, 13 <= L <= 29: at least one tile, and the local bits above the tile
+// (at most 16) stay partner loads of the single-pass geometry
+constexpr int kShardMaxLocalBits = 29;
 
 // once per device and process: SM count, > 48 KB of dynamic shared memory for the tile kernels
 static int device_setup(int dev) {
@@ -174,6 +177,8 @@ static int device_setup(int dev) {
     CUDA_CHECK(cudaFuncSetAttribute(stage_d2_taylor_kernel<true, true, kTaylorTileBits, kTaylorRegBits>, cudaFuncAttributeMaxDynamicSharedMemorySize, taylor_smem));
     CUDA_CHECK(cudaFuncSetAttribute(stage_d2_taylor_kernel<true, false, kTaylorTileBits, kTaylorRegBits>, cudaFuncAttributeMaxDynamicSharedMemorySize, taylor_smem));
     CUDA_CHECK(cudaFuncSetAttribute(stage_d2_taylor_kernel<false, false, kTaylorTileBits, kTaylorRegBits>, cudaFuncAttributeMaxDynamicSharedMemorySize, taylor_smem));
+    CUDA_CHECK(cudaFuncSetAttribute(stage_d2_taylor_kernel<true, true, kTaylorTileBits, kTaylorRegBits, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, taylor_smem));
+    CUDA_CHECK(cudaFuncSetAttribute(stage_d2_taylor_kernel<true, false, kTaylorTileBits, kTaylorRegBits, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, taylor_smem));
     CUDA_CHECK(cudaFuncSetAttribute(stage_d2_fwd_kernel<true, 11, 3>, cudaFuncAttributeMaxDynamicSharedMemorySize, 2 * 2048 * 16 + 256));
     CUDA_CHECK(cudaFuncSetAttribute(stage_d2_fwd_kernel<false, 11, 3>, cudaFuncAttributeMaxDynamicSharedMemorySize, 2 * 2048 * 16 + 256));
     if (dev >= 0 && dev < PB200_MAX_DEVICES) sm_count[dev] = sms;
@@ -275,6 +280,11 @@ struct Plan {
     bool use_taylor = true;         // PB200_TAYLOR=0: never chosen automatically
     bool use_lanczos_fuse = true;   // PB200_LANCZOS_FUSE=0: separate vector-update kernel (cross-check)
     int use_tiled = 1;              // PB200_TILED: d = 3 / 4 registers: 1 register-blocked tiled kernel, 0 generic
+    // state-vector shard (pb200_plan_create_shard): the top shard_bits qubits of the global index equal `shard`; n is
+    // the global N, D = 2^(N - shard_bits) the slice this plan holds.  `group` = every shard, by index, once linked
+    int shard_bits = 0, shard = 0;
+    std::vector<Plan*> group;
+    long long shard_offset() const { return (long long)shard << (n - shard_bits); }
     bool all_uniform() const {
         for (int q = 0; q < n_drives; ++q)
             if (!desc.drives[q].uniform) return false;
@@ -1358,7 +1368,7 @@ static void propagate_mcwf(Plan& P, double t_start, double t_stop, const pb200_r
                 CUDA_CHECK(cudaMemsetAsync(d_occ, 0, sizeof(double) * P.n, P.stream));
                 const long long nb = std::min<long long>((P.D + 255) / 256, (long long)P.sm_count * 4);
                 occupation_kernel<<<(unsigned)std::max<long long>(nb, 1), 256, sizeof(double) * P.n, P.stream>>>(
-                    psi, d_occ, P.D, P.n, P.dim, dgt);
+                    psi, d_occ, P.D, P.n, P.dim, dgt, 0LL);
                 CUDA_CHECK(cudaMemcpyAsync(occ.data() + (size_t)dgt * P.n, d_occ, sizeof(double) * P.n, cudaMemcpyDeviceToHost, P.stream));
             }
             CUDA_CHECK(cudaStreamSynchronize(P.stream));
@@ -2103,54 +2113,67 @@ static bool taylor_geometry(const Plan& P, std::vector<PassGeom>& passes, bool& 
     return use_rb || P.n <= 16;
 }
 
-static void propagate_taylor(Plan& P, double t_start, double t_stop, const pb200_run_opts* o, pb200_run_stats* stats) {
-    const double tlo = P.times.front(), thi = P.times.back();
-    const double eps = 1e-12;
-    const double gtol = (o && o->tol > 0.0) ? o->tol : 1e-8;
-    const double rate = gtol / std::max(thi - tlo, 1e-30);       // error budget per unit of time
-    const double rho_max = env_int("PB200_TAYLOR_RHO_MILLI", 14000) * 1e-3;
-    const int pmax = std::min(PB200_TAYLOR_PMAX, std::max(1, env_int("PB200_TAYLOR_P", PB200_TAYLOR_PMAX)));
-    const int order = P.desc.interp_order;
-    const int N = P.n;
-    const int nt = (int)P.times.size();
-    std::vector<PassGeom> passes;
-    bool use_rb = false;
-    if (!taylor_geometry(P, passes, use_rb)) fail(PB200_ERR_UNSUPPORTED, "Taylor propagator: unsupported register size");
-    const PiecewiseCubic<double>& om_pc = P.tay.om;
-    const PiecewiseCubic<double>& th_pc = P.tabs[0][0].det[0];
-    Plan::TaylorCache& C = P.tay;
-    taylor_knot_widths(P);
-    // Step length: rho = h W <= rho_max, lowered where the fp64 cancellation of the series would eat the tolerance.  The
-    // rounding error of a step grows like e^rho: ~0.05 eps e^rho measured (tools/taylor_rho_sweep.py: 6e-12 per
-    // step at rho = 14, 1.4e-10 at 18), random from step to step, n ~ (int W dt) / rho steps over the whole sequence;
-    // it may use a fifth of the tolerance.  At the default 1e-8 this never binds (17 > 14 for C2, C4, C5).
-    const double kRoundUnit = 0.05 * 1.1102230246251565e-16;
-    double rho_target = rho_max;
-    {
-        double w_total = 0.0;
-        for (int i = 0; i + 1 < nt; ++i) w_total += 0.5 * (C.w_knot[i] + C.w_knot[i + 1]) * (P.times[i + 1] - P.times[i]);
-        for (int it = 0; it < 3; ++it) {
-            const double n_est = std::max(w_total / std::max(rho_target, 1.0), 1.0);
-            rho_target = std::min(rho_max, std::max(4.0, std::log(0.2 * gtol / (kRoundUnit * std::sqrt(n_est)))));
-        }
-    }
-    double round2 = 0.0;   // sum of squares of the per-step rounding estimates
-    const PiecewiseCubic<double>& m_pc = C.mshape;
-    const double A_sum = std::max(C.a_sum_max, 1e-300), C_sum = std::max(C.c_sum_max, 1e-300);
-    pb200_run_stats st{};
-    EventPair evs;
-    CUDA_CHECK(cudaEventRecord(evs.a, P.stream));
-    ensure_aux_buffers(P);
+// One step of the Taylor propagator as the host schedules it: the polynomial fits, the centres gamma_j, the order K and
+// the ring it needs.  Everything here is decided a priori, before any launch of the step.
+struct TaylorStep {
+    double t = 0.0, h = 0.0;
+    std::vector<double> om, th, m;   // monomial coefficients in u of omega, theta, M (trailing zeros trimmed)
+    int p_om = 0, p_th = 0, p = 0;
+    std::vector<double> gam;         // centres of H_j
+    int K = 0;
+    double phi = 0.0;                // phase of the scalar centre over the step
+    int n_chi = 0, n_g = 0;          // chi ring (slot 0 = the current state), G ring
+    int ring() const { return (n_chi - 1) + n_g + 1; }   // state-sized buffers beyond the state itself
+};
 
-    // fit of both coefficient functions on [a, a+h] with the smallest degrees that meet the residual budget
-    // The fit error is budgeted over the call: 50 % of its share of the tolerance (10 % goes to the Taylor remainders).  Smooth stretches fit to rounding
-    // and spend nothing, so a step may also use 2 % of what is still unspent -- this is what shortens the stretches of
-    // one-interval steps around a non-smooth sample, where the not-a-knot spline rings with a factor 0.268 per
-    // interval (|dH| <= (r_om + r_th) N, state error <= h |dH|).
-    const double fit_total = 0.5 * rate * (t_stop - t_start);
-    double fit_spent = 0.0;
+// Host half of propagate_taylor: the steps of one call [t_start, t_stop], one at a time (next()), with the statistics
+// the launches do not change.  The single-plan path launches every step as soon as it is scheduled (the host fit of
+// the next step overlaps the device work); the sharded path schedules the whole call before its first launch.
+struct TaylorScheduler {
+    Plan& P;
+    double t_stop, eps = 1e-12, gtol, rate, rho_target, fit_total, fit_spent = 0.0, round2 = 0.0;
+    double t, steps_len = 0.0, t_retry_len = 0.0, A_sum, C_sum, kRoundUnit = 0.05 * 1.1102230246251565e-16;
+    int pmax, order, N, nt;
+    bool log_steps;
+    pb200_run_stats st{};
     struct Fit { TaylorPoly om, th, m; bool ok; };
-    auto fit_step = [&](double a, double h, bool single_piece) {
+
+    TaylorScheduler(Plan& P_, double t_start, double t_stop_, const pb200_run_opts* o) : P(P_), t_stop(t_stop_), t(t_start) {
+        const double tlo = P.times.front(), thi = P.times.back();
+        gtol = (o && o->tol > 0.0) ? o->tol : 1e-8;
+        rate = gtol / std::max(thi - tlo, 1e-30);       // error budget per unit of time
+        const double rho_max = env_int("PB200_TAYLOR_RHO_MILLI", 14000) * 1e-3;
+        pmax = std::min(PB200_TAYLOR_PMAX, std::max(1, env_int("PB200_TAYLOR_P", PB200_TAYLOR_PMAX)));
+        order = P.desc.interp_order;
+        N = P.n;
+        nt = (int)P.times.size();
+        Plan::TaylorCache& C = P.tay;
+        taylor_knot_widths(P);
+        // Step length: rho = h W <= rho_max, lowered where the fp64 cancellation of the series would eat the tolerance.  The
+        // rounding error of a step grows like e^rho: ~0.05 eps e^rho measured (tools/taylor_rho_sweep.py: 6e-12 per
+        // step at rho = 14, 1.4e-10 at 18), random from step to step, n ~ (int W dt) / rho steps over the whole sequence;
+        // it may use a fifth of the tolerance.  At the default 1e-8 this never binds (17 > 14 for C2, C4, C5).
+        rho_target = rho_max;
+        {
+            double w_total = 0.0;
+            for (int i = 0; i + 1 < nt; ++i) w_total += 0.5 * (C.w_knot[i] + C.w_knot[i + 1]) * (P.times[i + 1] - P.times[i]);
+            for (int it = 0; it < 3; ++it) {
+                const double n_est = std::max(w_total / std::max(rho_target, 1.0), 1.0);
+                rho_target = std::min(rho_max, std::max(4.0, std::log(0.2 * gtol / (kRoundUnit * std::sqrt(n_est)))));
+            }
+        }
+        A_sum = std::max(C.a_sum_max, 1e-300); C_sum = std::max(C.c_sum_max, 1e-300);
+        // The fit error is budgeted over the call: 50 % of its share of the tolerance (10 % goes to the Taylor remainders).
+        fit_total = 0.5 * rate * (t_stop - t_start);
+        log_steps = env_int("PB200_TAYLOR_LOG", 0) != 0;
+    }
+
+    // fit of both coefficient functions on [a, a+h] with the smallest degrees that meet the residual budget.
+    // Smooth stretches fit to rounding and spend nothing, so a step may also use 2 % of what is still unspent -- this is
+    // what shortens the stretches of one-interval steps around a non-smooth sample, where the not-a-knot spline rings with
+    // a factor 0.268 per interval (|dH| <= (r_om + r_th) N, state error <= h |dH|).
+    Fit fit_step(double a, double h, bool single_piece) {
+        const Plan::TaylorCache& C = P.tay;
         Fit F; F.ok = false;
         const double budget = std::max(0.5 * rate * h, 0.02 * std::max(fit_total - fit_spent, 0.0));
         // |dH| <= r_om sum|a| + r_th N + r_M sum|c| : a third of the step's allowance each
@@ -2169,177 +2192,226 @@ static void propagate_taylor(Plan& P, double t_start, double t_stop, const pb200
             if (single_piece) out = taylor_fit(pc, P.times, order, a, h, pmax);
             return true;
         };
-        F.ok = one(om_pc, F.om, third / A_sum) && one(th_pc, F.th, third / N);
-        if (F.ok && C.has_m) F.ok = one(m_pc, F.m, third / C_sum);
+        F.ok = one(C.om, F.om, third / A_sum) && one(P.tabs[0][0].det[0], F.th, third / N);
+        if (F.ok && C.has_m) F.ok = one(C.mshape, F.m, third / C_sum);
         if (!C.has_m) { F.m.c.assign(1, 0.0); F.m.resid = 0.0; }
         return F;
-    };
+    }
 
-    double t = t_start;
-    double steps_len = 0.0;
-    double t_retry_len = 0.0;   // > 0: the previous attempt at this step overshot rho; cap on the step length
-    const bool log_steps = env_int("PB200_TAYLOR_LOG", 0) != 0;
-    while (t < t_stop - eps) {
-        const int i0 = find_piece(P.times, t + eps);
-        // longest candidate: accumulate rho over the sampling intervals
-        double b = t;
-        {
-            double acc = 0.0;
-            int i = i0;
-            double cur = t;
-            while (i < nt - 1) {
-                const double e1 = std::min(P.times[i + 1], t_stop);
-                const double w = std::max(C.w_knot[i], C.w_knot[i + 1]);
-                const double need = w * (e1 - cur);
-                if (acc + need > rho_target) {
-                    if (i == i0 || acc == 0.0) b = cur + (rho_target - acc) / std::max(w, 1e-300);  // inside the first interval
-                    else b = cur;
-                    break;
+    // the next step of the call; false once t_stop is reached
+    bool next(TaylorStep& s) {
+        const Plan::TaylorCache& C = P.tay;
+        while (t < t_stop - eps) {
+            const int i0 = find_piece(P.times, t + eps);
+            // longest candidate: accumulate rho over the sampling intervals
+            double b = t;
+            {
+                double acc = 0.0;
+                int i = i0;
+                double cur = t;
+                while (i < nt - 1) {
+                    const double e1 = std::min(P.times[i + 1], t_stop);
+                    const double w = std::max(C.w_knot[i], C.w_knot[i + 1]);
+                    const double need = w * (e1 - cur);
+                    if (acc + need > rho_target) {
+                        if (i == i0 || acc == 0.0) b = cur + (rho_target - acc) / std::max(w, 1e-300);  // inside the first interval
+                        else b = cur;
+                        break;
+                    }
+                    acc += need; cur = e1; b = e1; ++i;
+                    if (e1 >= t_stop - eps) break;
                 }
-                acc += need; cur = e1; b = e1; ++i;
-                if (e1 >= t_stop - eps) break;
+                b = std::min(b, t_stop);
+                if (t_retry_len > 0.0) { b = std::min(b, t + t_retry_len); t_retry_len = 0.0; }
+                if (b <= t + eps) b = std::min(P.times[i0 + 1], t_stop);
             }
-            b = std::min(b, t_stop);
-            if (t_retry_len > 0.0) { b = std::min(b, t + t_retry_len); t_retry_len = 0.0; }
-            if (b <= t + eps) b = std::min(P.times[i0 + 1], t_stop);
-        }
-        // longest step on which both splines are polynomials of degree <= pmax to within the budget: bisection over
-        // the number of whole sampling intervals beyond the first one (a step inside one interval is a cubic: exact)
-        Fit F;
-        {
-            bool single = b <= P.times[i0 + 1] + eps;
-            F = fit_step(t, b - t, single);
-            if (!F.ok && !single) {
-                int lo_keep = 0, hi_keep = find_piece(P.times, b - eps) - i0;   // lo passes (one interval), hi fails
-                Fit Flo; bool have_lo = false;
-                while (hi_keep - lo_keep > 1) {
-                    const int mid = (lo_keep + hi_keep) / 2;
-                    const double bm = P.times[i0 + 1 + mid];
-                    Fit Fm = fit_step(t, bm - t, false);
-                    if (Fm.ok) { lo_keep = mid; Flo = Fm; have_lo = true; } else hi_keep = mid;
+            // longest step on which both splines are polynomials of degree <= pmax to within the budget: bisection over
+            // the number of whole sampling intervals beyond the first one (a step inside one interval is a cubic: exact)
+            Fit F;
+            {
+                bool single = b <= P.times[i0 + 1] + eps;
+                F = fit_step(t, b - t, single);
+                if (!F.ok && !single) {
+                    int lo_keep = 0, hi_keep = find_piece(P.times, b - eps) - i0;   // lo passes (one interval), hi fails
+                    Fit Flo; bool have_lo = false;
+                    while (hi_keep - lo_keep > 1) {
+                        const int mid = (lo_keep + hi_keep) / 2;
+                        const double bm = P.times[i0 + 1 + mid];
+                        Fit Fm = fit_step(t, bm - t, false);
+                        if (Fm.ok) { lo_keep = mid; Flo = Fm; have_lo = true; } else hi_keep = mid;
+                    }
+                    b = P.times[i0 + 1 + lo_keep];
+                    single = lo_keep == 0;
+                    F = have_lo ? Flo : fit_step(t, b - t, single);
                 }
-                b = P.times[i0 + 1 + lo_keep];
-                single = lo_keep == 0;
-                F = have_lo ? Flo : fit_step(t, b - t, single);
             }
-        }
-        double h = b - t;
-        // strip trailing zero coefficients
-        auto trim = [](std::vector<double>& c, double scale) {
-            while (c.size() > 1 && std::fabs(c.back()) <= 1e-15 * scale) c.pop_back();
-        };
-        {
-            double so = 0.0, sh = 0.0, sm = 0.0;
-            for (double v : F.om.c) so = std::max(so, std::fabs(v));
-            for (double v : F.th.c) sh = std::max(sh, std::fabs(v));
-            for (double v : F.m.c) sm = std::max(sm, std::fabs(v));
-            trim(F.om.c, std::max(so, 1e-300)); trim(F.th.c, std::max(sh, 1e-300)); trim(F.m.c, std::max(sm, 1e-300));
-        }
-        const int p_om = (int)F.om.c.size() - 1, p_m = (int)F.m.c.size() - 1;
-        const int p_th = std::max((int)F.th.c.size() - 1, p_m);   // degree of the diagonal (own-element) history
-        const int p = std::max(p_om, p_th);
-        auto th_c = [&](int j) { return j < (int)F.th.c.size() ? F.th.c[j] : 0.0; };
-        auto m_c = [&](int j) { return j < (int)F.m.c.size() ? F.m.c[j] : 0.0; };
-        // centres and norm bounds of H_j
-        std::vector<double> gam(p + 1, 0.0), mj(p + 1, 0.0);
-        {
-            double c0, hw0;
-            taylor_bounds(P, F.om.c[0], F.th.c[0], m_c(0), c0, hw0);
-            gam[0] = c0; mj[0] = hw0;
-            for (int j = 1; j <= p; ++j) {
-                const double thj = th_c(j), omj = j <= p_om ? F.om.c[j] : 0.0;
-                gam[j] = -thj * 0.5 * N;
-                mj[j] = std::fabs(thj) * 0.5 * N + std::fabs(m_c(j)) * C_sum + std::fabs(omj) * A_sum;
+            double h = b - t;
+            // strip trailing zero coefficients
+            auto trim = [](std::vector<double>& c, double scale) {
+                while (c.size() > 1 && std::fabs(c.back()) <= 1e-15 * scale) c.pop_back();
+            };
+            {
+                double so = 0.0, sh = 0.0, sm = 0.0;
+                for (double v : F.om.c) so = std::max(so, std::fabs(v));
+                for (double v : F.th.c) sh = std::max(sh, std::fabs(v));
+                for (double v : F.m.c) sm = std::max(sm, std::fabs(v));
+                trim(F.om.c, std::max(so, 1e-300)); trim(F.th.c, std::max(sh, 1e-300)); trim(F.m.c, std::max(sm, 1e-300));
             }
-        }
-        {   // the fp64 cancellation of the series grows like e^rho: a step whose majorant exponent overshoots the
-            // target (the half-width grew inside the step) is cut and fitted again
+            const int p_om = (int)F.om.c.size() - 1, p_m = (int)F.m.c.size() - 1;
+            const int p_th = std::max((int)F.th.c.size() - 1, p_m);   // degree of the diagonal (own-element) history
+            const int p = std::max(p_om, p_th);
+            auto th_c = [&](int j) { return j < (int)F.th.c.size() ? F.th.c[j] : 0.0; };
+            auto m_c = [&](int j) { return j < (int)F.m.c.size() ? F.m.c[j] : 0.0; };
+            // centres and norm bounds of H_j
+            std::vector<double> gam(p + 1, 0.0), mj(p + 1, 0.0);
+            {
+                double c0, hw0;
+                taylor_bounds(P, F.om.c[0], F.th.c[0], m_c(0), c0, hw0);
+                gam[0] = c0; mj[0] = hw0;
+                for (int j = 1; j <= p; ++j) {
+                    const double thj = th_c(j), omj = j <= p_om ? F.om.c[j] : 0.0;
+                    gam[j] = -thj * 0.5 * N;
+                    mj[j] = std::fabs(thj) * 0.5 * N + std::fabs(m_c(j)) * C_sum + std::fabs(omj) * A_sum;
+                }
+            }
+            {   // the fp64 cancellation of the series grows like e^rho: a step whose majorant exponent overshoots the
+                // target (the half-width grew inside the step) is cut and fitted again
+                double rho_eff = 0.0;
+                for (int j = 0; j <= p; ++j) rho_eff += mj[j] / (j + 1);
+                rho_eff *= h;
+                if (rho_eff > 1.12 * rho_target && h > 1e-9) {
+                    t_retry_len = h * rho_target / rho_eff;
+                    continue;
+                }
+            }
+            double trunc_bound = 0.0;
+            const int K = taylor_order(h, mj, std::max(1e-15, 0.1 * rate * h), trunc_bound);
+            s.t = t; s.h = h;
+            s.om = F.om.c; s.th = F.th.c; s.m = F.m.c;
+            s.p_om = p_om; s.p_th = p_th; s.p = p;
+            s.gam = gam; s.K = K;
+            s.n_chi = p_th + 2;
+            s.n_g = p_om >= 1 ? p_om + 1 : 0;
+            // phase of the scalar centre: exp(-i h int_0^1 sum_j gam_j u^j du)
+            double phi = 0.0;
+            for (int j = 0; j <= p; ++j) phi += gam[j] / (j + 1);
+            s.phi = phi * h;
+            st.n_applies += K; st.n_exponentials += 1; ++st.n_steps;
+            if (log_steps)
+                fprintf(stderr, "taylor step t=%.6f h_ns=%.3f p_om=%d p_th=%d p_m=%d K=%d ring=%d rho=%.3f resid=%.2e/%.2e/%.2e\n", t,
+                        h * 1e3, p_om, p_th, p_m, K, s.ring() + 1, mj[0] * h, F.om.resid, F.th.resid, F.m.resid);
             double rho_eff = 0.0;
             for (int j = 0; j <= p; ++j) rho_eff += mj[j] / (j + 1);
-            rho_eff *= h;
-            if (rho_eff > 1.12 * rho_target && h > 1e-9) {
-                t_retry_len = h * rho_target / rho_eff;
-                continue;
-            }
+            st.max_rho = std::max(st.max_rho, rho_eff * h);
+            const double fit_err = h * (A_sum * F.om.resid + N * F.th.resid + C_sum * F.m.resid);
+            st.err_estimate += trunc_bound + fit_err;
+            fit_spent += fit_err;
+            { const double r = kRoundUnit * std::exp(std::min(rho_eff * h, 40.0)); round2 += r * r; }
+            steps_len += h;
+            t = b;
+            return true;
         }
-        double trunc_bound = 0.0;
-        const int K = taylor_order(h, mj, std::max(1e-15, 0.1 * rate * h), trunc_bound);
-        // buffers: chi ring (slot 0 = the current state), G ring, accumulator
-        const int n_chi = p_th + 2;
-        const int n_g = p_om >= 1 ? p_om + 1 : 0;
-        std::vector<c2**> free_slots;
-        for (int i = 0; i < 3; ++i) if (i != P.cur) free_slots.push_back(&P.buf[i]);
-        for (int i = 0; i < 6; ++i) free_slots.push_back(&P.aux[i]);
-        const int need = (n_chi - 1) + n_g + 1;
-        while ((int)free_slots.size() + (int)P.tay_ws.size() < need)
-            P.tay_ws.push_back((c2*)pool_alloc(P.desc.device, sizeof(c2) * (size_t)P.D * P.B));
-        for (size_t i = 0; i < P.tay_ws.size(); ++i) free_slots.push_back(&P.tay_ws[i]);
-        std::vector<c2*> chi(n_chi), gr(n_g);
-        int fs = 0;
-        chi[0] = P.buf[P.cur];
-        for (int i = 1; i < n_chi; ++i) chi[i] = *free_slots[fs++];
-        for (int i = 0; i < n_g; ++i) gr[i] = *free_slots[fs++];
-        c2** acc_slot = free_slots[fs++];
-        c2* acc = *acc_slot;
-        // phase of the scalar centre: exp(-i h int_0^1 sum_j gam_j u^j du)
-        double phi = 0.0;
-        for (int j = 0; j <= p; ++j) phi += gam[j] / (j + 1);
-        phi *= h;
-        long long launches = 0;
-        for (int k = 0; k < K; ++k) {
-            TaylorArgs a{};
-            a.v = chi[k % n_chi]; a.out = chi[(k + 1) % n_chi];
-            a.g_out = (n_g && k + 1 < K) ? gr[k % n_g] : nullptr;
-            a.acc = acc;
-            a.dint = P.has_interaction ? P.dint : nullptr;
-            a.dint_stride = P.dint_shared ? 0 : P.D;
-            a.D = P.D;
-            a.geo = passes[0];
-            a.unit = C.unit;
-            a.table = C.uniform ? nullptr : C.d_tab;
-            a.to_bit = P.desc.drives[0].state_to; a.from_is_one = P.desc.drives[0].state_from;
-            a.th0 = F.th.c[0]; a.gam0 = gam[0]; a.om0 = F.om.c[0]; a.m0 = m_c(0);
-            a.scale = {0.0, -h / (k + 1)};
-            a.nh = std::min(p, k);
-            for (int j = 1; j <= a.nh; ++j) {
-                const double thj = th_c(j), mjv = m_c(j), omj = j <= p_om ? F.om.c[j] : 0.0;
-                a.hth[j - 1] = thj; a.hgam[j - 1] = gam[j]; a.hom[j - 1] = omj; a.hm[j - 1] = mjv;
-                a.hchi[j - 1] = (thj != 0.0 || mjv != 0.0 || gam[j] != 0.0) ? chi[(k - j) % n_chi] : nullptr;
-                a.hg[j - 1] = (omj != 0.0) ? gr[(k - j) % n_g] : nullptr;
-            }
-            const bool last = (k + 1 == K);
-            if ((k & 1) == 0) { a.acc_on = 1; a.acc_add_v = 1; a.acc_read = k > 0; }
-            else { a.acc_on = last ? 1 : 0; a.acc_add_v = 0; a.acc_read = 1; }
-            a.acc_mul = last ? c2{std::cos(phi), -std::sin(phi)} : c2{1.0, 0.0};
-            launch_taylor_stage(P, use_rb ? &passes[0] : nullptr, a, launches);
-        }
+        return false;
+    }
+
+    // statistics of the whole call (gpu_ms and n_launches come from the launching half)
+    pb200_run_stats finish(double gpu_ms, long long launches) const {
+        pb200_run_stats out = st;
+        out.gpu_ms = gpu_ms;
+        out.n_launches = launches;
+        const double hi_mean = (P.times.back() - P.times.front()) / std::max(nt - 1, 1);
+        out.mean_step_samples = out.n_steps ? steps_len / out.n_steps / hi_mean : 0.0;
+        out.err_estimate += std::sqrt(round2);
+        out.integrator = 3;
+        return out;
+    }
+};
+
+// Ring of one step: chi[0] = the current state, the other slots from the buffers that are not the state (the Magnus
+// aux buffers too when the plan has them), then the plan's own Taylor work buffers, allocated on first need.
+struct TaylorRing {
+    std::vector<c2*> chi, gr;
+    c2** acc_slot = nullptr;
+};
+
+static void taylor_grow_ring(Plan& P, int need) {
+    int have = 2 + (P.aux[0] ? 6 : 0) + (int)P.tay_ws.size();
+    while (have < need) {
+        P.tay_ws.push_back((c2*)pool_alloc(P.desc.device, sizeof(c2) * (size_t)P.D * P.B));
+        ++have;
+    }
+}
+
+static TaylorRing taylor_ring(Plan& P, const TaylorStep& s) {
+    std::vector<c2**> free_slots;
+    for (int i = 0; i < 3; ++i) if (i != P.cur) free_slots.push_back(&P.buf[i]);
+    if (P.aux[0]) for (int i = 0; i < 6; ++i) free_slots.push_back(&P.aux[i]);
+    taylor_grow_ring(P, s.ring());
+    for (size_t i = 0; i < P.tay_ws.size(); ++i) free_slots.push_back(&P.tay_ws[i]);
+    TaylorRing R;
+    R.chi.resize(s.n_chi); R.gr.resize(s.n_g);
+    int fs = 0;
+    R.chi[0] = P.buf[P.cur];
+    for (int i = 1; i < s.n_chi; ++i) R.chi[i] = *free_slots[fs++];
+    for (int i = 0; i < s.n_g; ++i) R.gr[i] = *free_slots[fs++];
+    R.acc_slot = free_slots[fs++];
+    return R;
+}
+
+// arguments of order k of a step
+static TaylorArgs taylor_args(const Plan& P, const PassGeom& geo, const TaylorStep& s, const TaylorRing& R, int k) {
+    const Plan::TaylorCache& C = P.tay;
+    auto th_c = [&](int j) { return j < (int)s.th.size() ? s.th[j] : 0.0; };
+    auto m_c = [&](int j) { return j < (int)s.m.size() ? s.m[j] : 0.0; };
+    TaylorArgs a{};
+    a.v = R.chi[k % s.n_chi]; a.out = R.chi[(k + 1) % s.n_chi];
+    a.g_out = (s.n_g && k + 1 < s.K) ? R.gr[k % s.n_g] : nullptr;
+    a.acc = *R.acc_slot;
+    a.dint = P.has_interaction ? P.dint : nullptr;
+    a.dint_stride = P.dint_shared ? 0 : P.D;
+    a.D = P.D;
+    a.geo = geo;
+    a.unit = C.unit;
+    a.table = C.uniform ? nullptr : C.d_tab;
+    a.to_bit = P.desc.drives[0].state_to; a.from_is_one = P.desc.drives[0].state_from;
+    a.th0 = s.th[0]; a.gam0 = s.gam[0]; a.om0 = s.om[0]; a.m0 = m_c(0);
+    a.scale = {0.0, -s.h / (k + 1)};
+    a.nh = std::min(s.p, k);
+    for (int j = 1; j <= a.nh; ++j) {
+        const double thj = th_c(j), mjv = m_c(j), omj = j <= s.p_om ? s.om[j] : 0.0;
+        a.hth[j - 1] = thj; a.hgam[j - 1] = s.gam[j]; a.hom[j - 1] = omj; a.hm[j - 1] = mjv;
+        a.hchi[j - 1] = (thj != 0.0 || mjv != 0.0 || s.gam[j] != 0.0) ? R.chi[(k - j) % s.n_chi] : nullptr;
+        a.hg[j - 1] = (omj != 0.0) ? R.gr[(k - j) % s.n_g] : nullptr;
+    }
+    const bool last = (k + 1 == s.K);
+    if ((k & 1) == 0) { a.acc_on = 1; a.acc_add_v = 1; a.acc_read = k > 0; }
+    else { a.acc_on = last ? 1 : 0; a.acc_add_v = 0; a.acc_read = 1; }
+    a.acc_mul = last ? c2{std::cos(s.phi), -std::sin(s.phi)} : c2{1.0, 0.0};
+    return a;
+}
+
+static void propagate_taylor(Plan& P, double t_start, double t_stop, const pb200_run_opts* o, pb200_run_stats* stats) {
+    std::vector<PassGeom> passes;
+    bool use_rb = false;
+    if (!taylor_geometry(P, passes, use_rb)) fail(PB200_ERR_UNSUPPORTED, "Taylor propagator: unsupported register size");
+    EventPair evs;
+    CUDA_CHECK(cudaEventRecord(evs.a, P.stream));
+    ensure_aux_buffers(P);
+    TaylorScheduler S(P, t_start, t_stop, o);
+    TaylorStep s;
+    long long launches = 0;
+    while (S.next(s)) {
+        const TaylorRing R = taylor_ring(P, s);
+        for (int k = 0; k < s.K; ++k) launch_taylor_stage(P, use_rb ? &passes[0] : nullptr, taylor_args(P, passes[0], s, R, k), launches);
         CUDA_CHECK(cudaGetLastError());
         // the accumulator becomes the current state buffer
-        std::swap(P.buf[P.cur], *acc_slot);
-        st.n_launches += launches; st.n_applies += K; st.n_exponentials += 1; ++st.n_steps;
-        if (log_steps)
-            fprintf(stderr, "taylor step t=%.6f h_ns=%.3f p_om=%d p_th=%d p_m=%d K=%d rho=%.3f resid=%.2e/%.2e/%.2e\n", t, h * 1e3, p_om,
-                    p_th, p_m, K, mj[0] * h, F.om.resid, F.th.resid, F.m.resid);
-        double rho_eff = 0.0;
-        for (int j = 0; j <= p; ++j) rho_eff += mj[j] / (j + 1);
-        st.max_rho = std::max(st.max_rho, rho_eff * h);
-        const double fit_err = h * (A_sum * F.om.resid + N * F.th.resid + C_sum * F.m.resid);
-        st.err_estimate += trunc_bound + fit_err;
-        fit_spent += fit_err;
-        { const double r = kRoundUnit * std::exp(std::min(rho_eff * h, 40.0)); round2 += r * r; }
-        steps_len += h;
-        t = b;
+        std::swap(P.buf[P.cur], *R.acc_slot);
     }
     CUDA_CHECK(cudaEventRecord(evs.b, P.stream));
     CUDA_CHECK(cudaEventSynchronize(evs.b));
     float ms = 0.f;
     CUDA_CHECK(cudaEventElapsedTime(&ms, evs.a, evs.b));
-    st.gpu_ms = ms;
-    const double hi_mean = (thi - tlo) / std::max(nt - 1, 1);
-    st.mean_step_samples = st.n_steps ? steps_len / st.n_steps / hi_mean : 0.0;
-    st.err_estimate += std::sqrt(round2);
-    st.integrator = 3;
-    if (stats) *stats = st;
+    if (stats) *stats = S.finish(ms, launches);
 }
 
 // H(t) parameters as an "exponential" description with w = 1 (for apply_h)
@@ -2417,6 +2489,101 @@ struct pb200_plan {
     Plan p;
 };
 
+// entry points that act on a whole state through one plan: a shard only holds a slice
+static void refuse_shard(const Plan& P, const char* who, const char* instead) {
+    if (P.shard_bits)
+        fail(PB200_ERR_STATE, "%s: the plan is shard %d of %d of a state; use %s on the linked shards", who, P.shard,
+             1 << P.shard_bits, instead);
+}
+
+// ---- state-vector shards -------------------------------------------------------------------------------------------
+// A shard is an ordinary plan holding 2^L amplitudes (L = N - shard_bits) of one state: the global indices
+// [shard 2^L, (shard + 1) 2^L).  One process drives every shard of a group: the host schedule of a call is computed
+// once, then every order of the Taylor series is launched on every shard (stage_d2_taylor_kernel<..., true>), whose
+// partners across a shard bit are loads from the peer's chi_k (peer access between distinct devices).
+
+// the one-pass geometry of a slice: the 2^13 tile, the local bits above it as partner loads; n_bits = global N
+static PassGeom shard_geometry(const Plan& P) {
+    const std::vector<PassGeom> passes = plan_passes(P.n - P.shard_bits, kTaylorTileBits, kShardMaxLocalBits - kTaylorTileBits);
+    if (passes.size() != 1) fail(PB200_ERR_UNSUPPORTED, "shard of 2^%d amplitudes: no single-pass geometry", P.n - P.shard_bits);
+    PassGeom g = passes[0];
+    g.n_bits = P.n;
+    return g;
+}
+
+// one order on one shard; no programmatic dependent launch: an order waits for its peers through events
+static void launch_taylor_shard(Plan& P, const TaylorArgs& a) {
+    constexpr int TB = kTaylorTileBits, RB = kTaylorRegBits;
+    const bool real_g = a.unit.y == 0.0;
+    dim3 grid((unsigned)(P.D >> TB)), block(1 << (TB - RB));
+    const size_t smem = ((size_t)16 << TB) + (real_g ? 0 : (size_t)d2_table_stride(P.n) * 8);
+    if (real_g) launch_k(stage_d2_taylor_kernel<true, true, TB, RB, true>, grid, block, smem, P.stream, false, a);
+    else launch_k(stage_d2_taylor_kernel<true, false, TB, RB, true>, grid, block, smem, P.stream, false, a);
+}
+
+// plans[i] = shard i of a group linked by pb200_shards_link
+static std::vector<Plan*> shard_group(pb200_plan** plans, int count, const char* who) {
+    if (!plans || count < 2) fail(PB200_ERR_INVALID, "%s: pass the plans of every shard", who);
+    std::vector<Plan*> G(count);
+    for (int i = 0; i < count; ++i) {
+        if (!plans[i]) fail(PB200_ERR_INVALID, "%s: null plan", who);
+        G[i] = &plans[i]->p;
+    }
+    for (int i = 0; i < count; ++i)
+        if (G[i]->group != G)
+            fail(PB200_ERR_STATE, "%s: plans[] is not a linked shard group in shard order (pb200_shards_link)", who);
+    return G;
+}
+
+// CUDA events of a group, one per shard, released on every exit path
+struct ShardEvents {
+    std::vector<cudaEvent_t> ev;
+    ShardEvents(const std::vector<Plan*>& G, unsigned flags) : ev(G.size(), nullptr) {
+        for (size_t r = 0; r < G.size(); ++r) {
+            CUDA_CHECK(cudaSetDevice(G[r]->desc.device));
+            CUDA_CHECK(cudaEventCreateWithFlags(&ev[r], flags));
+        }
+    }
+    ~ShardEvents() { for (cudaEvent_t e : ev) if (e) cudaEventDestroy(e); }
+    ShardEvents(const ShardEvents&) = delete;
+    ShardEvents& operator=(const ShardEvents&) = delete;
+};
+
+static void shards_sync(const std::vector<Plan*>& G) {
+    for (Plan* P : G) {
+        CUDA_CHECK(cudaSetDevice(P->desc.device));
+        CUDA_CHECK(cudaStreamSynchronize(P->stream));
+    }
+}
+
+// out_r = H(t) in_r on every shard: the sharded stage with scale 1, no history and the accumulator off computes
+// (Dint - theta n_from + omega X) v.  The inputs are complete (every stream synchronised) before any shard reads a peer's.
+static void shards_apply_h(const std::vector<Plan*>& G, double t, const std::vector<c2*>& in, const std::vector<c2*>& out) {
+    const Plan& P0 = *G[0];
+    const PassGeom geo = shard_geometry(P0);
+    const int order = P0.desc.interp_order;
+    const double om = eval_at(P0.tay.om, P0.times, t, order), th = eval_at(P0.tabs[0][0].det[0], P0.times, t, order);
+    shards_sync(G);
+    const int count = (int)G.size();
+    for (int r = 0; r < count; ++r) {
+        Plan& P = *G[r];
+        TaylorArgs a{};
+        a.v = in[r]; a.out = out[r];
+        a.dint = P.has_interaction ? P.dint : nullptr;
+        a.D = P.D; a.geo = geo; a.unit = P.tay.unit;
+        a.to_bit = P.desc.drives[0].state_to; a.from_is_one = P.desc.drives[0].state_from;
+        a.th0 = th; a.om0 = om;
+        a.scale = {1.0, 0.0};
+        a.acc_mul = {1.0, 0.0};
+        a.shard_bits = P.shard_bits; a.shard = r;
+        for (int q = 0; q < P.shard_bits; ++q) a.peer[q] = in[r ^ (1 << q)];
+        CUDA_CHECK(cudaSetDevice(P.desc.device));
+        launch_taylor_shard(P, a);
+    }
+    CUDA_CHECK(cudaGetLastError());
+    shards_sync(G);
+}
+
 #define PB200_TRY try {
 #define PB200_CATCH                                         \
     }                                                       \
@@ -2442,11 +2609,8 @@ int pb200_device_count(void) {
     return n;
 }
 
-int pb200_plan_create(pb200_plan** out, const pb200_plan_desc* d) {
-    PB200_TRY
-    NvtxRange nvtx_range("pb200_plan_create");
-    if (!out || !d) fail(PB200_ERR_INVALID, "null argument");
-    *out = nullptr;
+// checks of a plan description that need no device
+static void check_desc(const pb200_plan_desc* d) {
     if (d->n_qudits < 1 || d->n_qudits > PB200_MAX_QUDITS) fail(PB200_ERR_INVALID, "n_qudits out of range");
     if (d->dim < 2 || d->dim > 4) fail(PB200_ERR_INVALID, "dim must be 2, 3 or 4");
     if (d->n_times < 2 || !d->sampling_times) fail(PB200_ERR_INVALID, "need >= 2 sampling times");
@@ -2462,7 +2626,11 @@ int pb200_plan_create(pb200_plan** out, const pb200_plan_desc* d) {
             dd.state_to == dd.state_from)
             fail(PB200_ERR_INVALID, "drive %d: bad eigenstate indices", q);
     }
-    double Dd = std::pow((double)d->dim, d->n_qudits);
+}
+
+// shard_bits = 0: a whole state; else the plan holds shard `shard` of 2^shard_bits (checked by the caller)
+static void create_plan(pb200_plan** out, const pb200_plan_desc* d, int shard_bits, int shard) {
+    double Dd = std::pow((double)d->dim, d->n_qudits) / (double)(1LL << shard_bits);
     if (Dd * d->n_traj > 4.0e9) fail(PB200_ERR_UNSUPPORTED, "state too large: %g amplitudes", Dd * d->n_traj);
     int ndev = 0;
     if (cudaGetDeviceCount(&ndev) != cudaSuccess || ndev == 0) {
@@ -2479,7 +2647,9 @@ int pb200_plan_create(pb200_plan** out, const pb200_plan_desc* d) {
     P.n = d->n_qudits; P.dim = d->dim; P.B = d->n_traj; P.n_drives = d->n_drives;
     long long D = 1;
     for (int i = 0; i < P.n; ++i) D *= P.dim;
+    D >>= shard_bits;
     P.D = D;
+    P.shard_bits = shard_bits; P.shard = shard;
     P.tile_bits = std::min(13, std::max(2, env_int("PB200_TILE_BITS", 11)));
     P.max_extra = std::max(0, env_int("PB200_MAX_EXTRA", 16));
     P.force_v1 = env_int("PB200_FORCE_V1", 0) != 0;
@@ -2504,6 +2674,36 @@ int pb200_plan_create(pb200_plan** out, const pb200_plan_desc* d) {
     P.tabs_set.assign(P.B, std::vector<bool>(P.n_drives, false));
     P.has_interaction = false;
     *out = h;
+}
+
+int pb200_plan_create(pb200_plan** out, const pb200_plan_desc* d) {
+    PB200_TRY
+    NvtxRange nvtx_range("pb200_plan_create");
+    if (!out || !d) fail(PB200_ERR_INVALID, "null argument");
+    *out = nullptr;
+    check_desc(d);
+    create_plan(out, d, 0, 0);
+    PB200_CATCH
+}
+
+int pb200_plan_create_shard(pb200_plan** out, const pb200_plan_desc* d, int32_t shard_bits, int32_t shard_index) {
+    PB200_TRY
+    NvtxRange nvtx_range("pb200_plan_create_shard");
+    if (!out || !d) fail(PB200_ERR_INVALID, "null argument");
+    *out = nullptr;
+    check_desc(d);
+    if (shard_bits < 1 || shard_bits > PB200_MAX_SHARD_BITS)
+        fail(PB200_ERR_INVALID, "shard_bits = %d: must be 1, 2 or 3 (2, 4 or 8 shards)", shard_bits);
+    if (shard_index < 0 || shard_index >= (1 << shard_bits))
+        fail(PB200_ERR_INVALID, "shard_index = %d out of range [0, %d)", shard_index, 1 << shard_bits);
+    const int L = d->n_qudits - shard_bits;
+    if (L < kTaylorTileBits || L > kShardMaxLocalBits)
+        fail(PB200_ERR_INVALID, "N - shard_bits = %d: a shard holds 2^%d to 2^%d amplitudes", L, kTaylorTileBits,
+             kShardMaxLocalBits);
+    if (d->dim != 2 || d->n_drives != 1 || d->n_traj != 1)
+        fail(PB200_ERR_UNSUPPORTED, "shards hold one state (n_traj = 1) of a d = 2 register with one drive (got d = %d, %d drives, "
+                                    "%d trajectories)", d->dim, d->n_drives, d->n_traj);
+    create_plan(out, d, shard_bits, shard_index);
     PB200_CATCH
 }
 
@@ -2511,6 +2711,8 @@ int pb200_plan_destroy(pb200_plan* h) {
     if (!h) return PB200_OK;
     Plan& P = h->p;
     const int dev = P.desc.device;
+    for (Plan* m : P.group)   // the other shards of a linked group are unlinked
+        if (m != &P) m->group.clear();
     cudaSetDevice(dev);
     if (P.stream) cudaStreamSynchronize(P.stream);  // nothing may still be using the buffers that go back to the pool
     for (int i = 0; i < 3; ++i) pool_free(dev, P.buf[i]);
@@ -2591,14 +2793,14 @@ int pb200_plan_set_interaction(pb200_plan* h, int32_t traj0, int32_t count, cons
         const int threads = 256;
         const long long blocks = std::min<long long>((P.D + threads - 1) / threads, (long long)P.sm_count * 16);
         dint_kernel<<<(unsigned)std::max<long long>(blocks, 1), threads, sizeof(double) * N * N, P.stream>>>(
-            dst, dU, N, P.dim, P.desc.rydberg_state, P.D);
+            dst, dU, N, P.dim, P.desc.rydberg_state, P.D, P.shard_offset());
         CUDA_CHECK(cudaGetLastError());
         // bounds per |r>-count
         std::vector<double> mins(N + 1, 1e300), maxs(N + 1, -1e300);
         CUDA_CHECK(cudaMemcpyAsync(P.d_scratch, mins.data(), sizeof(double) * (N + 1), cudaMemcpyHostToDevice, P.stream));
         CUDA_CHECK(cudaMemcpyAsync(P.d_scratch + 64, maxs.data(), sizeof(double) * (N + 1), cudaMemcpyHostToDevice, P.stream));
         dint_bounds_kernel<<<(unsigned)std::max<long long>(blocks, 1), threads, 0, P.stream>>>(
-            dst, N, P.dim, P.desc.rydberg_state, P.D, P.d_scratch, P.d_scratch + 64);
+            dst, N, P.dim, P.desc.rydberg_state, P.D, P.d_scratch, P.d_scratch + 64, P.shard_offset());
         CUDA_CHECK(cudaGetLastError());
         CUDA_CHECK(cudaMemcpyAsync(mins.data(), P.d_scratch, sizeof(double) * (N + 1), cudaMemcpyDeviceToHost, P.stream));
         CUDA_CHECK(cudaMemcpyAsync(maxs.data(), P.d_scratch + 64, sizeof(double) * (N + 1), cudaMemcpyDeviceToHost, P.stream));
@@ -2787,9 +2989,12 @@ int pb200_state_set(pb200_plan* h, int32_t traj0, int32_t count, const double* p
             const double* src = broadcast ? psi : psi + (size_t)c * P.D * 2;
             CUDA_CHECK(cudaMemcpyAsync(dst, src, sizeof(c2) * (size_t)P.D, cudaMemcpyHostToDevice, P.stream));
         } else {
-            if (basis_index < 0 || basis_index >= P.D) fail(PB200_ERR_INVALID, "basis_index out of range");
+            // a shard takes the global index: the shard that owns it sets it, the others zero their slice
+            if (basis_index < 0 || basis_index >= (P.D << P.shard_bits)) fail(PB200_ERR_INVALID, "basis_index out of range");
+            long long local = basis_index - P.shard_offset();
+            if (local >= P.D) local = -1;
             const long long blocks = std::min<long long>((P.D + 255) / 256, (long long)P.sm_count * 16);
-            set_basis_kernel<<<(unsigned)blocks, 256, 0, P.stream>>>(dst, P.D, basis_index);
+            set_basis_kernel<<<(unsigned)blocks, 256, 0, P.stream>>>(dst, P.D, local);
             CUDA_CHECK(cudaGetLastError());
         }
     }
@@ -2857,7 +3062,7 @@ int pb200_state_occupation(pb200_plan* h, int32_t traj0, int32_t count, int32_t 
     const long long blocks = std::min<long long>((P.D + 255) / 256, (long long)P.sm_count * 4);
     dim3 grid((unsigned)std::max<long long>(blocks, 1), (unsigned)count);
     occupation_kernel<<<grid, 256, sizeof(double) * P.n, P.stream>>>(P.buf[P.cur] + (size_t)traj0 * P.D, d_occ, P.D, P.n,
-                                                                       P.dim, digit);
+                                                                       P.dim, digit, P.shard_offset());
     cudaError_t e = cudaGetLastError();
     if (e == cudaSuccess) e = cudaMemcpyAsync(occ, d_occ, sizeof(double) * (size_t)count * P.n, cudaMemcpyDeviceToHost, P.stream);
     if (e == cudaSuccess) e = cudaStreamSynchronize(P.stream);
@@ -2880,7 +3085,8 @@ int pb200_state_correlation(pb200_plan* h, int32_t traj0, int32_t count, int32_t
     CUDA_CHECK(cudaMemsetAsync(d_c, 0, sizeof(double) * count * nn, P.stream));
     const long long blocks = std::min<long long>((P.D + 2047) / 2048, (long long)P.sm_count * 4);
     dim3 grid((unsigned)std::max<long long>(blocks, 1), (unsigned)count);
-    correlation_kernel<<<grid, 256, 0, P.stream>>>(P.buf[P.cur] + (size_t)traj0 * P.D, d_c, P.D, P.n, P.dim, digit);
+    correlation_kernel<<<grid, 256, 0, P.stream>>>(P.buf[P.cur] + (size_t)traj0 * P.D, d_c, P.D, P.n, P.dim, digit,
+                                                   P.shard_offset());
     cudaError_t e = cudaGetLastError();
     if (e == cudaSuccess) e = cudaMemcpyAsync(corr, d_c, sizeof(double) * count * nn, cudaMemcpyDeviceToHost, P.stream);
     if (e == cudaSuccess) e = cudaStreamSynchronize(P.stream);
@@ -2896,6 +3102,7 @@ int pb200_state_energy(pb200_plan* h, double t_us, double* energy, double* h2) {
     PB200_TRY
     if (!h || !energy || !h2) fail(PB200_ERR_INVALID, "null argument");
     Plan& P = h->p;
+    refuse_shard(P, "pb200_state_energy", "pb200_shards_energy");
     for (int tr = 0; tr < P.B; ++tr)
         for (int q = 0; q < P.n_drives; ++q)
             if (!P.tabs_set[tr][q]) fail(PB200_ERR_STATE, "drive %d of trajectory %d not set", q, tr);
@@ -2949,9 +3156,11 @@ int pb200_state_sample(pb200_plan* h, int32_t traj, int32_t one_digit, const dou
     Plan& P = h->p;
     if (traj < 0 || traj >= P.B) fail(PB200_ERR_INVALID, "trajectory out of range");
     if (one_digit < 0 || one_digit >= P.dim) fail(PB200_ERR_INVALID, "one_digit out of range");
-    if (P.n > 30) fail(PB200_ERR_UNSUPPORTED, "bitstring sampling: at most 30 qudits (32-bit item count of the prefix scan)");
+    // a shard samples its own slice: M = its 2^L bitstrings, out[i] = the low L bits of the global bitstring
+    const int nbits = P.n - P.shard_bits;
+    if (nbits > 30) fail(PB200_ERR_UNSUPPORTED, "bitstring sampling: at most 30 qudits (32-bit item count of the prefix scan)");
     CUDA_CHECK(cudaSetDevice(P.desc.device));
-    const long long M = 1LL << P.n;
+    const long long M = 1LL << nbits;
     double *d_w = nullptr, *d_u = nullptr; long long* d_idx = nullptr; void* d_tmp = nullptr;
     size_t tmp_bytes = 0;
     cudaError_t e = cudaSuccess;
@@ -2964,7 +3173,7 @@ int pb200_state_sample(pb200_plan* h, int32_t traj, int32_t one_digit, const dou
         CUDA_CHECK(cudaMemcpyAsync(d_u, uniforms, sizeof(double) * (size_t)n_shots, cudaMemcpyHostToDevice, P.stream));
         const long long blocks = std::min<long long>((P.D + 255) / 256, (long long)P.sm_count * 8);
         bitstring_weights_kernel<<<(unsigned)std::max<long long>(blocks, 1), 256, 0, P.stream>>>(
-            P.buf[P.cur] + (size_t)traj * P.D, d_w, P.D, P.n, P.dim, one_digit);
+            P.buf[P.cur] + (size_t)traj * P.D, d_w, P.D, P.n, P.dim, one_digit, P.shard_offset());
         CUDA_CHECK(cudaGetLastError());
         CUDA_CHECK(cub::DeviceScan::InclusiveSum(nullptr, tmp_bytes, d_w, d_w, (int)M, P.stream));
         d_tmp = (decltype(d_tmp))pool_alloc(P.desc.device, tmp_bytes);
@@ -2987,6 +3196,7 @@ int pb200_state_copy(pb200_plan* dst, int32_t dst_traj, pb200_plan* src, int32_t
     if (!dst || !src) fail(PB200_ERR_INVALID, "null argument");
     Plan& A = dst->p;
     Plan& S = src->p;
+    if (A.shard_bits || S.shard_bits) fail(PB200_ERR_UNSUPPORTED, "pb200_state_copy: shards hold a slice of a state, not a state");
     if (!S.state_set) fail(PB200_ERR_STATE, "pb200_state_copy: the source plan has no state");
     if (A.D != S.D || A.dim != S.dim) fail(PB200_ERR_INVALID, "pb200_state_copy: different Hilbert spaces");
     if (A.desc.device != S.desc.device) fail(PB200_ERR_UNSUPPORTED, "pb200_state_copy: plans on different devices");
@@ -3012,6 +3222,7 @@ int pb200_propagate(pb200_plan* h, double t_start, double t_stop, const pb200_ru
     PB200_TRY
     NvtxRange nvtx_range("pb200_propagate");
     if (!h) fail(PB200_ERR_INVALID, "null plan");
+    refuse_shard(h->p, "pb200_propagate", "pb200_shards_propagate");
     CUDA_CHECK(cudaSetDevice(h->p.desc.device));
     propagate(h->p, t_start, t_stop, opts, stats);
     PB200_CATCH
@@ -3022,6 +3233,7 @@ int pb200_apply_h(pb200_plan* h, int32_t traj, double t_us, const double* in, do
     NvtxRange nvtx_range("pb200_apply_h");
     if (!h || !in || !out) fail(PB200_ERR_INVALID, "null argument");
     Plan& P = h->p;
+    refuse_shard(P, "pb200_apply_h", "pb200_shards_apply_h");
     if (traj < 0 || traj >= P.B) fail(PB200_ERR_INVALID, "trajectory out of range");
     for (int tr = 0; tr < P.B; ++tr)
         for (int q = 0; q < P.n_drives; ++q)
@@ -3057,6 +3269,7 @@ int pb200_bench_apply(pb200_plan* h, double t_us, int32_t reps, double* ms_out, 
     PB200_TRY
     if (!h || !ms_out || reps < 1) fail(PB200_ERR_INVALID, "bad argument");
     Plan& P = h->p;
+    refuse_shard(P, "pb200_bench_apply", "pb200_shards_apply_h");
     if (!P.state_set) fail(PB200_ERR_STATE, "no state set");
     CUDA_CHECK(cudaSetDevice(P.desc.device));
     c2* in = P.buf[P.cur];
@@ -3084,6 +3297,198 @@ int pb200_bench_apply(pb200_plan* h, double t_us, int32_t reps, double* ms_out, 
     CUDA_CHECK(cudaEventElapsedTime(&ms, e0, e1));
     *ms_out = ms;
     if (launches_out) *launches_out = launches;
+    PB200_CATCH
+}
+
+int pb200_shards_link(pb200_plan** plans, int32_t count) {
+    PB200_TRY
+    NvtxRange nvtx_range("pb200_shards_link");
+    if (!plans) fail(PB200_ERR_INVALID, "null argument");
+    if (count != 2 && count != 4 && count != 8) fail(PB200_ERR_INVALID, "pb200_shards_link: count = %d, must be 2, 4 or 8", count);
+    std::vector<Plan*> G(count);
+    for (int i = 0; i < count; ++i) {
+        if (!plans[i]) fail(PB200_ERR_INVALID, "pb200_shards_link: null plan");
+        G[i] = &plans[i]->p;
+    }
+    for (int i = 0; i < count; ++i) {
+        Plan& P = *G[i];
+        if ((1 << P.shard_bits) != count) fail(PB200_ERR_INVALID, "pb200_shards_link: plans[%d] is not one of %d shards", i, count);
+        if (P.shard != i) fail(PB200_ERR_INVALID, "pb200_shards_link: plans[%d] is shard %d (plans[i] must be shard i)", i, P.shard);
+        if (P.n != G[0]->n || P.times != G[0]->times || P.desc.interp_order != G[0]->desc.interp_order)
+            fail(PB200_ERR_INVALID, "pb200_shards_link: the shards differ in N, sampling times or interpolation order");
+        if (P.has_interaction != G[0]->has_interaction || (P.has_interaction && !P.dint_shared))
+            fail(PB200_ERR_INVALID, "pb200_shards_link: every shard needs the same (shared) interaction");
+        if (!P.tabs_set[0][0]) fail(PB200_ERR_STATE, "pb200_shards_link: the drive of shard %d is not set", i);
+        if (!taylor_prepare(P)) fail(PB200_ERR_UNSUPPORTED, "pb200_shards_link: no Taylor propagator for this sequence: %s", g_taylor_why);
+        if (!P.tay.uniform)
+            fail(PB200_ERR_UNSUPPORTED, "pb200_shards_link: shards need one drive coefficient for every qubit (per-qubit factors are not sharded)");
+    }
+    // peer access between distinct devices of neighbouring shards (a flip of one shard bit)
+    for (int i = 0; i < count; ++i)
+        for (int q = 0; (1 << q) < count; ++q) {
+            const int di = G[i]->desc.device, dj = G[i ^ (1 << q)]->desc.device;
+            if (di == dj) continue;
+            int can = 0;
+            CUDA_CHECK(cudaDeviceCanAccessPeer(&can, di, dj));
+            if (!can) fail(PB200_ERR_UNSUPPORTED, "pb200_shards_link: device %d cannot access the memory of device %d (no peer access)", di, dj);
+            CUDA_CHECK(cudaSetDevice(di));
+            const cudaError_t e = cudaDeviceEnablePeerAccess(dj, 0);
+            if (e == cudaErrorPeerAccessAlreadyEnabled) cudaGetLastError();
+            else CUDA_CHECK(e);
+        }
+    // spectral bounds of the whole interaction diagonal: min / max over the shards' slices, so that the host schedule
+    // (taylor_bounds) is the one of the unsharded plan
+    if (G[0]->has_interaction) {
+        std::vector<double> mins = G[0]->dmin_cnt, maxs = G[0]->dmax_cnt;
+        double mn = G[0]->dmin_traj[0], mx = G[0]->dmax_traj[0];
+        for (int i = 1; i < count; ++i) {
+            for (size_t c = 0; c < mins.size(); ++c) {
+                mins[c] = std::min(mins[c], G[i]->dmin_cnt[c]);
+                maxs[c] = std::max(maxs[c], G[i]->dmax_cnt[c]);
+            }
+            mn = std::min(mn, G[i]->dmin_traj[0]); mx = std::max(mx, G[i]->dmax_traj[0]);
+        }
+        for (Plan* P : G) { P->dmin_cnt = mins; P->dmax_cnt = maxs; P->dmin_traj[0] = mn; P->dmax_traj[0] = mx; }
+    }
+    for (Plan* P : G) { P->tay.w_knot.clear(); P->group = G; }
+    PB200_CATCH
+}
+
+int pb200_shards_propagate(pb200_plan** plans, int32_t count, double t_start, double t_stop, const pb200_run_opts* o,
+                           pb200_run_stats* stats) {
+    PB200_TRY
+    NvtxRange nvtx_range("pb200_shards_propagate");
+    const std::vector<Plan*> G = shard_group(plans, count, "pb200_shards_propagate");
+    if (o && ((o->integrator != 0 && o->integrator != 3) || o->max_step_samples > 0 || o->tol < 0.0))
+        fail(PB200_ERR_UNSUPPORTED, "pb200_shards_propagate: shards run the Taylor propagator only (integrator 0 or 3, "
+                                    "max_step_samples = 0, tol >= 0)");
+    for (int r = 0; r < count; ++r)
+        if (!G[r]->state_set) fail(PB200_ERR_STATE, "pb200_shards_propagate: no state set on shard %d", r);
+    Plan& P0 = *G[0];
+    const double tlo = P0.times.front(), thi = P0.times.back(), eps = 1e-12;
+    if (t_start < tlo - eps || t_stop > thi + eps || t_stop < t_start)
+        fail(PB200_ERR_INVALID, "pb200_shards_propagate: [%g, %g] outside sampling times [%g, %g]", t_start, t_stop, tlo, thi);
+    t_start = std::max(t_start, tlo); t_stop = std::min(t_stop, thi);
+    const PassGeom geo = shard_geometry(P0);
+    // host half: the whole call, before any launch
+    TaylorScheduler S(P0, t_start, t_stop, o);
+    std::vector<TaylorStep> steps;
+    for (TaylorStep s; S.next(s);) steps.push_back(s);
+    int need = 0;
+    for (const TaylorStep& s : steps) need = std::max(need, s.ring());
+    // every shard's ring for the largest step, before the first launch: a ring that does not fit leaves the state as it was
+    for (Plan* P : G) {
+        CUDA_CHECK(cudaSetDevice(P->desc.device));
+        try {
+            taylor_grow_ring(*P, need);
+        } catch (const Error& e) {
+            fail(PB200_ERR_CUDA, "pb200_shards_propagate: this call needs the state and %d more state-sized buffers per shard, "
+                                 "%lld bytes each (%d amplitudes x 16 B) besides the 8 B/amplitude interaction diagonal: %s",
+                 need, (long long)(16 * P->D), (int)P->D, e.what());
+        }
+    }
+    ShardEvents order_ev(G, cudaEventDisableTiming), t0(G, cudaEventDefault), t1(G, cudaEventDefault);
+    for (int r = 0; r < count; ++r) {
+        CUDA_CHECK(cudaSetDevice(G[r]->desc.device));
+        CUDA_CHECK(cudaEventRecord(t0.ev[r], G[r]->stream));
+    }
+    // launching half.  Order k on shard r reads chi_k of its peers: it waits for the previous launch (order k - 1, or the
+    // last order of the previous step) of every peer, and every shard's waits for an order are enqueued before any
+    // shard records that order's event.  A slot a peer may still be gathering from is never overwritten: n_chi >= 2,
+    // and every order waits for the one before it.  The previous call ended with every stream synchronised.
+    const int sb = P0.shard_bits;
+    long long launches = 0;
+    bool first = true;
+    std::vector<TaylorRing> R(count);
+    for (const TaylorStep& s : steps) {
+        for (int r = 0; r < count; ++r) R[r] = taylor_ring(*G[r], s);
+        for (int k = 0; k < s.K; ++k) {
+            for (int r = 0; r < count; ++r) {
+                Plan& P = *G[r];
+                CUDA_CHECK(cudaSetDevice(P.desc.device));
+                TaylorArgs a = taylor_args(P, geo, s, R[r], k);
+                a.shard_bits = sb; a.shard = r;
+                for (int q = 0; q < sb; ++q) {
+                    const int peer = r ^ (1 << q);
+                    a.peer[q] = R[peer].chi[k % s.n_chi];
+                    if (!first) CUDA_CHECK(cudaStreamWaitEvent(P.stream, order_ev.ev[peer], 0));
+                }
+                launch_taylor_shard(P, a);
+                ++launches;
+            }
+            for (int r = 0; r < count; ++r) {
+                CUDA_CHECK(cudaSetDevice(G[r]->desc.device));
+                CUDA_CHECK(cudaEventRecord(order_ev.ev[r], G[r]->stream));
+            }
+            first = false;
+        }
+        CUDA_CHECK(cudaGetLastError());
+        // the accumulator becomes the current state buffer
+        for (int r = 0; r < count; ++r) std::swap(G[r]->buf[G[r]->cur], *R[r].acc_slot);
+    }
+    float ms_max = 0.f;
+    for (int r = 0; r < count; ++r) {
+        CUDA_CHECK(cudaSetDevice(G[r]->desc.device));
+        CUDA_CHECK(cudaEventRecord(t1.ev[r], G[r]->stream));
+    }
+    for (int r = 0; r < count; ++r) {
+        CUDA_CHECK(cudaEventSynchronize(t1.ev[r]));
+        float ms = 0.f;
+        CUDA_CHECK(cudaEventElapsedTime(&ms, t0.ev[r], t1.ev[r]));
+        ms_max = std::max(ms_max, ms);
+    }
+    if (stats) *stats = S.finish(ms_max, launches);
+    PB200_CATCH
+}
+
+int pb200_shards_apply_h(pb200_plan** plans, int32_t count, double t_us, const double* in, double* out) {
+    PB200_TRY
+    NvtxRange nvtx_range("pb200_shards_apply_h");
+    if (!in || !out) fail(PB200_ERR_INVALID, "null argument");
+    const std::vector<Plan*> G = shard_group(plans, count, "pb200_shards_apply_h");
+    std::vector<c2*> bin(count), bout(count);
+    for (int r = 0; r < count; ++r) {
+        Plan& P = *G[r];
+        bin[r] = P.buf[(P.cur + 1) % 3]; bout[r] = P.buf[(P.cur + 2) % 3];
+        CUDA_CHECK(cudaSetDevice(P.desc.device));
+        CUDA_CHECK(cudaMemcpyAsync(bin[r], in + (size_t)2 * P.D * r, sizeof(c2) * (size_t)P.D, cudaMemcpyHostToDevice, P.stream));
+    }
+    shards_apply_h(G, t_us, bin, bout);
+    for (int r = 0; r < count; ++r) {
+        Plan& P = *G[r];
+        CUDA_CHECK(cudaSetDevice(P.desc.device));
+        CUDA_CHECK(cudaMemcpyAsync(out + (size_t)2 * P.D * r, bout[r], sizeof(c2) * (size_t)P.D, cudaMemcpyDeviceToHost, P.stream));
+    }
+    shards_sync(G);
+    PB200_CATCH
+}
+
+int pb200_shards_energy(pb200_plan** plans, int32_t count, double t_us, double* energy, double* h2) {
+    PB200_TRY
+    NvtxRange nvtx_range("pb200_shards_energy");
+    if (!energy || !h2) fail(PB200_ERR_INVALID, "null argument");
+    const std::vector<Plan*> G = shard_group(plans, count, "pb200_shards_energy");
+    std::vector<c2*> psi(count), hpsi(count);
+    for (int r = 0; r < count; ++r) {
+        if (!G[r]->state_set) fail(PB200_ERR_STATE, "pb200_shards_energy: no state set on shard %d", r);
+        psi[r] = G[r]->buf[G[r]->cur]; hpsi[r] = G[r]->buf[(G[r]->cur + 2) % 3];
+    }
+    shards_apply_h(G, t_us, psi, hpsi);
+    // Re<psi, H psi> and <H psi, H psi>, summed over the shards
+    double e = 0.0, e2 = 0.0;
+    for (int r = 0; r < count; ++r) {
+        Plan& P = *G[r];
+        CUDA_CHECK(cudaSetDevice(P.desc.device));
+        CUDA_CHECK(cudaMemsetAsync(P.d_scratch, 0, sizeof(double) * 2, P.stream));
+        const long long blocks = std::min<long long>((P.D + 255) / 256, (long long)P.sm_count * 8);
+        dot2_kernel<<<dim3((unsigned)std::max<long long>(blocks, 1), 1), 256, 0, P.stream>>>(psi[r], hpsi[r], P.D, P.d_scratch);
+        CUDA_CHECK(cudaGetLastError());
+        double acc[2];
+        CUDA_CHECK(cudaMemcpyAsync(acc, P.d_scratch, sizeof(double) * 2, cudaMemcpyDeviceToHost, P.stream));
+        CUDA_CHECK(cudaStreamSynchronize(P.stream));
+        e += acc[0]; e2 += acc[1];
+    }
+    energy[0] = e; h2[0] = e2;
     PB200_CATCH
 }
 

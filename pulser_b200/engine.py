@@ -67,13 +67,19 @@ def _with_common_drives(specs: list[HamiltonianSpec]) -> list[HamiltonianSpec]:
 
 
 class DevicePlan:
-    """A batch of trajectories of one sequence resident on one GPU."""
+    """A batch of trajectories of one sequence resident on one GPU.
+
+    ``shard=(bits, index)``: the plan holds shard ``index`` of ``2**bits`` of one state
+    (``pb200_plan_create_shard``): the ``D = 2**(N - bits)`` amplitudes whose top ``bits`` qubits
+    equal ``index``.  Shards are driven together by ``pulser_b200.sharded.ShardedPlan``.
+    """
 
     def __init__(
         self,
         specs: HamiltonianSpec | Sequence[HamiltonianSpec],
         interp_order: int = 3,
         device: int = 0,
+        shard: tuple[int, int] | None = None,
     ) -> None:
         if isinstance(specs, HamiltonianSpec):
             specs = [specs]
@@ -101,7 +107,8 @@ class DevicePlan:
         self.n_traj = len(specs)
         self.n = s0.n_qudits
         self.dim = s0.dim
-        self.D = s0.hilbert_dim
+        self.shard = None if shard is None else (int(shard[0]), int(shard[1]))
+        self.D = s0.hilbert_dim if shard is None else s0.hilbert_dim >> self.shard[0]
         self.interp_order = interp_order
         self._handle = C.c_void_p()
         times = np.ascontiguousarray(s0.sampling_times, dtype=np.float64)
@@ -126,7 +133,10 @@ class DevicePlan:
             uni = all(s.drives[q].uniform for s in specs)
             desc.drives[q].uniform = int(uni)
             self._uniform.append(uni)
-        check(lib.pb200_plan_create(C.byref(self._handle), C.byref(desc)))
+        if self.shard is None:
+            check(lib.pb200_plan_create(C.byref(self._handle), C.byref(desc)))
+        else:
+            check(lib.pb200_plan_create_shard(C.byref(self._handle), C.byref(desc), *self.shard))
         try:
             self._upload(any_inter)
         except Exception:
