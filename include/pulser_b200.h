@@ -232,6 +232,27 @@ int pb200_state_energy(pb200_plan* plan, double t_us, double* energy, double* h2
 int pb200_state_overlap(pb200_plan* plan, int32_t traj0, int32_t count,
                         const double* phi, double* out);
 
+/* An operator as a sum of monomial terms (Expectation observable,
+ * default_observables.py:240-288, on an operator of Pulser's operator
+ * representation, qutip_op.py:148-218).  Term t is
+ *     coeff[t] (x)_{e in [site_start[t], site_start[t+1])} M_e,
+ *     M_e[a, (a + shift[e]) mod d] = weight[e][a]  (zero elsewhere)
+ * on qudit site[e]; a qudit no entry names carries the identity.  The sites of
+ * one term are distinct. */
+typedef struct pb200_op_terms {
+    int32_t n_terms;
+    const double*  coeff;       /* complex128 [n_terms] */
+    const int32_t* site_start;  /* [n_terms + 1] into the per-site arrays */
+    const int32_t* site;        /* qudit index k (0 = most significant digit) */
+    const int32_t* shift;       /* m in [0, d) */
+    const double*  weight;      /* complex128 [n_site_entries][d]: w_k[a] */
+} pb200_op_terms;
+/* out[c] = <psi_{traj0+c}| op |psi_{traj0+c}> as (re, im), not normalised,
+ * matrix-free on the device.  A shard plan is refused (pb200_shards_expect),
+ * as is a plan that carries a density matrix (PB200_ERR_UNSUPPORTED). */
+int pb200_state_expect(pb200_plan* plan, int32_t traj0, int32_t count,
+                       const pb200_op_terms* op, double* out);
+
 /* Bitstring sampling on the device (QutipResult._weights + multinomial,
  * qutip_result.py:101-158, pulser/math/multinomial.py:17-36): weights over the
  * 2^N bitstrings (bit k = [digit_k == one_digit]), normalised, cumulated, and
@@ -304,6 +325,12 @@ int pb200_shards_apply_h(pb200_plan** plans, int32_t count, double t_us,
 /* <psi|H(t)|psi> and <psi|H(t)^2|psi> of the sharded state (energy[1], h2[1]). */
 int pb200_shards_energy(pb200_plan** plans, int32_t count, double t_us,
                         double* energy, double* h2);
+/* <psi| op |psi> of the sharded state, out[2] = (re, im), not normalised.  A
+ * term that changes shard bits x reads shard r ^ x from shard r: peer access
+ * between the devices of every such pair is enabled here when missing
+ * (PB200_ERR_UNSUPPORTED where there is none). */
+int pb200_shards_expect(pb200_plan** plans, int32_t count,
+                        const pb200_op_terms* op, double* out);
 
 /* ---- host-side math, usable without a device (exercised by the CPU tests) -- */
 /* Interpolant of complex samples y[n] (re,im) over x[n] at nq query points:

@@ -69,6 +69,19 @@ class RunStats(C.Structure):
     ]
 
 
+class OpTermsDesc(C.Structure):
+    """``pb200_op_terms``: an operator as monomial terms (packed by ``pulser_b200.opterms.OpTerms.c_desc``)."""
+
+    _fields_ = [
+        ("n_terms", C.c_int32),
+        ("coeff", C.POINTER(C.c_double)),
+        ("site_start", C.POINTER(C.c_int32)),
+        ("site", C.POINTER(C.c_int32)),
+        ("shift", C.POINTER(C.c_int32)),
+        ("weight", C.POINTER(C.c_double)),
+    ]
+
+
 class LibraryMissing(ImportError):
     pass
 
@@ -107,6 +120,7 @@ def _load() -> C.CDLL:
         "pb200_state_correlation": (C.c_int, [vp, C.c_int32, C.c_int32, C.c_int32, dp]),
         "pb200_state_energy": (C.c_int, [vp, C.c_double, dp, dp]),
         "pb200_state_overlap": (C.c_int, [vp, C.c_int32, C.c_int32, dp, dp]),
+        "pb200_state_expect": (C.c_int, [vp, C.c_int32, C.c_int32, C.POINTER(OpTermsDesc), dp]),
         "pb200_state_sample": (
             C.c_int, [vp, C.c_int32, C.c_int32, dp, C.c_int32, C.POINTER(C.c_int64)]),
         "pb200_state_copy": (C.c_int, [vp, C.c_int32, vp, C.c_int32]),
@@ -124,6 +138,7 @@ def _load() -> C.CDLL:
             C.c_int, [C.POINTER(vp), C.c_int32, C.c_double, C.c_double, C.POINTER(RunOpts), C.POINTER(RunStats)]),
         "pb200_shards_apply_h": (C.c_int, [C.POINTER(vp), C.c_int32, C.c_double, dp, dp]),
         "pb200_shards_energy": (C.c_int, [C.POINTER(vp), C.c_int32, C.c_double, dp, dp]),
+        "pb200_shards_expect": (C.c_int, [C.POINTER(vp), C.c_int32, C.POINTER(OpTermsDesc), dp]),
         "pb200_host_interpolate": (
             C.c_int, [dp, dp, C.c_int32, C.c_int32, dp, C.c_int32, dp]),
         "pb200_host_moments": (
@@ -150,10 +165,11 @@ EXPORTED_SYMBOLS = [
     "pb200_plan_set_interaction", "pb200_plan_set_xy", "pb200_plan_set_slm_mask", "pb200_plan_set_drive", "pb200_plan_set_dissipator", "pb200_plan_set_collapse",
     "pb200_plan_jump_counts", "pb200_state_set",
     "pb200_state_get", "pb200_state_probabilities", "pb200_state_norm2",
-    "pb200_state_occupation", "pb200_state_correlation", "pb200_state_energy", "pb200_state_overlap", "pb200_state_sample", "pb200_state_copy", "pb200_state_device_ptr", "pb200_propagate", "pb200_apply_h",
+    "pb200_state_occupation", "pb200_state_correlation", "pb200_state_energy", "pb200_state_overlap", "pb200_state_expect", "pb200_state_sample", "pb200_state_copy", "pb200_state_device_ptr", "pb200_propagate", "pb200_apply_h",
     "pb200_coefficients_at", "pb200_bench_apply", "pb200_host_interpolate",
     "pb200_host_moments", "pb200_host_chebyshev", "pb200_host_taylor_fit", "pb200_host_taylor_order", "pb200_host_taylor_separable",
     "pb200_plan_create_shard", "pb200_shards_link", "pb200_shards_propagate", "pb200_shards_apply_h", "pb200_shards_energy",
+    "pb200_shards_expect",
 ]
 
 lib = _load()

@@ -33,6 +33,7 @@ from pulser.backend.results import Results  # noqa: E402
 from pulser.backend.state import State  # noqa: E402
 
 from .emulator import B200Emulator, Solver, _has_stochastic_noise  # noqa: E402
+from .opterms import OpTerms  # noqa: E402
 from .results import multinomial  # noqa: E402
 
 
@@ -161,6 +162,10 @@ class _DeviceResident:
     def _projector_expect(self, coeff: complex, letter: str | None, targets: frozenset) -> complex | None:
         raise NotImplementedError
 
+    def _terms_expect(self, terms: OpTerms) -> complex | None:
+        """``<O>`` of an operator given as monomial terms, or ``None`` when this state cannot reduce it on the device."""
+        return None
+
 
 class DeviceStateView(_DeviceResident, B200State):
     """The current state of one trajectory of a ``DevicePlan``, left on the GPU.
@@ -169,7 +174,8 @@ class DeviceStateView(_DeviceResident, B200State):
     evaluation times: ``Occupation`` / ``CorrelationMatrix`` (number-operator
     expectations), ``Energy*`` (with ``DeviceHamiltonian``), ``Fidelity`` and
     ``BitStrings`` reduce on the device (``pb200_state_occupation / _correlation /
-    _energy / _overlap / _sample``); anything else falls back to a host copy
+    _energy / _overlap / _sample``), and so does ``Expectation`` of an operator with
+    monomial terms (``pb200_state_expect``); anything else falls back to a host copy
     (``to_array``), fetched once.  Replaces the replay of stored ``QutipState``s of
     ``qutip_backend.py:254-280``, which cannot hold one state per step at N >= 20.
     """
@@ -210,6 +216,12 @@ class DeviceStateView(_DeviceResident, B200State):
             return None
         idx = sorted(targets)
         return complex(coeff) * float(self._correlations(letter)[idx[0], idx[-1]])
+
+    def _terms_expect(self, terms: OpTerms) -> complex | None:
+        expect_terms = getattr(self._plan, "expect_terms", None)
+        if expect_terms is None:
+            return None
+        return complex(expect_terms(terms, self._traj, 1)[0]) / self._norm2
 
     def _energy_moments(self, plan: Any, t_us: float) -> tuple[float, float] | None:
         """``<H>``, ``<H^2>`` of this state under the Hamiltonian of ``plan``.  ``plan`` is either the plan that
@@ -285,16 +297,20 @@ class _HPsiView(_DeviceResident, B200State):
 class B200Operator(Operator[complex, complex, B200State]):
     """An operator as a scipy sparse matrix (``QutipOperator`` mirror)."""
 
-    def __init__(self, operator: Any, eigenstates: Sequence[str], *, pattern: tuple | None = None):
+    def __init__(self, operator: Any, eigenstates: Sequence[str], *, pattern: tuple | None = None,
+                 terms: OpTerms | None = None):
         """``operator``: a matrix, or a zero-argument callable building it on first use.
 
         ``pattern = (coeff, state, frozenset(qudits))`` marks ``coeff * prod_k |state><state|_k`` (identity for an
         empty set): its expectation on a device-resident state is a reduction on the GPU, the matrix is never built.
+        ``terms``: the same operator as monomial terms (``pulser_b200.opterms``); its expectation on a device-resident
+        state is computed matrix-free on the GPU.
         """
         super().__init__()
         B200State._validate_eigenstates(eigenstates)
         self._eigenstates = eigenstates
         self._pattern = pattern
+        self._terms = terms
         if callable(operator):
             self._builder, self._matrix = operator, None
         else:
@@ -354,6 +370,8 @@ class B200Operator(Operator[complex, complex, B200State]):
 
     @property
     def _isherm(self) -> bool:
+        if not hasattr(self, "_herm_cache") and self._terms is not None and self._terms.adjoint_matches():
+            self._herm_cache = True
         if not hasattr(self, "_herm_cache"):
             m = self._operator
             self._herm_cache = bool(abs(m - m.getH()).max() < 1e-12) if m.nnz else True
@@ -366,6 +384,10 @@ class B200Operator(Operator[complex, complex, B200State]):
             val = state._projector_expect(*self._pattern)
             if val is not None:
                 return val.real if val.imag == 0.0 else val
+        if self._terms is not None and isinstance(state, _DeviceResident) and state.is_ket:
+            val = state._terms_expect(self._terms)
+            if val is not None:
+                return val.real if self._isherm else val
         if state.is_ket:
             val = complex(np.vdot(state._state, self._matvec(state._state)))
         else:
@@ -374,13 +396,20 @@ class B200Operator(Operator[complex, complex, B200State]):
 
     def __add__(self, other: "B200Operator", /) -> "B200Operator":
         self._validate_other(other, B200Operator, "__add__")
-        return B200Operator(self._operator + other._operator, eigenstates=self.eigenstates)
+        a, b = self._terms, getattr(other, "_terms", None)
+        # operators on different registers have no compiled sum: the matrices report the mismatch, as they always did
+        terms = a + b if a is not None and b is not None and a.compatible(b) else None
+        if terms is None:
+            return B200Operator(self._operator + other._operator, eigenstates=self.eigenstates)
+        return B200Operator(lambda: self._operator + other._operator, eigenstates=self.eigenstates, terms=terms)
 
     def __rmul__(self, scalar: complex) -> "B200Operator":
         pat = self._pattern
         if pat is not None:
             pat = (complex(scalar) * pat[0], pat[1], pat[2])
-        return B200Operator(lambda: complex(scalar) * self._operator, eigenstates=self.eigenstates, pattern=pat)
+        terms = None if self._terms is None else self._terms.scaled(scalar)
+        return B200Operator(lambda: complex(scalar) * self._operator, eigenstates=self.eigenstates, pattern=pat,
+                            terms=terms)
 
     def __matmul__(self, other: "B200Operator") -> "B200Operator":
         self._validate_other(other, B200Operator, "__matmul__")
@@ -389,7 +418,10 @@ class B200Operator(Operator[complex, complex, B200State]):
         if a is not None and b is not None and (a[1] == b[1] or not a[2] or not b[2]):
             # projectors on one eigenstate commute and are idempotent: the product is the projector on the union
             pat = (a[0] * b[0], a[1] if a[2] else b[1], a[2] | b[2])
-        return B200Operator(lambda: self._operator @ other._operator, eigenstates=self.eigenstates, pattern=pat)
+        a, b = self._terms, getattr(other, "_terms", None)
+        terms = a @ b if a is not None and b is not None and a.compatible(b) else None
+        return B200Operator(lambda: self._operator @ other._operator, eigenstates=self.eigenstates, pattern=pat,
+                            terms=terms)
 
     @classmethod
     def _from_operator_repr(cls, *, eigenstates: Sequence[str], n_qudits: int, operations: Any):
@@ -444,7 +476,8 @@ class B200Operator(Operator[complex, complex, B200State]):
                 scale *= val ** len(inds)
             if ok and len(letters) <= 1:
                 pattern = (coeff * scale, next(iter(letters)) if letters else None, frozenset(targets))
-        return B200Operator(build, eigenstates=eigenstates, pattern=pattern), reconstructed
+        terms = OpTerms.from_operations(reconstructed, eigenstates, n_qudits)
+        return B200Operator(build, eigenstates=eigenstates, pattern=pattern, terms=terms), reconstructed
 
     def __repr__(self) -> str:
         return f"B200Operator(eigenstates={self.eigenstates}, shape={self._operator.shape})"
@@ -469,6 +502,7 @@ class DeviceHamiltonian(B200Operator):
         self._plan = plan
         self._t = t_us
         self._pattern = None
+        self._terms = None
         self._builder, self._matrix = None, None  # never materialised
         self._herm_cache = True
 

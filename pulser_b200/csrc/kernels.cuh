@@ -1543,6 +1543,128 @@ __global__ void overlap_kernel(const c2* phi, const c2* psi, long long D, double
     }
 }
 
+// ---- expectation of an operator given as monomial terms (Expectation observable) --------------------------------
+// A term is c (x)_{k in S} M_k with M_k[a, (a + m_k) mod d] = w_k[a]:
+//     <psi|term|psi> = c sum_s conj(psi_s) prod_k w_k[s_k] psi_{s'},  s' = s with digit (s_k + m_k) mod d on S.
+// The term table is staged through shared memory in chunks (chunk i: terms [chunk_t[i], chunk_t[i+1]) and site
+// entries [chunk_s[i], chunk_s[i+1]), site offsets relative to the chunk), so any term count works.
+constexpr int kExpChunkTerms = 256, kExpChunkSites = 256;
+
+// d = 2: the host folds the site factors of a term into masks of the GLOBAL index g (shard offset + local index):
+// partner g ^ f; zero unless (g & care) == val; sign (-1)^popc(g & z); times r_j for every general site j whose bit
+// is set in g.  Terms arrive sorted by f, so one partner load serves every term of a run of equal masks.
+struct ExpD2Term {
+    c2 c;
+    unsigned long long f, care, val, z;
+    int s0, sn;  // general sites of the term in the staged chunk
+};
+struct ExpGenSite { c2 r; unsigned long long bit; };
+// where the partners live: src[shard ^ (f >> local_bits)] holds the slice of index bits above local_bits (one
+// pointer and shard 0 for a whole state; a shard group passes every shard's state, peers through peer access)
+struct ExpSrc { const c2* p[8]; int shard; int local_bits; };
+
+__device__ __forceinline__ void exp_reduce(double re, double im, double* acc) {
+    for (int o = 16; o > 0; o >>= 1) {
+        re += __shfl_xor_sync(0xffffffffu, re, o);
+        im += __shfl_xor_sync(0xffffffffu, im, o);
+    }
+    __shared__ double ws[2][8];
+    if ((threadIdx.x & 31) == 0) { ws[0][threadIdx.x >> 5] = re; ws[1][threadIdx.x >> 5] = im; }
+    __syncthreads();
+    if (threadIdx.x == 0) {
+        double s0 = 0.0, s1 = 0.0;
+        for (int i = 0; i < (int)(blockDim.x >> 5); ++i) { s0 += ws[0][i]; s1 += ws[1][i]; }
+        atomicAdd(acc + 2 * blockIdx.y, s0);
+        atomicAdd(acc + 2 * blockIdx.y + 1, s1);
+    }
+}
+
+// acc[traj] += sum_terms (blockIdx.y = trajectory; D = 2^local_bits amplitudes per trajectory; 256 threads)
+__global__ void __launch_bounds__(256) expect_terms_d2_kernel(const __grid_constant__ ExpSrc src, long long D,
+                                                              const ExpD2Term* terms, const ExpGenSite* gens,
+                                                              const int* chunk_t, const int* chunk_s, int n_chunks,
+                                                              double* acc) {
+    __shared__ ExpD2Term st[kExpChunkTerms];
+    __shared__ ExpGenSite sg[kExpChunkSites];
+    const long long traj_off = (long long)blockIdx.y * D;
+    const c2* own = src.p[src.shard] + traj_off;
+    const unsigned long long off = (unsigned long long)src.shard << src.local_bits;
+    const unsigned long long lmask = (unsigned long long)D - 1ull;
+    double re = 0.0, im = 0.0;
+    for (int ch = 0; ch < n_chunks; ++ch) {
+        const int t0 = chunk_t[ch], nt = chunk_t[ch + 1] - t0, s0 = chunk_s[ch], ns = chunk_s[ch + 1] - s0;
+        __syncthreads();  // the previous chunk is consumed
+        for (int i = threadIdx.x; i < nt; i += blockDim.x) st[i] = terms[t0 + i];
+        for (int i = threadIdx.x; i < ns; i += blockDim.x) sg[i] = gens[s0 + i];
+        __syncthreads();
+        for (long long s = blockIdx.x * (long long)blockDim.x + threadIdx.x; s < D; s += (long long)gridDim.x * blockDim.x) {
+            const c2 v = own[s];
+            const unsigned long long g = off | (unsigned long long)s;
+            unsigned long long fcur = ~0ull;
+            c2 q = {0.0, 0.0};  // conj(psi_g) psi_{g ^ f}
+            for (int t = 0; t < nt; ++t) {
+                const ExpD2Term& T = st[t];
+                if (T.f != fcur) {  // uniform across the block: the loads of a warp are coalesced
+                    fcur = T.f;
+                    c2 p = v;
+                    if (fcur) p = src.p[src.shard ^ (int)(fcur >> src.local_bits)][traj_off + (long long)((unsigned long long)s ^ (fcur & lmask))];
+                    q = {v.x * p.x + v.y * p.y, v.x * p.y - v.y * p.x};
+                }
+                if ((g & T.care) != T.val) continue;
+                c2 c = T.c;
+                for (int j = 0; j < T.sn; ++j)
+                    if (g & sg[T.s0 + j].bit) c = cmul(c, sg[T.s0 + j].r);
+                if (__popcll(g & T.z) & 1) c = {-c.x, -c.y};
+                re = fma(c.x, q.x, re); re = fma(-c.y, q.y, re);
+                im = fma(c.x, q.y, im); im = fma(c.y, q.x, im);
+            }
+        }
+    }
+    exp_reduce(re, im, acc);
+}
+
+// d = 3 / 4: digit a = (s / stride) mod d of each site, factor w[a], partner digit (a + shift) mod d
+struct ExpTerm { c2 c; int s0, sn; };
+struct ExpSite { long long stride; int shift, pad; c2 w[4]; };
+
+__global__ void __launch_bounds__(256) expect_terms_kernel(const c2* psi, long long D, int dim, const ExpTerm* terms,
+                                                           const ExpSite* sites, const int* chunk_t, const int* chunk_s,
+                                                           int n_chunks, double* acc) {
+    __shared__ ExpTerm st[kExpChunkTerms];
+    __shared__ ExpSite ss[kExpChunkSites];
+    const c2* v_traj = psi + (long long)blockIdx.y * D;
+    double re = 0.0, im = 0.0;
+    for (int ch = 0; ch < n_chunks; ++ch) {
+        const int t0 = chunk_t[ch], nt = chunk_t[ch + 1] - t0, s0 = chunk_s[ch], ns = chunk_s[ch + 1] - s0;
+        __syncthreads();
+        for (int i = threadIdx.x; i < nt; i += blockDim.x) st[i] = terms[t0 + i];
+        for (int i = threadIdx.x; i < ns; i += blockDim.x) ss[i] = sites[s0 + i];
+        __syncthreads();
+        for (long long s = blockIdx.x * (long long)blockDim.x + threadIdx.x; s < D; s += (long long)gridDim.x * blockDim.x) {
+            const c2 v = v_traj[s];
+            for (int t = 0; t < nt; ++t) {
+                const ExpTerm& T = st[t];
+                c2 c = T.c;
+                long long sp = s;
+                for (int j = 0; j < T.sn; ++j) {
+                    const ExpSite& S = ss[T.s0 + j];
+                    const int a = (int)((s / S.stride) % dim);
+                    int b = a + S.shift;
+                    if (b >= dim) b -= dim;
+                    c = cmul(c, S.w[a]);
+                    sp += (long long)(b - a) * S.stride;
+                }
+                if (c.x == 0.0 && c.y == 0.0) continue;
+                const c2 p = v_traj[sp];
+                const c2 q = {v.x * p.x + v.y * p.y, v.x * p.y - v.y * p.x};
+                re = fma(c.x, q.x, re); re = fma(-c.y, q.y, re);
+                im = fma(c.x, q.y, im); im = fma(c.y, q.x, im);
+            }
+        }
+    }
+    exp_reduce(re, im, acc);
+}
+
 // indices[i] = first j with cum[j] >= u[i] * total  (np.searchsorted(cumsum(w / sum w), rnd), side="left")
 __global__ void search_sorted_kernel(const double* cum, long long M, const double* u, long long* idx, int n_shots) {
     const int i = blockIdx.x * blockDim.x + threadIdx.x;

@@ -2584,6 +2584,174 @@ static void shards_apply_h(const std::vector<Plan*>& G, double t, const std::vec
     shards_sync(G);
 }
 
+// ---- expectation of an operator given as monomial terms (pb200_state_expect / pb200_shards_expect) -----------------
+// argument checks of an operator on n qudits of dimension dim; no device call
+static void check_op_terms(const pb200_op_terms* op, int n, int dim, const char* who) {
+    if (!op) fail(PB200_ERR_INVALID, "%s: null operator", who);
+    if (op->n_terms < 0) fail(PB200_ERR_INVALID, "%s: n_terms = %d", who, op->n_terms);
+    if (op->n_terms == 0) return;
+    if (!op->coeff || !op->site_start) fail(PB200_ERR_INVALID, "%s: null coeff or site_start", who);
+    if (op->site_start[0] != 0) fail(PB200_ERR_INVALID, "%s: site_start[0] = %d, must be 0", who, op->site_start[0]);
+    for (int t = 0; t < op->n_terms; ++t)
+        if (op->site_start[t + 1] < op->site_start[t]) fail(PB200_ERR_INVALID, "%s: site_start decreases at term %d", who, t);
+    if (op->site_start[op->n_terms] > 0 && (!op->site || !op->shift || !op->weight))
+        fail(PB200_ERR_INVALID, "%s: null site, shift or weight", who);
+    for (int t = 0; t < op->n_terms; ++t) {
+        unsigned long long seen = 0;
+        for (int e = op->site_start[t]; e < op->site_start[t + 1]; ++e) {
+            const int k = op->site[e], m = op->shift[e];
+            if (k < 0 || k >= n) fail(PB200_ERR_INVALID, "%s: term %d names qudit %d of a %d-qudit register", who, t, k, n);
+            if ((seen >> k) & 1ull) fail(PB200_ERR_INVALID, "%s: term %d names qudit %d twice", who, t, k);
+            seen |= 1ull << k;
+            if (m < 0 || m >= dim) fail(PB200_ERR_INVALID, "%s: term %d: shift %d outside [0, %d)", who, t, m, dim);
+        }
+    }
+}
+
+// host image of an operator's device table: terms, their site entries and the chunk bounds of the kernels' staging
+struct ExpHost {
+    bool d2 = true;
+    std::vector<char> img;                 // terms | sites | chunk_t | chunk_s, each 256-byte aligned
+    size_t off_sites = 0, off_ct = 0, off_cs = 0;
+    int n_chunks = 0;
+    unsigned used_shard_bits = 0;          // d = 2: bit x set when some mask flips shard bits x (f >> local_bits)
+};
+
+// cut the terms (sorted as the kernel reads them) into chunks of at most kExpChunkTerms terms and kExpChunkSites site
+// entries; a term's site offset s0 is relative to its chunk
+template <typename TermT, typename SiteT>
+static void exp_pack(std::vector<std::pair<TermT, std::vector<SiteT>>>& B, ExpHost& H) {
+    std::vector<TermT> T;
+    std::vector<SiteT> S;
+    std::vector<int> ct{0}, cs{0};
+    int nt = 0, ns = 0;
+    for (auto& b : B) {
+        if (nt == kExpChunkTerms || ns + (int)b.second.size() > kExpChunkSites) {
+            ct.push_back((int)T.size()); cs.push_back((int)S.size());
+            nt = ns = 0;
+        }
+        b.first.s0 = ns; b.first.sn = (int)b.second.size();
+        T.push_back(b.first);
+        S.insert(S.end(), b.second.begin(), b.second.end());
+        ++nt; ns += (int)b.second.size();
+    }
+    if (nt) { ct.push_back((int)T.size()); cs.push_back((int)S.size()); }
+    H.n_chunks = (int)ct.size() - 1;
+    auto al = [](size_t x) { return (x + 255) & ~(size_t)255; };
+    H.off_sites = al(sizeof(TermT) * T.size());
+    H.off_ct = H.off_sites + al(sizeof(SiteT) * S.size());
+    H.off_cs = H.off_ct + al(sizeof(int) * ct.size());
+    H.img.assign(H.off_cs + sizeof(int) * cs.size(), 0);
+    if (!T.empty()) std::memcpy(H.img.data(), T.data(), sizeof(TermT) * T.size());
+    if (!S.empty()) std::memcpy(H.img.data() + H.off_sites, S.data(), sizeof(SiteT) * S.size());
+    std::memcpy(H.img.data() + H.off_ct, ct.data(), sizeof(int) * ct.size());
+    std::memcpy(H.img.data() + H.off_cs, cs.data(), sizeof(int) * cs.size());
+}
+
+// d = 2: each site folds into the masks of expect_terms_d2_kernel; terms sorted by flip mask.  local_bits: index bits
+// held by one plan (N for a whole state)
+static ExpHost exp_host_d2(const pb200_op_terms* op, int n, int local_bits) {
+    std::vector<std::pair<ExpD2Term, std::vector<ExpGenSite>>> B;
+    const cplx* co = reinterpret_cast<const cplx*>(op->coeff);
+    const cplx* w = reinterpret_cast<const cplx*>(op->weight);
+    for (int t = 0; t < op->n_terms; ++t) {
+        ExpD2Term T{};
+        std::vector<ExpGenSite> gen;
+        cplx c = co[t];
+        for (int e = op->site_start[t]; e < op->site_start[t + 1] && c != 0.0; ++e) {
+            const unsigned long long bit = 1ull << (n - 1 - op->site[e]);
+            const cplx w0 = w[2 * e], w1 = w[2 * e + 1];
+            if (op->shift[e]) T.f |= bit;
+            if (w0 == 0.0) { T.care |= bit; T.val |= bit; c *= w1; }    // needs digit 1 (c = 0 when w1 = 0 too)
+            else if (w1 == 0.0) { T.care |= bit; c *= w0; }             // needs digit 0
+            else {
+                c *= w0;
+                const cplx r = w1 / w0;
+                if (r == -1.0) T.z |= bit;
+                else if (r != 1.0) gen.push_back({{r.real(), r.imag()}, bit});
+            }
+        }
+        if (c == 0.0) continue;
+        T.c = {c.real(), c.imag()};
+        B.emplace_back(T, std::move(gen));
+    }
+    std::stable_sort(B.begin(), B.end(), [](const auto& x, const auto& y) { return x.first.f < y.first.f; });
+    ExpHost H;
+    for (const auto& b : B) H.used_shard_bits |= 1u << (unsigned)(b.first.f >> local_bits);
+    exp_pack(B, H);
+    return H;
+}
+
+// d = 3 / 4: strides of the digits, weights padded to 4
+static ExpHost exp_host_general(const pb200_op_terms* op, int n, int dim) {
+    std::vector<std::pair<ExpTerm, std::vector<ExpSite>>> B;
+    const cplx* co = reinterpret_cast<const cplx*>(op->coeff);
+    const cplx* w = reinterpret_cast<const cplx*>(op->weight);
+    for (int t = 0; t < op->n_terms; ++t) {
+        if (co[t] == 0.0) continue;
+        ExpTerm T{};
+        T.c = {co[t].real(), co[t].imag()};
+        std::vector<ExpSite> sites;
+        for (int e = op->site_start[t]; e < op->site_start[t + 1]; ++e) {
+            ExpSite S{};
+            S.stride = 1;
+            for (int j = op->site[e] + 1; j < n; ++j) S.stride *= dim;
+            S.shift = op->shift[e];
+            for (int a = 0; a < dim; ++a) S.w[a] = {w[(size_t)e * dim + a].real(), w[(size_t)e * dim + a].imag()};
+            sites.push_back(S);
+        }
+        B.emplace_back(T, std::move(sites));
+    }
+    ExpHost H;
+    H.d2 = false;
+    exp_pack(B, H);
+    return H;
+}
+
+static ExpHost exp_host(const pb200_op_terms* op, int n, int dim, int local_bits) {
+    return dim == 2 ? exp_host_d2(op, n, local_bits) : exp_host_general(op, n, dim);
+}
+
+// the device copy of an ExpHost on one plan's device.  The pool buffer is released on every exit path, once the plan's
+// stream is idle: the pool is not stream-ordered, and on an error exit a kernel reading the table may still be queued
+struct ExpTable {
+    int dev = -1;
+    cudaStream_t stream = nullptr;
+    char* buf = nullptr;
+    ExpTable() = default;
+    ExpTable(const ExpTable&) = delete;
+    ExpTable& operator=(const ExpTable&) = delete;
+    ~ExpTable() {
+        if (!buf) return;
+        if (cudaStreamSynchronize(stream) != cudaSuccess) cudaGetLastError();
+        pool_free(dev, buf);
+    }
+    void upload(const ExpHost& H, const Plan& P) {
+        dev = P.desc.device;
+        stream = P.stream;
+        buf = (char*)pool_alloc(dev, H.img.size());
+        CUDA_CHECK(cudaMemcpyAsync(buf, H.img.data(), H.img.size(), cudaMemcpyHostToDevice, P.stream));
+    }
+};
+
+// acc[2 c] += <psi_c| op |psi_c> for `count` trajectories; src.p[src.shard] + c D is trajectory c (d = 2), psi (d > 2)
+static void launch_expect(const Plan& P, const ExpHost& H, const ExpTable& X, const ExpSrc& src, const c2* psi, int count,
+                          double* d_acc) {
+    const long long blocks = std::min<long long>((P.D + 255) / 256, (long long)P.sm_count * 8);
+    const dim3 grid((unsigned)std::max<long long>(blocks, 1), (unsigned)count);
+    const int* ct = reinterpret_cast<const int*>(X.buf + H.off_ct);
+    const int* cs = reinterpret_cast<const int*>(X.buf + H.off_cs);
+    if (H.d2)
+        expect_terms_d2_kernel<<<grid, 256, 0, P.stream>>>(src, P.D, reinterpret_cast<const ExpD2Term*>(X.buf),
+                                                           reinterpret_cast<const ExpGenSite*>(X.buf + H.off_sites), ct, cs,
+                                                           H.n_chunks, d_acc);
+    else
+        expect_terms_kernel<<<grid, 256, 0, P.stream>>>(psi, P.D, P.dim, reinterpret_cast<const ExpTerm*>(X.buf),
+                                                        reinterpret_cast<const ExpSite*>(X.buf + H.off_sites), ct, cs,
+                                                        H.n_chunks, d_acc);
+    CUDA_CHECK(cudaGetLastError());
+}
+
 #define PB200_TRY try {
 #define PB200_CATCH                                         \
     }                                                       \
@@ -3148,6 +3316,43 @@ int pb200_state_overlap(pb200_plan* h, int32_t traj0, int32_t count, const doubl
     PB200_CATCH
 }
 
+int pb200_state_expect(pb200_plan* h, int32_t traj0, int32_t count, const pb200_op_terms* op, double* out) {
+    PB200_TRY
+    NvtxRange nvtx_range("pb200_state_expect");
+    if (!h || !out) fail(PB200_ERR_INVALID, "pb200_state_expect: null argument");
+    Plan& P = h->p;
+    refuse_shard(P, "pb200_state_expect", "pb200_shards_expect");
+    if (P.has_diss)
+        fail(PB200_ERR_UNSUPPORTED, "pb200_state_expect: the plan holds a vectorised density matrix, not state vectors");
+    if (traj0 < 0 || count < 1 || traj0 + count > P.B)
+        fail(PB200_ERR_INVALID, "pb200_state_expect: trajectories [%d, %d) outside [0, %d)", traj0, traj0 + count, P.B);
+    check_op_terms(op, P.n, P.dim, "pb200_state_expect");
+    if (!P.state_set) fail(PB200_ERR_STATE, "pb200_state_expect: no state set");
+    std::fill(out, out + 2 * (size_t)count, 0.0);
+    const ExpHost H = exp_host(op, P.n, P.dim, P.n);
+    if (H.n_chunks == 0) return PB200_OK;
+    CUDA_CHECK(cudaSetDevice(P.desc.device));
+    ExpTable X;
+    X.upload(H, P);
+    double* d_acc = (double*)pool_alloc(P.desc.device, sizeof(double) * 2 * count);
+    const c2* psi = P.buf[P.cur] + (size_t)traj0 * P.D;
+    ExpSrc src{};
+    src.p[0] = psi; src.shard = 0; src.local_bits = P.n;
+    cudaError_t e = cudaMemsetAsync(d_acc, 0, sizeof(double) * 2 * count, P.stream);
+    try {
+        if (e == cudaSuccess) launch_expect(P, H, X, src, psi, count, d_acc);
+    } catch (...) {
+        if (cudaStreamSynchronize(P.stream) != cudaSuccess) cudaGetLastError();  // the kernel no longer writes d_acc
+        pool_free(P.desc.device, d_acc);
+        throw;
+    }
+    if (e == cudaSuccess) e = cudaMemcpyAsync(out, d_acc, sizeof(double) * 2 * count, cudaMemcpyDeviceToHost, P.stream);
+    if (e == cudaSuccess) e = cudaStreamSynchronize(P.stream);
+    pool_free(P.desc.device, d_acc);
+    if (e != cudaSuccess) fail(PB200_ERR_CUDA, "pb200_state_expect: %s", cudaGetErrorString(e));
+    PB200_CATCH
+}
+
 int pb200_state_sample(pb200_plan* h, int32_t traj, int32_t one_digit, const double* uniforms, int32_t n_shots,
                        int64_t* out) {
     PB200_TRY
@@ -3489,6 +3694,76 @@ int pb200_shards_energy(pb200_plan** plans, int32_t count, double t_us, double* 
         e += acc[0]; e2 += acc[1];
     }
     energy[0] = e; h2[0] = e2;
+    PB200_CATCH
+}
+
+int pb200_shards_expect(pb200_plan** plans, int32_t count, const pb200_op_terms* op, double* out) {
+    PB200_TRY
+    NvtxRange nvtx_range("pb200_shards_expect");
+    if (!out) fail(PB200_ERR_INVALID, "pb200_shards_expect: null argument");
+    const std::vector<Plan*> G = shard_group(plans, count, "pb200_shards_expect");
+    const Plan& P0 = *G[0];
+    check_op_terms(op, P0.n, P0.dim, "pb200_shards_expect");
+    for (int r = 0; r < count; ++r)
+        if (!G[r]->state_set) fail(PB200_ERR_STATE, "pb200_shards_expect: no state set on shard %d", r);
+    out[0] = out[1] = 0.0;
+    const int L = P0.n - P0.shard_bits;
+    const ExpHost H = exp_host(op, P0.n, P0.dim, L);
+    if (H.n_chunks == 0) return PB200_OK;
+    // shard r reads shard r ^ x for every shard-bit pattern x the masks use: peer access where their devices differ
+    // (pb200_shards_link enables only the single-bit pairs)
+    for (int x = 1; x < count; ++x) {
+        if (!((H.used_shard_bits >> x) & 1u)) continue;
+        for (int r = 0; r < count; ++r) {
+            const int di = G[r]->desc.device, dj = G[r ^ x]->desc.device;
+            if (di == dj) continue;
+            int can = 0;
+            CUDA_CHECK(cudaDeviceCanAccessPeer(&can, di, dj));
+            if (!can)
+                fail(PB200_ERR_UNSUPPORTED, "pb200_shards_expect: the operator pairs shards %d and %d, but device %d cannot "
+                                            "access the memory of device %d (no peer access)", r, r ^ x, di, dj);
+            CUDA_CHECK(cudaSetDevice(di));
+            const cudaError_t e = cudaDeviceEnablePeerAccess(dj, 0);
+            if (e == cudaErrorPeerAccessAlreadyEnabled) cudaGetLastError();
+            else CUDA_CHECK(e);
+        }
+    }
+    ExpSrc src{};
+    src.local_bits = L;
+    for (int r = 0; r < count; ++r) src.p[r] = G[r]->buf[G[r]->cur];
+    std::vector<ExpTable> X(count);
+    std::vector<double*> acc(count, nullptr);
+    // every shard's kernel reads its peers' slices: all streams are idle before any accumulator returns to the pool
+    auto release = [&]() {
+        for (int r = 0; r < count; ++r)
+            if (cudaStreamSynchronize(G[r]->stream) != cudaSuccess) cudaGetLastError();
+        for (int r = 0; r < count; ++r) if (acc[r]) pool_free(G[r]->desc.device, acc[r]);
+    };
+    try {
+        shards_sync(G);  // every slice is complete before a shard reads a peer's
+        for (int r = 0; r < count; ++r) {
+            Plan& P = *G[r];
+            CUDA_CHECK(cudaSetDevice(P.desc.device));
+            X[r].upload(H, P);
+            acc[r] = (double*)pool_alloc(P.desc.device, sizeof(double) * 2);
+            CUDA_CHECK(cudaMemsetAsync(acc[r], 0, sizeof(double) * 2, P.stream));
+            src.shard = r;
+            launch_expect(P, H, X[r], src, nullptr, 1, acc[r]);
+        }
+        for (int r = 0; r < count; ++r) {
+            Plan& P = *G[r];
+            double a[2];
+            CUDA_CHECK(cudaSetDevice(P.desc.device));
+            CUDA_CHECK(cudaMemcpyAsync(a, acc[r], sizeof(double) * 2, cudaMemcpyDeviceToHost, P.stream));
+            CUDA_CHECK(cudaStreamSynchronize(P.stream));
+            out[0] += a[0]; out[1] += a[1];
+        }
+        shards_sync(G);  // no shard still reads a peer's slice
+    } catch (...) {
+        release();
+        throw;
+    }
+    release();
     PB200_CATCH
 }
 

@@ -9,13 +9,16 @@ happens in ``libpulser_b200.so`` on the GPU; there is no CPU path.
 from __future__ import annotations
 
 import ctypes as C
-from typing import Sequence
+from typing import TYPE_CHECKING, Sequence
 
 import numpy as np
 
 from . import _lib
 from ._lib import PlanDesc, RunOpts, RunStats, check, lib
 from .spec import BASIS_ROLES, DriveTable, HamiltonianSpec
+
+if TYPE_CHECKING:
+    from .opterms import OpTerms
 
 _dp = C.POINTER(C.c_double)
 
@@ -308,6 +311,16 @@ class DevicePlan:
             raise ValueError(f"state of length {v.shape[0]}, expected {self.D}")
         out = np.empty((count, 2), dtype=np.float64)
         check(lib.pb200_state_overlap(self._handle, traj0, count, _p(v.view(np.float64)), _p(out)))
+        return out[:, 0] + 1j * out[:, 1]
+
+    def expect_terms(self, terms: "OpTerms", traj0: int = 0, count: int | None = None) -> np.ndarray:
+        """``<psi_b|O|psi_b>`` (complex, not normalised) for the selected trajectories, with ``O`` given as monomial
+        terms (``pulser_b200.opterms.OpTerms``), matrix-free on the device (``pb200_state_expect``)."""
+        count = self.n_traj - traj0 if count is None else count
+        if (terms.n, terms.d) != (self.n, self.dim):
+            raise ValueError(f"operator on {terms.n} qudits of dimension {terms.d}, the plan holds {self.n} of {self.dim}")
+        out = np.empty((count, 2), dtype=np.float64)
+        check(lib.pb200_state_expect(self._handle, traj0, count, C.byref(terms.c_desc()), _p(out)))
         return out[:, 0] + 1j * out[:, 1]
 
     def copy_state_from(self, other: "DevicePlan", src_traj: int = 0, dst_traj: int = 0) -> None:

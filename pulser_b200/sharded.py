@@ -173,6 +173,14 @@ class ShardedPlan:
             raise ValueError(f"state of length {v.shape[0]}, expected {self.D}")
         return sum(s.overlap(v[i * self.Dl:(i + 1) * self.Dl]) for i, s in enumerate(self.shards))
 
+    def expect_terms(self, terms, traj0: int = 0, count: int | None = None) -> np.ndarray:
+        """``<psi|O|psi>`` of the whole state, ``O`` as monomial terms (``pb200_shards_expect``); shape ``[1]``."""
+        if (terms.n, terms.d) != (self.n, self.dim):
+            raise ValueError(f"operator on {terms.n} qudits of dimension {terms.d}, the plan holds {self.n} of {self.dim}")
+        out = np.empty(2, dtype=np.float64)
+        check(lib.pb200_shards_expect(self._arr, self.G, C.byref(terms.c_desc()), _p(out)))
+        return np.array([complex(out[0], out[1])])
+
     def energy(self, t_us: float) -> tuple[np.ndarray, np.ndarray]:
         e = np.empty(1, dtype=np.float64)
         e2 = np.empty(1, dtype=np.float64)
