@@ -1242,6 +1242,8 @@ static void ensure_aux_buffers(Plan& P) {
 }
 
 // ---- Monte-Carlo wave-function propagation (collapse operators without a density matrix) ------------------------
+static constexpr double kMcwfJumpPerStep = 0.01;   // bound on N * rate_max * step
+
 static void propagate_mcwf(Plan& P, double t_start, double t_stop, const pb200_run_opts* o, pb200_run_stats* stats) {
     const double eps = 1e-12;
     const int nt = (int)P.times.size();
@@ -1320,8 +1322,10 @@ static void propagate_mcwf(Plan& P, double t_start, double t_stop, const pb200_r
             const int nsub = jump_substeps(P, t, std::min(P.times[i + 1], t_stop), 1e-9);
             b = std::min(P.times[i + 1], t + hi_i / nsub);
         }
-        // jump times are resolved to one step: keep the jump probability of a qudit per step below 5 %
-        if (rate_max > 0.0) b = std::min(b, std::max(t + 0.05 / rate_max, std::min(P.times[i + 1], t + hi_i / 64.0)));
+        // jump times are resolved to one step and a trajectory jumps at most once per step, so the clocks of the other
+        // qudits restart at the step end: keep the jump probability of the whole register per step below 1 %, which
+        // holds the resulting deficit of jumps (first order in the step) near 1e-3 of the decayed population
+        if (rate_max > 0.0) b = std::min(b, t + kMcwfJumpPerStep / (P.n * rate_max));
         b = std::min(b, t_stop);
         const double h = b - t;
         // exp(-i H_eff h) ~ decay(h/2) U(h) decay(h/2)
