@@ -151,6 +151,11 @@ static void pool_free(int dev, void* p) {
 // store of chi_{k+1} (DESIGN.md section 8).
 constexpr int kTaylorTileBits = 13;
 constexpr int kTaylorRegBits = 4;
+// tile of the Chebyshev / Lanczos stage kernels (stage_d2_rb_kernel, stage_d2_fwd_kernel): 2^11 amplitudes, 8 per thread
+constexpr int kStageTileBits = 11;
+constexpr int kStageRegBits = 3;
+// qubits above the tile that a pass still reaches by partner loads from global memory (plan_passes)
+constexpr int kMaxExtraBits = 16;
 // a state-vector shard holds 2^L amplitudes, 13 <= L <= 29: at least one tile, and the local bits above the tile
 // (at most 16) stay partner loads of the single-pass geometry
 constexpr int kShardMaxLocalBits = 29;
@@ -167,20 +172,18 @@ static int device_setup(int dev) {
     CUDA_CHECK(cudaFuncSetAttribute(stage_d2_kernel<true, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, max_smem));
     CUDA_CHECK(cudaFuncSetAttribute(stage_d2_kernel<true, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, max_smem));
     CUDA_CHECK(cudaFuncSetAttribute(stage_d2_kernel<false, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, max_smem));
-#define PB200_RB_ATTR(TB, RB)                                                                                                            \
-    CUDA_CHECK(cudaFuncSetAttribute(stage_d2_rb_kernel<true, true, TB, RB>, cudaFuncAttributeMaxDynamicSharedMemorySize, max_smem));   \
-    CUDA_CHECK(cudaFuncSetAttribute(stage_d2_rb_kernel<true, false, TB, RB>, cudaFuncAttributeMaxDynamicSharedMemorySize, max_smem));  \
+    constexpr int TB = kStageTileBits, RB = kStageRegBits;
+    CUDA_CHECK(cudaFuncSetAttribute(stage_d2_rb_kernel<true, true, TB, RB>, cudaFuncAttributeMaxDynamicSharedMemorySize, max_smem));
+    CUDA_CHECK(cudaFuncSetAttribute(stage_d2_rb_kernel<true, false, TB, RB>, cudaFuncAttributeMaxDynamicSharedMemorySize, max_smem));
     CUDA_CHECK(cudaFuncSetAttribute(stage_d2_rb_kernel<false, false, TB, RB>, cudaFuncAttributeMaxDynamicSharedMemorySize, max_smem));
-    PB200_RB_ATTR(11, 2) PB200_RB_ATTR(11, 3) PB200_RB_ATTR(12, 2) PB200_RB_ATTR(12, 3)
-#undef PB200_RB_ATTR
     const int taylor_smem = (1 << kTaylorTileBits) * 16 + 2048;   // tile + per-bit table
     CUDA_CHECK(cudaFuncSetAttribute(stage_d2_taylor_kernel<true, true, kTaylorTileBits, kTaylorRegBits>, cudaFuncAttributeMaxDynamicSharedMemorySize, taylor_smem));
     CUDA_CHECK(cudaFuncSetAttribute(stage_d2_taylor_kernel<true, false, kTaylorTileBits, kTaylorRegBits>, cudaFuncAttributeMaxDynamicSharedMemorySize, taylor_smem));
     CUDA_CHECK(cudaFuncSetAttribute(stage_d2_taylor_kernel<false, false, kTaylorTileBits, kTaylorRegBits>, cudaFuncAttributeMaxDynamicSharedMemorySize, taylor_smem));
     CUDA_CHECK(cudaFuncSetAttribute(stage_d2_taylor_kernel<true, true, kTaylorTileBits, kTaylorRegBits, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, taylor_smem));
     CUDA_CHECK(cudaFuncSetAttribute(stage_d2_taylor_kernel<true, false, kTaylorTileBits, kTaylorRegBits, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, taylor_smem));
-    CUDA_CHECK(cudaFuncSetAttribute(stage_d2_fwd_kernel<true, 11, 3>, cudaFuncAttributeMaxDynamicSharedMemorySize, 2 * 2048 * 16 + 256));
-    CUDA_CHECK(cudaFuncSetAttribute(stage_d2_fwd_kernel<false, 11, 3>, cudaFuncAttributeMaxDynamicSharedMemorySize, 2 * 2048 * 16 + 256));
+    CUDA_CHECK(cudaFuncSetAttribute(stage_d2_fwd_kernel<true, TB, RB>, cudaFuncAttributeMaxDynamicSharedMemorySize, 2 * 2048 * 16 + 256));
+    CUDA_CHECK(cudaFuncSetAttribute(stage_d2_fwd_kernel<false, TB, RB>, cudaFuncAttributeMaxDynamicSharedMemorySize, 2 * 2048 * 16 + 256));
     if (dev >= 0 && dev < PB200_MAX_DEVICES) sm_count[dev] = sms;
     return sms;
 }
@@ -216,12 +219,7 @@ struct Plan {
     std::vector<double> dmin_cnt, dmax_cnt;
     std::vector<double> dmin_traj, dmax_traj;
     bool state_set = false;
-    int tile_bits = 12;
-    int max_extra = 3;
     int sm_count = 132;
-    bool force_v1 = false;
-    int reg_bits = 3;
-    bool use_dual = true;
     // Lindblad: per-qudit generators of the dissipator on the (row, column) digit pair
     std::vector<std::vector<cplx>> diss_gen;
     // Krylov (Lanczos) propagator workspace
@@ -248,14 +246,12 @@ struct Plan {
     std::mt19937_64 rng;
     std::vector<double> thresholds;               // per trajectory
     std::vector<long long> jump_count;
-    bool use_pdl = true;
     // step-controller state kept between pb200_propagate calls (evaluation times cut a run into many calls):
     // interval classification of the sampling grid (cache key = window, rough_tol) and the current smooth-step length
     struct FineCache { bool valid = false; int window = -1; double rtol = -1.0; std::vector<char> fine, jump; std::vector<int> dist; } fine_cache;
     double ctrl_Kc = -1.0; double ctrl_key = 0.0; double ctrl_t_end = -1e300;
     // partner-sum forwarding between Clenshaw stages (stage_d2_fwd_kernel): geometry of a chain's first stage [0],
     // of the high-bit tile [1] and of the later low-bit stages [2]; one buffer of forwarded sums per chain
-    bool use_fwd = true;            // PB200_FWD=0: single-pass stages only
     bool fwd_now = false;           // decided per propagate call
     PassGeom fwd_geo[3];
     c2* wbuf[2] = {nullptr, nullptr};
@@ -277,9 +273,6 @@ struct Plan {
         double* d_tab = nullptr;
     } tay;
     std::vector<c2*> tay_ws;
-    bool use_taylor = true;         // PB200_TAYLOR=0: never chosen automatically
-    bool use_lanczos_fuse = true;   // PB200_LANCZOS_FUSE=0: separate vector-update kernel (cross-check)
-    int use_tiled = 1;              // PB200_TILED: d = 3 / 4 registers: 1 register-blocked tiled kernel, 0 generic
     // state-vector shard (pb200_plan_create_shard): the top shard_bits qubits of the global index equal `shard`; n is
     // the global N, D = 2^(N - shard_bits) the slice this plan holds.  `group` = every shard, by index, once linked
     int shard_bits = 0, shard = 0;
@@ -396,20 +389,19 @@ static StageArgs make_stage_args(const Plan& P, const PassGeom& geo, const Stage
 
 // d = 3 / 4 registers without an exchange term run on the register-blocked tiled kernel
 static bool multilevel_eligible(const Plan& P) {
-    return P.use_tiled == 1 && !P.has_xy && (P.dim == 3 || P.dim == 4) && P.n <= PB200_TILED_MAX_HIGH &&
+    return !P.has_xy && (P.dim == 3 || P.dim == 4) && P.n <= PB200_TILED_MAX_HIGH &&
            P.n >= (P.dim == 3 ? 2 : 1) && !(P.dim == 2);
 }
 
-static bool rb_eligible(const Plan& P, const PassGeom& geo) {
-    const int tbits = geo.lo_bits + geo.hi_bits;
-    return (tbits == 11 || tbits == 12) && (geo.first_pass || geo.hi_bits >= P.reg_bits) && !P.force_v1;
+static bool rb_eligible(const PassGeom& geo) {
+    return geo.lo_bits + geo.hi_bits == kStageTileBits && (geo.first_pass || geo.hi_bits >= kStageRegBits);
 }
 
 // every pass of the geometry can carry two chains in one launch
 static bool dual_chain_ok(const Plan& P, const std::vector<PassGeom>& passes) {
-    if (!is_d2path(P) || !P.use_dual) return false;
+    if (!is_d2path(P)) return false;
     for (const PassGeom& g : passes)
-        if (!rb_eligible(P, g)) return false;
+        if (!rb_eligible(g)) return false;
     return (long long)P.B * 2 <= 65535;
 }
 
@@ -427,29 +419,17 @@ static void launch_stage_multi(Plan& P, const std::vector<PassGeom>& passes, con
             const long long tiles = P.D >> tbits;
             const int tsize = 1 << tbits;
             const size_t tab_bytes = uniform ? 0 : (size_t)d2_table_stride(N) * 8;
-            const int RBv = P.reg_bits;
-            if (rb_eligible(P, geo)) {
-                const int threads = tsize >> RBv;
-                {
-                    StageArgs2 m{};
-                    for (int c = 0; c < n; ++c) m.a[c] = make_stage_args(P, geo, io[c], last_pass);
-                    m.n_traj = P.B;
-                    dim3 grid((unsigned)tiles, (unsigned)(P.B * n));
-                    const size_t smem = (size_t)tsize * 16 + tab_bytes;
-#define PB200_LAUNCH_RB(TB, RB)                                                                                \
-    do {                                                                                                       \
-        if (uniform) {                                                                                         \
-            if (real_g) launch_k(stage_d2_rb_kernel<true, true, TB, RB>, grid, dim3(threads), smem, P.stream, P.use_pdl, m);   \
-            else launch_k(stage_d2_rb_kernel<true, false, TB, RB>, grid, dim3(threads), smem, P.stream, P.use_pdl, m);         \
-        } else {                                                                                               \
-            launch_k(stage_d2_rb_kernel<false, false, TB, RB>, grid, dim3(threads), smem, P.stream, P.use_pdl, m);             \
-        }                                                                                                      \
-    } while (0)
-                    if (tbits == 11) { if (RBv == 3) PB200_LAUNCH_RB(11, 3); else PB200_LAUNCH_RB(11, 2); }
-                    else { if (RBv == 3) PB200_LAUNCH_RB(12, 3); else PB200_LAUNCH_RB(12, 2); }
-#undef PB200_LAUNCH_RB
-                    ++launches;
-                }
+            if (rb_eligible(geo)) {
+                constexpr int TB = kStageTileBits, RB = kStageRegBits;
+                StageArgs2 m{};
+                for (int c = 0; c < n; ++c) m.a[c] = make_stage_args(P, geo, io[c], last_pass);
+                m.n_traj = P.B;
+                dim3 grid((unsigned)tiles, (unsigned)(P.B * n)), block(tsize >> RB);
+                const size_t smem = (size_t)tsize * 16 + tab_bytes;
+                if (!uniform) launch_k(stage_d2_rb_kernel<false, false, TB, RB>, grid, block, smem, P.stream, true, m);
+                else if (real_g) launch_k(stage_d2_rb_kernel<true, true, TB, RB>, grid, block, smem, P.stream, true, m);
+                else launch_k(stage_d2_rb_kernel<true, false, TB, RB>, grid, block, smem, P.stream, true, m);
+                ++launches;
             } else {
                 for (int c = 0; c < n; ++c) {
                     StageArgs a = make_stage_args(P, geo, io[c]);
@@ -503,18 +483,19 @@ static void launch_stage_multi(Plan& P, const std::vector<PassGeom>& passes, con
 }
 
 // ---- partner-sum forwarding (uniform drives, Chebyshev chains) ----------------------------------------------------
+// The second in-tile gather and the 64-byte rows of the high-bit tile cost as much shared-memory / LSU time as the
+// forwarded sums save in L2 traffic once N >= 20, while at N = 18 (256-byte rows) forwarding saves L2 traffic
+// without that penalty: it is used for the registers in between only (DESIGN.md section 6 gives both sides).
+constexpr int kFwdMinN = 17, kFwdMaxN = 19;
+
 static bool fwd_eligible(const Plan& P, const std::vector<PassGeom>& passes) {
-    if (!P.use_fwd || !is_d2path(P) || P.force_v1 || !P.all_uniform() || P.B != 1) return false;
-    if (P.tile_bits != 11 || P.reg_bits != 3) return false;
-    if (passes.size() != 1 || passes[0].hi_bits != 0 || passes[0].lo_bits != 11) return false;
-    // The second in-tile gather and the 64-byte rows of the high-bit tile cost as much shared-memory / LSU time as the
-    // forwarded sums save in L2 traffic once N >= 20, while at N = 18 (256-byte rows) forwarding saves L2 traffic
-    // without that penalty: it is used for the registers in between only (tools/fwd_ab.py measures both sides).
-    return P.n >= env_int("PB200_FWD_MIN_N", 17) && P.n <= env_int("PB200_FWD_MAX_N", 19);
+    if (!is_d2path(P) || !P.all_uniform() || P.B != 1) return false;
+    if (passes.size() != 1 || passes[0].hi_bits != 0 || passes[0].lo_bits != kStageTileBits) return false;
+    return P.n >= kFwdMinN && P.n <= kFwdMaxN;
 }
 
 static void plan_fwd_geometry(Plan& P) {
-    const int N = P.n, TB = P.tile_bits;
+    const int N = P.n, TB = kStageTileBits;
     const int hb = std::min(N - TB, TB - 2);
     const unsigned long long all = (N >= 64) ? ~0ULL : ((1ULL << N) - 1ULL);
     const unsigned long long rest = all & ~((1ULL << (TB + hb)) - 1ULL);
@@ -535,7 +516,7 @@ static void plan_fwd_geometry(Plan& P) {
 static void launch_stage_fwd(Plan& P, const StageIO* io, int n, long long& launches) {
     bool real_g = true;
     for (int c = 0; c < n; ++c) real_g = real_g && io[c].real_g;
-    const int tbits = P.tile_bits;
+    constexpr int TB = kStageTileBits, RB = kStageRegBits;
     StageArgs2 m{};
     for (int c = 0; c < n; ++c) {
         StageArgs& a = m.a[c];
@@ -545,10 +526,10 @@ static void launch_stage_fwd(Plan& P, const StageIO* io, int n, long long& launc
         a.w_plane = P.D * (long long)P.B;
     }
     m.n_traj = P.B;
-    dim3 grid((unsigned)(P.D >> tbits), (unsigned)(P.B * n));
-    const size_t smem = (size_t)2 * ((size_t)16 << tbits);
-    if (real_g) launch_k(stage_d2_fwd_kernel<true, 11, 3>, grid, dim3(256), smem, P.stream, P.use_pdl, m);
-    else launch_k(stage_d2_fwd_kernel<false, 11, 3>, grid, dim3(256), smem, P.stream, P.use_pdl, m);
+    dim3 grid((unsigned)(P.D >> TB), (unsigned)(P.B * n));
+    const size_t smem = (size_t)2 * ((size_t)16 << TB);
+    if (real_g) launch_k(stage_d2_fwd_kernel<true, TB, RB>, grid, dim3(256), smem, P.stream, true, m);
+    else launch_k(stage_d2_fwd_kernel<false, TB, RB>, grid, dim3(256), smem, P.stream, true, m);
     ++launches;
 }
 
@@ -895,9 +876,9 @@ static void krylov_exponential(Plan& P, const ExpParams& E, double tol, const st
     ud.g = {E.g[0].real(), E.g[0].imag()}; ud.theta = E.th[0]; ud.w = E.w; ud.gamma = 0.0;
     const bool real_g = E.g[0].imag() == 0.0;
     bool fused_dot = d2path;
-    for (const PassGeom& g : passes) fused_dot = fused_dot && rb_eligible(P, g);
+    for (const PassGeom& g : passes) fused_dot = fused_dot && rb_eligible(g);
     // one launch per iteration: single-pass register-blocked d = 2 geometry, or the tiled d = 3 / 4 kernel
-    const bool fused = P.use_lanczos_fuse && ((fused_dot && passes.size() == 1) || (!d2path && multilevel_eligible(P)));
+    const bool fused = (fused_dot && passes.size() == 1) || (!d2path && multilevel_eligible(P));
     if (fused) fused_dot = true;
     c2* psi = P.buf[P.cur];
     c2* outb = P.buf[(P.cur + 1) % 3];
@@ -1249,7 +1230,7 @@ static void propagate_mcwf(Plan& P, double t_start, double t_stop, const pb200_r
     const int nt = (int)P.times.size();
     pb200_run_stats st{};
     P.use_krylov = false; P.fwd_now = false;
-    const std::vector<PassGeom> passes = plan_passes(P.n, P.tile_bits, P.max_extra);
+    const std::vector<PassGeom> passes = plan_passes(P.n, kStageTileBits, kMaxExtraBits);
     std::vector<char> jump; std::vector<int> dist;
     const std::vector<char> fine = fine_intervals(P, 8, 1e-4, 0.05, jump, dist);
     (void)fine;
@@ -1442,7 +1423,7 @@ static void propagate(Plan& P, double t_start, double t_stop, const pb200_run_op
         const int req = o ? o->integrator : 0;
         if (req < 0 || req > 3) fail(PB200_ERR_INVALID, "integrator must be 0 (auto), 1, 2 or 3");
         bool want = req == 3;
-        if (req == 0 && P.use_taylor) {
+        if (req == 0) {
             const bool steered = o && (o->max_step_samples > 0 || o->tol < 0.0 || o->extrapolate < 0 || o->check_every > 0 ||
                                        o->cheb_tol > 0.0 || (o->magnus_order != 0 && o->magnus_order != 4));
             want = !steered && t_stop > t_start;   // short calls too ("Full" evaluation times: one call per sampling
@@ -1465,9 +1446,11 @@ static void propagate(Plan& P, double t_start, double t_stop, const pb200_run_op
     // Richardson extrapolation: on by default (extrapolate = 0 or 1), -1 switches it off
     const bool extrap = !(o && o->extrapolate < 0);
     const bool adaptive = gtol > 0.0;
+    // defaults of max_step_samples (adaptive + extrapolated / adaptive / fixed steps) and refine_window
+    constexpr int kMaxStepExtrap = 32, kMaxStepAdaptive = 16, kMaxStepFixed = 4, kRefineWindow = 8;
     int Kmax = (o && o->max_step_samples > 0) ? o->max_step_samples
-                                               : env_int("PB200_MAX_STEP", adaptive ? (extrap ? 32 : 16) : 4);
-    int W = (o && o->refine_window >= 0) ? o->refine_window : env_int("PB200_REFINE_WINDOW", 8);
+                                               : (adaptive ? (extrap ? kMaxStepExtrap : kMaxStepAdaptive) : kMaxStepFixed);
+    int W = (o && o->refine_window >= 0) ? o->refine_window : kRefineWindow;
     const double tol_user = (o && o->cheb_tol > 0) ? o->cheb_tol : 0.0;
     double rtol = (o && o->rough_tol > 0) ? o->rough_tol : 1e-4;
     int order = (o && o->magnus_order) ? o->magnus_order : 4;
@@ -1475,7 +1458,7 @@ static void propagate(Plan& P, double t_start, double t_stop, const pb200_run_op
     if (order != 2 && order != 4) fail(PB200_ERR_INVALID, "magnus_order must be 2 or 4");
 
     pb200_run_stats st{};
-    const std::vector<PassGeom> passes = plan_passes(P.n, P.tile_bits, P.max_extra);
+    const std::vector<PassGeom> passes = plan_passes(P.n, kStageTileBits, kMaxExtraBits);
     if (!P.fine_cache.valid || P.fine_cache.window != W || P.fine_cache.rtol != rtol) {
         P.fine_cache.fine = fine_intervals(P, W, rtol, 0.05, P.fine_cache.jump, P.fine_cache.dist);
         for (size_t i = 0; i < P.fine_cache.fine.size(); ++i) if (P.fine_cache.jump[i]) P.fine_cache.fine[i] = 1;
@@ -1534,6 +1517,8 @@ static void propagate(Plan& P, double t_start, double t_stop, const pb200_run_op
     // auto picks Lanczos when one sampling interval already spans a Chebyshev half-width near 1, i.e. for
     // strongly blockaded registers whose high-energy states are not populated
     {
+        constexpr double kKrylovRhoPerInterval = 0.9;
+        constexpr double kKrylovStateBytes = 64.0 * 1048576.0;
         const int req = o ? o->integrator : 0;
         bool kry = (req == 2);
         if (req == 0) {
@@ -1545,14 +1530,14 @@ static void propagate(Plan& P, double t_start, double t_stop, const pb200_run_op
             double gm, rh1; std::vector<double> scratch_tab;
             build_tables(P, E, gm, rh1, scratch_tab, is_d2path(P));
             // ... or when the state no longer fits L2 (fewer, fatter iterations win once HBM-bound)
-            kry = rh1 > env_int("PB200_KRYLOV_RHO_MILLI", 900) * 1e-3 ||
-                  (double)P.D * P.B * 16.0 > (double)env_int("PB200_KRYLOV_MIB", 64) * 1048576.0;
+            kry = rh1 > kKrylovRhoPerInterval || (double)P.D * P.B * 16.0 > kKrylovStateBytes;
             (void)tb;
         }
         P.use_krylov = kry;
     }
-    const double rho_cap = P.use_krylov ? env_int("PB200_RHO_CAP_KRYLOV_MILLI", 12000) * 1e-3
-                                        : env_int("PB200_RHO_CAP_MILLI", 3600) * 1e-3;
+    // spectral half-width of one step's exponential: Chebyshev / Lanczos
+    constexpr double kRhoCapChebyshev = 3.6, kRhoCapKrylov = 12.0;
+    const double rho_cap = P.use_krylov ? kRhoCapKrylov : kRhoCapChebyshev;
     const bool dual_ok = dual_chain_ok(P, passes) && !P.has_diss && !P.use_krylov;
     P.fwd_now = !P.use_krylov && !P.has_diss && fwd_eligible(P, passes);
     if (P.fwd_now) plan_fwd_geometry(P);
@@ -1854,7 +1839,7 @@ static bool taylor_prepare(Plan& P) {
     Plan::TaylorCache& C = P.tay;
     g_taylor_why = "structure (d, drives, collapse / dissipator / mask, interpolation order)";
     if (!is_d2path(P)) return false;
-    if (P.has_diss || P.has_collapse || P.has_slm || P.force_v1) return false;
+    if (P.has_diss || P.has_collapse || P.has_slm) return false;
     if (P.desc.interp_order != 3 && P.desc.interp_order != 1) return false;
     if (C.valid) { if (C.ok) g_taylor_why = ""; return C.ok; }
     C.valid = true; C.ok = false;
@@ -2008,7 +1993,8 @@ static bool taylor_worthwhile(Plan& P, double gtol) {
     for (int i = 0; i + 1 < nt; ++i) wsum += 0.5 * (P.tay.w_knot[i] + P.tay.w_knot[i + 1]) * (P.times[i + 1] - P.times[i]);
     const double applies_per_interval = 4.1 * wsum / std::max(nt - 1, 1);
     const double hi_mean_ns = (P.times.back() - P.times.front()) / std::max(nt - 1, 1) * 1e3;
-    const bool cheap = applies_per_interval / std::max(hi_mean_ns, 1e-30) <= env_int("PB200_TAYLOR_MAX_APPLIES_MILLI", 12000) * 1e-3;
+    constexpr double kTaylorMaxAppliesPerNs = 12.0;
+    const bool cheap = applies_per_interval / std::max(hi_mean_ns, 1e-30) <= kTaylorMaxAppliesPerNs;
     if (!cheap) g_taylor_why = "spectrum too wide: the Krylov path is expected to be cheaper";
     return cheap;
 }
@@ -2099,9 +2085,9 @@ static void launch_taylor_stage(Plan& P, const PassGeom* geo, const TaylorArgs& 
         dim3 grid((unsigned)(P.D >> TB), (unsigned)(uniform ? 1 : P.B)), block(1 << (TB - RB));
         // the kernel keeps a per-bit table behind the tile unless the drive is uniform and real
         const size_t smem = ((size_t)16 << TB) + (uniform && real_g ? 0 : (size_t)d2_table_stride(P.n) * 8);
-        if (!uniform) launch_k(stage_d2_taylor_kernel<false, false, TB, RB>, grid, block, smem, P.stream, P.use_pdl, a);
-        else if (real_g) launch_k(stage_d2_taylor_kernel<true, true, TB, RB>, grid, block, smem, P.stream, P.use_pdl, a);
-        else launch_k(stage_d2_taylor_kernel<true, false, TB, RB>, grid, block, smem, P.stream, P.use_pdl, a);
+        if (!uniform) launch_k(stage_d2_taylor_kernel<false, false, TB, RB>, grid, block, smem, P.stream, true, a);
+        else if (real_g) launch_k(stage_d2_taylor_kernel<true, true, TB, RB>, grid, block, smem, P.stream, true, a);
+        else launch_k(stage_d2_taylor_kernel<true, false, TB, RB>, grid, block, smem, P.stream, true, a);
     } else {
         dim3 grid((unsigned)((P.D + 255) / 256), (unsigned)P.B);
         stage_d2_taylor_small_kernel<<<grid, 256, 0, P.stream>>>(a);
@@ -2112,7 +2098,7 @@ static void launch_taylor_stage(Plan& P, const PassGeom* geo, const TaylorArgs& 
 // geometry of the Taylor stage: the register-blocked single-pass kernel on its own 2^kTaylorTileBits tile (whatever
 // tile the Magnus stages use), or the plain kernel for small registers
 static bool taylor_geometry(const Plan& P, std::vector<PassGeom>& passes, bool& use_rb) {
-    passes = plan_passes(P.n, kTaylorTileBits, P.max_extra);
+    passes = plan_passes(P.n, kTaylorTileBits, kMaxExtraBits);
     use_rb = passes.size() == 1 && passes[0].first_pass && passes[0].hi_bits == 0 && passes[0].lo_bits == kTaylorTileBits;
     return use_rb || P.n <= 16;
 }
@@ -2137,7 +2123,7 @@ struct TaylorScheduler {
     Plan& P;
     double t_stop, eps = 1e-12, gtol, rate, rho_target, fit_total, fit_spent = 0.0, round2 = 0.0;
     double t, steps_len = 0.0, t_retry_len = 0.0, A_sum, C_sum, kRoundUnit = 0.05 * 1.1102230246251565e-16;
-    int pmax, order, N, nt;
+    int order, N, nt;
     bool log_steps;
     pb200_run_stats st{};
     struct Fit { TaylorPoly om, th, m; bool ok; };
@@ -2146,24 +2132,23 @@ struct TaylorScheduler {
         const double tlo = P.times.front(), thi = P.times.back();
         gtol = (o && o->tol > 0.0) ? o->tol : 1e-8;
         rate = gtol / std::max(thi - tlo, 1e-30);       // error budget per unit of time
-        const double rho_max = env_int("PB200_TAYLOR_RHO_MILLI", 14000) * 1e-3;
-        pmax = std::min(PB200_TAYLOR_PMAX, std::max(1, env_int("PB200_TAYLOR_P", PB200_TAYLOR_PMAX)));
+        constexpr double kTaylorRhoMax = 14.0;
         order = P.desc.interp_order;
         N = P.n;
         nt = (int)P.times.size();
         Plan::TaylorCache& C = P.tay;
         taylor_knot_widths(P);
-        // Step length: rho = h W <= rho_max, lowered where the fp64 cancellation of the series would eat the tolerance.  The
-        // rounding error of a step grows like e^rho: ~0.05 eps e^rho measured (tools/taylor_rho_sweep.py: 6e-12 per
+        // Step length: rho = h W <= kTaylorRhoMax, lowered where the fp64 cancellation of the series would eat the tolerance.  The
+        // rounding error of a step grows like e^rho: ~0.05 eps e^rho measured (DESIGN.md section 3a: 6e-12 per
         // step at rho = 14, 1.4e-10 at 18), random from step to step, n ~ (int W dt) / rho steps over the whole sequence;
         // it may use a fifth of the tolerance.  At the default 1e-8 this never binds (17 > 14 for C2, C4, C5).
-        rho_target = rho_max;
+        rho_target = kTaylorRhoMax;
         {
             double w_total = 0.0;
             for (int i = 0; i + 1 < nt; ++i) w_total += 0.5 * (C.w_knot[i] + C.w_knot[i + 1]) * (P.times[i + 1] - P.times[i]);
             for (int it = 0; it < 3; ++it) {
                 const double n_est = std::max(w_total / std::max(rho_target, 1.0), 1.0);
-                rho_target = std::min(rho_max, std::max(4.0, std::log(0.2 * gtol / (kRoundUnit * std::sqrt(n_est)))));
+                rho_target = std::min(kTaylorRhoMax, std::max(4.0, std::log(0.2 * gtol / (kRoundUnit * std::sqrt(n_est)))));
             }
         }
         A_sum = std::max(C.a_sum_max, 1e-300); C_sum = std::max(C.c_sum_max, 1e-300);
@@ -2183,17 +2168,17 @@ struct TaylorScheduler {
         // |dH| <= r_om sum|a| + r_th N + r_M sum|c| : a third of the step's allowance each
         const double third = budget / (3.0 * h);
         // smallest passing degree; a candidate that spans several intervals is first tried at the highest degree so
-        // that a step across a non-smooth sample is refused after one fit instead of pmax + 1
+        // that a step across a non-smooth sample is refused after one fit instead of PB200_TAYLOR_PMAX + 1
         auto one = [&](const PiecewiseCubic<double>& pc, TaylorPoly& out, double allow) {
             if (!single_piece) {
-                out = taylor_fit(pc, P.times, order, a, h, pmax);
+                out = taylor_fit(pc, P.times, order, a, h, PB200_TAYLOR_PMAX);
                 if (out.resid > allow) return false;
             }
-            for (int p = 0; p < pmax; ++p) {
+            for (int p = 0; p < PB200_TAYLOR_PMAX; ++p) {
                 TaylorPoly f = taylor_fit(pc, P.times, order, a, h, p);
                 if (f.resid <= allow || (single_piece && p >= 3)) { out = f; return true; }
             }
-            if (single_piece) out = taylor_fit(pc, P.times, order, a, h, pmax);
+            if (single_piece) out = taylor_fit(pc, P.times, order, a, h, PB200_TAYLOR_PMAX);
             return true;
         };
         F.ok = one(C.om, F.om, third / A_sum) && one(P.tabs[0][0].det[0], F.th, third / N);
@@ -2229,7 +2214,7 @@ struct TaylorScheduler {
                 if (t_retry_len > 0.0) { b = std::min(b, t + t_retry_len); t_retry_len = 0.0; }
                 if (b <= t + eps) b = std::min(P.times[i0 + 1], t_stop);
             }
-            // longest step on which both splines are polynomials of degree <= pmax to within the budget: bisection over
+            // longest step on which both splines are polynomials of degree <= PB200_TAYLOR_PMAX to within the budget: bisection over
             // the number of whole sampling intervals beyond the first one (a step inside one interval is a cubic: exact)
             Fit F;
             {
@@ -2477,7 +2462,7 @@ static void apply_h_device(Plan& P, double t, const c2* in, c2* out, long long& 
     UniformDrive ud{};
     ud.g = {E.g[0].real(), E.g[0].imag()}; ud.theta = E.th[0]; ud.w = 1.0; ud.gamma = 0.0;
     StageCoef sc{{0, 0}, {0, 0}, {1, 0}};
-    const std::vector<PassGeom> passes = plan_passes(P.n, P.tile_bits, P.max_extra);
+    const std::vector<PassGeom> passes = plan_passes(P.n, kStageTileBits, kMaxExtraBits);
     launch_stage(P, passes, in, nullptr, nullptr, out, sc, uniform, E.g[0].imag() == 0.0, ud, P.d_table, launches);
     CUDA_CHECK(cudaGetLastError());
 }
@@ -2822,16 +2807,6 @@ static void create_plan(pb200_plan** out, const pb200_plan_desc* d, int shard_bi
     D >>= shard_bits;
     P.D = D;
     P.shard_bits = shard_bits; P.shard = shard;
-    P.tile_bits = std::min(13, std::max(2, env_int("PB200_TILE_BITS", 11)));
-    P.max_extra = std::max(0, env_int("PB200_MAX_EXTRA", 16));
-    P.force_v1 = env_int("PB200_FORCE_V1", 0) != 0;
-    P.reg_bits = env_int("PB200_REG_BITS", 3) == 2 ? 2 : 3;
-    P.use_dual = env_int("PB200_DUAL", 1) != 0;
-    P.use_pdl = env_int("PB200_PDL", 1) != 0;
-    P.use_lanczos_fuse = env_int("PB200_LANCZOS_FUSE", 1) != 0;
-    P.use_taylor = env_int("PB200_TAYLOR", 1) != 0;
-    P.use_fwd = env_int("PB200_FWD", 1) != 0;
-    P.use_tiled = env_int("PB200_TILED", 1);
     P.sm_count = device_setup(d->device);
     try {
         CUDA_CHECK(cudaStreamCreateWithFlags(&P.stream, cudaStreamNonBlocking));
@@ -3492,7 +3467,7 @@ int pb200_bench_apply(pb200_plan* h, double t_us, int32_t reps, double* ms_out, 
     UniformDrive ud{};
     ud.g = {E.g[0].real(), E.g[0].imag()}; ud.theta = E.th[0]; ud.w = 1.0; ud.gamma = 0.0;
     StageCoef sc{{0, 0}, {0, 0}, {1, 0}};
-    const std::vector<PassGeom> passes = plan_passes(P.n, P.tile_bits, P.max_extra);
+    const std::vector<PassGeom> passes = plan_passes(P.n, kStageTileBits, kMaxExtraBits);
     EventPair evs;
     cudaEvent_t e0 = evs.a, e1 = evs.b;
     launches = 0;

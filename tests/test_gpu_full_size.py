@@ -60,20 +60,19 @@ def test_c5_whole_sequence(engine):
     assert outs["auto"][1]["n_applies"] < 0.5 * outs["lanczos"][1]["n_applies"]
 
 
-def test_c5_code_path_vs_oracle(engine, monkeypatch):
-    """The same auto rule forced at N = 10 (PB200_KRYLOV_MIB = 0) against the DOP853 oracle."""
+def test_c5_lanczos_path_vs_oracle(engine):
+    """The Magnus / Krylov path C5 takes when the Taylor propagator does not apply, at N = 10 against the DOP853
+    oracle."""
     from oracle import evolve
     from oracle.ref_hamiltonian import OracleHamiltonian
 
-    monkeypatch.setenv("PB200_KRYLOV_MIB", "0")
-    monkeypatch.setenv("PB200_TAYLOR", "0")   # the Magnus / Krylov path is what this test pins
     spec = W.config_c5(n=10, t_total=800)
     psi0 = evolve.all_ground_state(spec)
     tf = spec.sampling_times[-1]
     ref = evolve.sesolve(OracleHamiltonian.from_spec(spec), psi0, [0.0, tf], rtol=1e-13, atol=1e-15)[-1]
     with engine.DevicePlan(spec) as plan:
         plan.set_state("all-ground")
-        st = plan.propagate(0.0, tf)
+        st = plan.propagate(0.0, tf, integrator=2)
         got = plan.get_state()[0]
     assert st["integrator"] == 2
     assert np.max(np.abs(got - ref)) < STATE_TOL

@@ -175,21 +175,64 @@ def test_full_size_properties(engine, n):
     assert np.max(np.abs(outs[0.0] - outs[1e-11])) < STATE_TOL
 
 
-@pytest.mark.parametrize("tile_bits,max_extra,reg_bits", [(11, 0, 3), (11, 2, 2), (12, 0, 3), (12, 3, 2), (11, 16, 3)])
-def test_pass_geometries(engine, monkeypatch, tile_bits, max_extra, reg_bits):
-    """Every tile / pass decomposition gives the same H psi (uniform and local drives)."""
-    from oracle.matfree import MatFreeHamiltonian
+def _sparse_apply_h(spec, t, states, amps):
+    """H(t) v for v = sum_i amps[i] |states[i]> (d = 2, one drive, Ising), from the coefficient functions and role
+    table of oracle/matfree.py: O(N^2) per basis state, for registers whose dense vectors the oracle cannot build."""
+    from scipy.interpolate import make_interp_spline
+    from oracle.matfree import BASIS_ROLES
 
-    monkeypatch.setenv("PB200_TILE_BITS", str(tile_bits))
-    monkeypatch.setenv("PB200_MAX_EXTRA", str(max_extra))
-    monkeypatch.setenv("PB200_REG_BITS", str(reg_bits))
-    for spec in (W.config_c2(n=17, seed=2), random_local_spec(16, T=32, seed=5)):
-        mf = MatFreeHamiltonian(spec)
+    n = spec.n_qudits
+    drv = spec.drives[0]
+    to, frm = (spec.eigenbasis.index(x) for x in BASIS_ROLES[drv.basis])
+    assert {to, frm} == {0, 1}
+    c = make_interp_spline(spec.sampling_times, drv.coef.T, k=3)(t)
+    det = make_interp_spline(spec.sampling_times, drv.det.T, k=3)(t)
+    r = spec.eigenbasis.index("r")
+    U = spec.pair_matrix()
+    out = {}
+    for s, a in zip(states, amps):
+        dig = [(s >> (n - 1 - k)) & 1 for k in range(n)]     # qudit 0 is the most significant bit
+        ryd = [k for k in range(n) if dig[k] == r]
+        diag = sum(U[i, j] for x, i in enumerate(ryd) for j in ryd[x + 1:]) - sum(det[k] for k in range(n) if dig[k] == frm)
+        out[s] = out.get(s, 0.0) + diag * a
+        for k in range(n):   # c |to><from| + conj(c) |from><to| on qudit k
+            s2 = s ^ (1 << (n - 1 - k))
+            out[s2] = out.get(s2, 0.0) + (c[k] if dig[k] == frm else np.conj(c[k])) * a
+    return out
+
+
+@pytest.mark.parametrize("n,kind", [(17, "uniform"), (16, "local"), (27, "local"), (28, "uniform"), (28, "local")])
+def test_pass_geometries(engine, n, kind):
+    """H psi on the pass decompositions production takes, uniform and local drives: one pass of the 2^11 tile with
+    partner loads for the bits above it (N <= 27), and from N = 28 a second pass over the next 9 bits with the rest as
+    partner loads.  N >= 27 against the sparse oracle, for a sparse input with partners in every pass and extra bit."""
+    spec = W.config_c2(n=n, seed=2) if kind == "uniform" else random_local_spec(n, T=32, seed=5)
+    if n < 27:
+        from oracle.matfree import MatFreeHamiltonian
+
         v = random_state(spec.hilbert_dim, 4)
         with engine.DevicePlan(spec) as plan:
             got = plan.apply_h(0.0123, v)
-        ref = mf.apply(0.0123, v)
+        ref = MatFreeHamiltonian(spec).apply(0.0123, v)
         assert np.max(np.abs(got - ref)) < 1e-12 * max(1.0, np.max(np.abs(ref)))
+        return
+    rng = np.random.default_rng(4)
+    states = [(1 << n) - 1, 1 << (n - 1)] + [int(x) for x in rng.integers(0, 1 << n, size=6)]
+    states = list(dict.fromkeys(states))
+    amps = rng.normal(size=len(states)) + 1j * rng.normal(size=len(states))
+    t = 0.0123
+    ref = _sparse_apply_h(spec, t, states, amps)
+    v = np.zeros(1 << n, dtype=np.complex128)
+    v[states] = amps
+    with engine.DevicePlan(spec) as plan:
+        got = plan.apply_h(t, v)
+    del v
+    idx = np.array(sorted(ref))
+    want = np.array([ref[i] for i in idx])
+    assert len(idx) <= len(states) * (n + 1)
+    assert np.max(np.abs(got[idx] - want)) < 1e-12 * max(1.0, np.max(np.abs(want)))
+    got[idx] = 0.0
+    assert not np.any(got)
 
 
 # ---------------------------------------------------------------------------
@@ -308,24 +351,20 @@ def _multilevel_spec(n, dim, seed=0, T=48):
     return base
 
 
-@pytest.mark.parametrize("n,dim", [(2, 3), (3, 3), (7, 3), (8, 3), (9, 3), (10, 3), (1, 4), (5, 4), (7, 4)])
-def test_tiled_multilevel_kernel_apply_h(engine, monkeypatch, n, dim):
-    """stage_multilevel_rb_kernel (d = 3 / 4) == matrix-free oracle == the one-thread-per-amplitude generic kernel."""
+@pytest.mark.parametrize("n,dim", [(1, 3), (2, 3), (3, 3), (7, 3), (8, 3), (9, 3), (10, 3), (1, 4), (5, 4), (7, 4)])
+def test_tiled_multilevel_kernel_apply_h(engine, n, dim):
+    """stage_multilevel_rb_kernel (d = 3 / 4) == matrix-free oracle; (1, 3) runs the one-thread-per-amplitude generic
+    kernel instead."""
     from oracle.matfree import MatFreeHamiltonian
 
     spec = _multilevel_spec(n, dim, seed=n)
     mf = MatFreeHamiltonian(spec)
     v = random_state(spec.hilbert_dim, n)
-    out = {}
-    for tiled in (1, 0):  # register-blocked tiled, generic
-        monkeypatch.setenv("PB200_TILED", str(tiled))
-        with engine.DevicePlan(spec) as plan:
-            out[tiled] = [plan.apply_h(t, v) for t in (0.0071, 0.0302)]
-    for i, t in enumerate((0.0071, 0.0302)):
-        ref = mf.apply(t, v)
-        scale = max(1.0, np.max(np.abs(ref)))
-        for tiled in (1, 0):
-            assert np.max(np.abs(out[tiled][i] - ref)) < 1e-12 * scale, tiled
+    with engine.DevicePlan(spec) as plan:
+        for t in (0.0071, 0.0302):
+            got = plan.apply_h(t, v)
+            ref = mf.apply(t, v)
+            assert np.max(np.abs(got - ref)) < 1e-12 * max(1.0, np.max(np.abs(ref)))
 
 
 def test_c4_noisy_trajectories_batch_vs_oracle(engine):
@@ -366,6 +405,8 @@ def test_krylov_integrator_vs_oracle(engine, builder):
         st = plan.propagate(0.0, spec.sampling_times[-1], integrator=2)
         got = plan.get_state()[0]
     assert st["integrator"] == 2 and st["n_applies"] > 0
+    # d = 2 below the 2^11 tile: stage_d2_kernel + dot2 + the separate vector update per iteration; d = 3: fused
+    assert st["n_launches"] == _krylov_launches(st, 3 if spec.dim == 2 else 1)
     assert np.max(np.abs(got - ref)) < STATE_TOL
     assert abs(np.linalg.norm(got) - 1.0) < 1e-9
 
@@ -390,10 +431,19 @@ def test_lanczos_needs_fewer_applies_on_blockaded_register(engine):
     assert out[2][0]["n_applies"] < out[1][0]["n_applies"]
 
 
+def _krylov_launches(st, per_apply):
+    """Kernel launches of a default (adaptive, extrapolated) Lanczos run without dissipator: per exponential dot2 +
+    normalize_copy + krylov_combine, `per_apply` per Lanczos iteration; per step one Richardson axpby, and a checked
+    step runs three extrapolated steps and one diffnorm2 (rejected steps included)."""
+    return (3 * st["n_exponentials"] + per_apply * st["n_applies"] + st["n_steps"] + st["n_rejected"]
+            + 3 * st["n_checks"])
+
+
 @pytest.mark.parametrize("kind", ["d2-uniform", "d2-batch", "d3", "d4-leak"])
-def test_fused_lanczos_equals_separate_update(engine, monkeypatch, kind):
+def test_fused_lanczos_one_launch_per_iteration(engine, kind):
     """The one-launch Lanczos iteration (normalisation / orthogonalisation folded into the next stage's own-element
-    operands, LanczosFuse in kernels.cuh) against the stage + vector-update pair and against the oracle."""
+    operands, LanczosFuse in kernels.cuh): one launch per iteration, and the oracle's state.  The stage + vector-update
+    pair runs below the register-blocked tile (test_krylov_integrator_vs_oracle)."""
     from oracle import evolve
 
     if kind == "d2-uniform":
@@ -407,18 +457,14 @@ def test_fused_lanczos_equals_separate_update(engine, monkeypatch, kind):
     first = spec[0] if isinstance(spec, list) else spec
     tf = first.sampling_times[-1]
     psi0 = evolve.all_ground_state(first)
-    out = {}
-    for fuse in (1, 0):
-        monkeypatch.setenv("PB200_LANCZOS_FUSE", str(fuse))
-        with engine.DevicePlan(spec) as plan:
-            plan.set_state("all-ground")
-            st = plan.propagate(0.0, tf, integrator=2)
-            out[fuse] = (plan.get_state().copy(), st)
-    assert out[1][1]["integrator"] == 2
-    assert np.max(np.abs(out[1][0] - out[0][0])) < 1e-10
-    assert out[1][1]["n_launches"] < out[0][1]["n_launches"]      # the update kernel is gone
+    with engine.DevicePlan(spec) as plan:
+        plan.set_state("all-ground")
+        st = plan.propagate(0.0, tf, integrator=2)
+        got = plan.get_state().copy()
+    assert st["integrator"] == 2
+    assert st["n_launches"] == _krylov_launches(st, 1)
     specs = spec if isinstance(spec, list) else [spec]
-    for g, s1 in zip(out[1][0], specs):
+    for g, s1 in zip(got, specs):
         assert np.max(np.abs(g - _oracle_final(s1, psi0))) < STATE_TOL
 
 
@@ -430,41 +476,30 @@ def _uniform_spec(kind, n):
     return W.ising_global_spec(W.disc_register(n, 38.0, 5.0, 3), W.C6_LEVEL_60, amp, det, phase=phase)
 
 
-@pytest.mark.parametrize("kind,n", [("real", 17), ("real", 20), ("real", 21), ("complex", 17), ("complex", 20)])
-def test_partner_sum_forwarding_equals_single_pass(engine, monkeypatch, kind, n):
-    """stage_d2_fwd_kernel (alternating tile geometries, forwarded partner sums) against the single-pass stage kernel
-    on the same Chebyshev chains: same H-applies, same launches, states equal to rounding.  N = 21 keeps one bit above
-    both geometries (coalesced partner loads in either)."""
+@pytest.mark.parametrize("kind,n", [("real", 17), ("complex", 17), ("real", 18), ("real", 19), ("complex", 19)])
+def test_partner_sum_forwarding_equals_single_pass(engine, kind, n):
+    """stage_d2_fwd_kernel (alternating tile geometries, forwarded partner sums; one state of uniform drives at
+    17 <= N <= 19) against the same spec as a batch of two identical trajectories, which runs the same Chebyshev chains
+    on the single-pass stage kernel: same H-applies, same launches, states equal to rounding.  At N = 17 it is also
+    held to the Lanczos path at a tight tolerance."""
     spec = _uniform_spec(kind, n)
     tf = spec.sampling_times[-1]
     psi0 = random_state(spec.hilbert_dim, 5)
     out = {}
-    monkeypatch.setenv("PB200_FWD_MAX_N", "30")   # the automatic rule keeps forwarding to 17 <= N <= 19
-    for fwd in (0, 1):
-        monkeypatch.setenv("PB200_FWD", str(fwd))
-        with engine.DevicePlan(spec) as plan:
+    for batch in ([spec], [spec, spec]):
+        with engine.DevicePlan(batch) as plan:
             plan.set_state(psi0)
             st = plan.propagate(0.0, tf, integrator=1)
-            out[fwd] = (plan.get_state()[0].copy(), st)
-    assert np.max(np.abs(out[0][0] - out[1][0])) < 5e-13
-    assert out[0][1]["n_applies"] == out[1][1]["n_applies"]
-    assert out[0][1]["n_launches"] == out[1][1]["n_launches"]  # one launch per stage either way
-
-
-def test_partner_sum_forwarding_vs_oracle(engine, monkeypatch):
-    """The forwarding path against the tight-tolerance oracle at the smallest register it is used on (N = 17 is
-    beyond the oracle: force it at N = 14)."""
-    from oracle import evolve
-
-    monkeypatch.setenv("PB200_FWD_MIN_N", "14")
-    spec = W.config_c2(n=14, seed=20, t_rise=100, t_sweep=300, t_fall=100)
-    psi0 = evolve.all_ground_state(spec)
-    ref = _oracle_final(spec, psi0)
-    with engine.DevicePlan(spec) as plan:
-        plan.set_state("all-ground")
-        plan.propagate(0.0, spec.sampling_times[-1], integrator=1)
-        got = plan.get_state()[0]
-    assert np.max(np.abs(got - ref)) < STATE_TOL
+            out[len(batch)] = (plan.get_state().copy(), st)
+    fwd, single = out[1][0][0], out[2][0]
+    assert np.max(np.abs(fwd - single[0])) < 5e-13 and np.max(np.abs(fwd - single[1])) < 5e-13
+    assert out[1][1]["n_applies"] == out[2][1]["n_applies"]
+    assert out[1][1]["n_launches"] == out[2][1]["n_launches"]  # one launch per stage either way
+    if n == 17:
+        with engine.DevicePlan(spec) as plan:
+            plan.set_state(psi0)
+            plan.propagate(0.0, tf, integrator=2, tol=1e-11)
+            assert np.max(np.abs(fwd - plan.get_state()[0])) < STATE_TOL
 
 
 # ---------------------------------------------------------------------------
