@@ -12,6 +12,7 @@
 
 #include <algorithm>
 #include <map>
+#include <memory>
 #include <mutex>
 #include <unordered_map>
 #include <cmath>
@@ -146,6 +147,49 @@ static void pool_free(int dev, void* p) {
     cudaFree(p);
 }
 
+struct Plan;
+
+// The one owner of a pool buffer, and the only caller of pool_alloc / pool_free.  The pool is not stream-ordered, so a
+// buffer goes back only once the stream that uses it is idle: release (destructor, reset, move-assignment) synchronises
+// the owning plan's `stream` field, read at that moment so that pb200_plan_set_stream is honoured.  Release also runs on
+// error exits, so a failed synchronisation is cleared, never thrown.
+template <typename T>
+class DevBuf {
+  public:
+    DevBuf() = default;
+    DevBuf(const Plan& P, size_t n) { reset(P, n); }
+    DevBuf(DevBuf&& o) noexcept : dev_(o.dev_), stream_(o.stream_), n_(o.n_), p_(o.p_) { o.p_ = nullptr; o.n_ = 0; }
+    DevBuf& operator=(DevBuf&& o) noexcept {
+        if (this != &o) {
+            release();
+            dev_ = o.dev_; stream_ = o.stream_; n_ = o.n_; p_ = o.p_;
+            o.p_ = nullptr; o.n_ = 0;
+        }
+        return *this;
+    }
+    DevBuf(const DevBuf&) = delete;
+    DevBuf& operator=(const DevBuf&) = delete;
+    ~DevBuf() { release(); }
+
+    // release the buffer, then take n elements on P's device, used by P's stream
+    void reset(const Plan& P, size_t n);
+    void release() noexcept {
+        if (!p_) return;
+        if (cudaStreamSynchronize(*stream_) != cudaSuccess) cudaGetLastError();
+        pool_free(dev_, p_);
+        p_ = nullptr; n_ = 0;
+    }
+    T* get() const { return p_; }
+    size_t size() const { return n_; }
+    explicit operator bool() const { return p_ != nullptr; }
+
+  private:
+    int dev_ = -1;
+    const cudaStream_t* stream_ = nullptr;
+    size_t n_ = 0;
+    T* p_ = nullptr;
+};
+
 // tile of the Taylor stage kernel: 2^13 amplitudes (128 KiB), one CTA of 512 threads per SM, 16 amplitudes per thread.
 // Measured on C2 (N = 20, H100): 44.1 us per order against 45.1 at 2^12 and 48.9 at 2^11, 42.9 with the evict-last
 // store of chi_{k+1} (DESIGN.md section 8).
@@ -201,17 +245,27 @@ struct Plan {
     long long D = 0;
     int n_drives = 0;
     cudaStream_t stream = nullptr;
-    bool own_stream = false;
+    // the stream the plan created (until pb200_plan_set_stream replaces it).  Declared before every DevBuf, so it is
+    // destroyed after them: their release synchronises `stream`
+    struct OwnedStream {
+        cudaStream_t s = nullptr;
+        OwnedStream() = default;
+        OwnedStream(const OwnedStream&) = delete;
+        OwnedStream& operator=(const OwnedStream&) = delete;
+        ~OwnedStream() { reset(); }
+        void reset() {
+            if (s) { cudaStreamSynchronize(s); cudaStreamDestroy(s); s = nullptr; }
+        }
+    } owned_stream;
     // device buffers
-    c2* buf[3] = {nullptr, nullptr, nullptr};
-    c2* aux[6] = {nullptr, nullptr, nullptr, nullptr, nullptr, nullptr};  // [0..3] chain pools, [4..5] check copies
+    DevBuf<c2> buf[3];
+    DevBuf<c2> aux[6];  // [0..3] chain pools, [4..5] check copies
     int cur = 0;  // index of the current state buffer
-    double* dint = nullptr;
+    DevBuf<double> dint;
     bool dint_shared = true;
     bool has_interaction = false;
-    double* d_table = nullptr;  // per-exponential coefficient tables
-    size_t d_table_cap = 0;
-    double* d_scratch = nullptr;  // bins for reductions
+    DevBuf<double> d_table;  // per-exponential coefficient tables
+    DevBuf<double> d_scratch;  // bins for reductions
     // host-side interpolants: [traj][drive]
     std::vector<std::vector<DriveTables>> tabs;
     std::vector<std::vector<bool>> tabs_set;
@@ -223,8 +277,8 @@ struct Plan {
     // Lindblad: per-qudit generators of the dissipator on the (row, column) digit pair
     std::vector<std::vector<cplx>> diss_gen;
     // Krylov (Lanczos) propagator workspace
-    c2* kry = nullptr; int kry_cap = 0;     // (kry_cap + 1) vectors of B*D
-    double* d_kry = nullptr;                // alpha[m][B], beta[m][B], acc[2][B][2], norm[B], y[B][m][2]
+    DevBuf<c2> kry; int kry_cap = 0;        // (kry_cap + 3) vectors of B*D
+    DevBuf<double> d_kry;                   // alpha[m][B], beta[m][B], acc[3][B][2], norm[B], y[B][m][2]
     int m_last = 8;
     bool use_krylov = false;
     long long kry_iters = 0;
@@ -236,12 +290,12 @@ struct Plan {
     bool jump_diag = true;                        // every L^+L is diagonal (decay = one elementwise kernel)
     bool has_collapse = false;
     // XY mode: exchange couplings on the device, their absolute row sums (spectral bound)
-    double* d_xy = nullptr; bool xy_shared = true; bool has_xy = false; int xy_u = 0, xy_d = 1;
+    DevBuf<double> d_xy; bool xy_shared = true; bool has_xy = false; int xy_u = 0, xy_d = 1;
     std::vector<double> xy_norm;  // per trajectory: sum_{i<j} |Uxy_ij| (pairs not touching the SLM mask)
     // XY mode with an SLM mask: the interaction of the pairs touching a masked qudit is weighted by the
     // interpolated 0/1 coefficient slm_coef(t) (hamiltonian.py:399-424)
     bool has_slm = false; unsigned long long slm_bits = 0; PiecewiseCubic<double> slm_coef;
-    double* dint2 = nullptr;                 // interaction diagonal of the pairs touching the mask
+    DevBuf<double> dint2;                    // interaction diagonal of the pairs touching the mask
     std::vector<double> xy_norm2, dmin2_traj, dmax2_traj;
     std::mt19937_64 rng;
     std::vector<double> thresholds;               // per trajectory
@@ -254,7 +308,7 @@ struct Plan {
     // of the high-bit tile [1] and of the later low-bit stages [2]; one buffer of forwarded sums per chain
     bool fwd_now = false;           // decided per propagate call
     PassGeom fwd_geo[3];
-    c2* wbuf[2] = {nullptr, nullptr};
+    DevBuf<c2> wbuf[2];
     // time-dependent Taylor propagator: drive projected on its constant phase, half-width of H at the sampling times,
     // extra ring buffers (beyond buf / aux) for polynomial degrees > 2
     struct TaylorCache {
@@ -270,9 +324,9 @@ struct Plan {
         std::vector<double> c;             // [B][N]
         double a_sum_max = 0.0, c_sum_max = 0.0;   // max over trajectories of sum_k |a|, sum_k |c|
         std::vector<double> tab_host;      // [B][3N+2] device table image
-        double* d_tab = nullptr;
+        DevBuf<double> d_tab;
     } tay;
-    std::vector<c2*> tay_ws;
+    std::vector<DevBuf<c2>> tay_ws;
     // state-vector shard (pb200_plan_create_shard): the top shard_bits qubits of the global index equal `shard`; n is
     // the global N, D = 2^(N - shard_bits) the slice this plan holds.  `group` = every shard, by index, once linked
     int shard_bits = 0, shard = 0;
@@ -284,6 +338,47 @@ struct Plan {
         return true;
     }
 };
+
+template <typename T>
+void DevBuf<T>::reset(const Plan& P, size_t n) {
+    release();
+    dev_ = P.desc.device;
+    stream_ = &P.stream;
+    p_ = static_cast<T*>(pool_alloc(dev_, sizeof(T) * n));
+    n_ = n;
+}
+
+// device sums: zero acc[0, n), queue the reduction kernels (`launch`), then copy the sums to `host` and wait for them.
+// sum_launch / sum_fetch split it where several streams reduce at once.
+template <typename F>
+static void sum_launch(const Plan& P, double* acc, size_t n, F&& launch) {
+    CUDA_CHECK(cudaMemsetAsync(acc, 0, sizeof(double) * n, P.stream));
+    launch();
+    CUDA_CHECK(cudaGetLastError());
+}
+
+static void sum_fetch(const Plan& P, const double* acc, size_t n, double* host) {
+    CUDA_CHECK(cudaMemcpyAsync(host, acc, sizeof(double) * n, cudaMemcpyDeviceToHost, P.stream));
+    CUDA_CHECK(cudaStreamSynchronize(P.stream));
+}
+
+template <typename F>
+static void device_sum(const Plan& P, double* acc, size_t n, double* host, F&& launch) {
+    sum_launch(P, acc, n, launch);
+    sum_fetch(P, acc, n, host);
+}
+
+// argument checks shared by the C-ABI entry points
+static void check_traj_range(const Plan& P, int traj0, int count, const char* who) {
+    if (traj0 < 0 || count < 1 || traj0 + count > P.B)
+        fail(PB200_ERR_INVALID, "%s: trajectory range [%d, %d) outside [0, %d)", who, traj0, traj0 + count, P.B);
+}
+
+static void check_drives_set(const Plan& P, const char* who) {
+    for (int tr = 0; tr < P.B; ++tr)
+        for (int q = 0; q < P.n_drives; ++q)
+            if (!P.tabs_set[tr][q]) fail(PB200_ERR_STATE, "%s: drive %d of trajectory %d not set", who, q, tr);
+}
 
 // launch with (optional) programmatic dependent launch: the kernel's prologue overlaps the tail of the
 // previous stage kernel; the kernel itself executes griddepcontrol.wait before its first global read
@@ -376,7 +471,7 @@ struct StageIO {  // one Clenshaw stage of one chain
 static StageArgs make_stage_args(const Plan& P, const PassGeom& geo, const StageIO& io, bool geo_is_last = true) {
     StageArgs a{};
     a.v = io.v; a.psi = io.psi; a.b2 = io.b2; a.out = io.out;
-    a.dint = P.has_interaction ? P.dint : nullptr;
+    a.dint = P.has_interaction ? P.dint.get() : nullptr;
     a.dint_stride = P.dint_shared ? 0 : P.D;
     a.D = P.D; a.geo = geo; a.coef = io.coef; a.u = io.ud; a.table = io.table;
     a.to_bit = P.desc.drives[0].state_to;
@@ -450,14 +545,14 @@ static void launch_stage_multi(Plan& P, const std::vector<PassGeom>& passes, con
         for (int c = 0; c < n; ++c) {
             GenArgs a{};
             a.v = io[c].v; a.psi = io[c].psi; a.b2 = io[c].b2; a.out = io[c].out;
-            a.dint = P.has_interaction ? P.dint : nullptr;
+            a.dint = P.has_interaction ? P.dint.get() : nullptr;
             a.dint_stride = P.dint_shared ? 0 : P.D;
             a.D = P.D; a.n = N; a.dim = P.dim; a.n_drives = P.n_drives;
             for (int q = 0; q < P.n_drives; ++q) { a.to[q] = P.desc.drives[q].state_to; a.from[q] = P.desc.drives[q].state_from; }
             a.coef = io[c].coef; a.table = io[c].table; a.beta_dev = io[c].beta_dev;
-            a.xy = P.has_xy ? P.d_xy : nullptr; a.xy_stride = P.xy_shared ? 0 : (long long)N * N;
+            a.xy = P.has_xy ? P.d_xy.get() : nullptr; a.xy_stride = P.xy_shared ? 0 : (long long)N * N;
             a.xy_u = P.xy_u; a.xy_d = P.xy_d;
-            a.slm_mask = P.has_slm ? P.slm_bits : 0ULL; a.dint2 = (P.has_slm && P.has_interaction) ? P.dint2 : nullptr;
+            a.slm_mask = P.has_slm ? P.slm_bits : 0ULL; a.dint2 = (P.has_slm && P.has_interaction) ? P.dint2.get() : nullptr;
             int threads = 256;
             if (multilevel_eligible(P)) {
                 a.dot_acc = io[c].dot_acc;
@@ -642,12 +737,8 @@ struct Program {  // a batch of exponentials prepared on the host
 };
 
 static void ensure_table_capacity(Plan& P, size_t doubles) {
-    if (doubles <= P.d_table_cap) return;
-    if (P.d_table) { CUDA_CHECK(cudaStreamSynchronize(P.stream)); pool_free(P.desc.device, P.d_table); }
-    P.d_table = nullptr;
-    size_t cap = std::max(doubles, (size_t)1 << 16);
-    P.d_table = (decltype(P.d_table))pool_alloc(P.desc.device, cap * sizeof(double));
-    P.d_table_cap = cap;
+    if (doubles <= P.d_table.size()) return;
+    P.d_table.reset(P, std::max(doubles, (size_t)1 << 16));
 }
 
 // One chain = a program (sequence of exponentials) applied to a state with its own buffers.  `next` emits
@@ -696,7 +787,7 @@ struct Chain {
         io.v = b1_buf; io.psi = psi; io.b2 = (b2_kind == 1) ? b2_buf : nullptr; io.out = out;
         io.coef = StageCoef{{cpsi.real(), cpsi.imag()}, {cb2.real(), cb2.imag()}, {cg.real(), cg.imag()}};
         io.ud = prog->ud[e];
-        io.table = uniform ? nullptr : P.d_table + table_base + prog->offset[e];
+        io.table = uniform ? nullptr : P.d_table.get() + table_base + prog->offset[e];
         io.real_g = prog->real_g[e] != 0;
         // partner-sum forwarding: this stage's geometry and whether a later stage of the chain consumes its sums
         io.fwd_role = !fwd_valid ? 0 : (fwd_parity ? 1 : 2);
@@ -731,7 +822,7 @@ static void run_chains(Plan& P, Chain* chains, int n, const std::vector<PassGeom
         ensure_table_capacity(P, total);
         for (int c = 0; c < n; ++c)
             if (!chains[c].prog->tables.empty())
-                CUDA_CHECK(cudaMemcpyAsync(P.d_table + chains[c].table_base, chains[c].prog->tables.data(),
+                CUDA_CHECK(cudaMemcpyAsync(P.d_table.get() + chains[c].table_base, chains[c].prog->tables.data(),
                                            chains[c].prog->tables.size() * sizeof(double), cudaMemcpyHostToDevice,
                                            P.stream));
     }
@@ -739,7 +830,7 @@ static void run_chains(Plan& P, Chain* chains, int n, const std::vector<PassGeom
     StageIO io[2];
     if (P.fwd_now)
         for (int c = 0; c < n; ++c)
-            if (!P.wbuf[c]) P.wbuf[c] = (c2*)pool_alloc(P.desc.device, sizeof(c2) * (size_t)P.D * P.B * 2);
+            if (!P.wbuf[c]) P.wbuf[c].reset(P, (size_t)P.D * P.B * 2);
     if (P.has_diss && n != 1) fail(PB200_ERR_STATE, "internal: Lindblad splitting runs one chain at a time");
     while (true) {
         int k = 0;
@@ -751,7 +842,7 @@ static void run_chains(Plan& P, Chain* chains, int n, const std::vector<PassGeom
                     if (chains[c].j < 0 && chains[c].prog->pre_diss[e_before] > 0.0)
                         apply_dissipator(P, chains[c].psi, chains[c].prog->pre_diss[e_before], launches);
                 }
-                io[k].wbuf = P.wbuf[c];
+                io[k].wbuf = P.wbuf[c].get();
                 chains[c].next(P, uniform, io[k++]);
             }
         if (k == 0) break;
@@ -827,13 +918,10 @@ static std::vector<cplx> tridiag_exp_e1(const double* alpha, const double* beta,
 
 static void ensure_krylov(Plan& P, int m_cap) {
     if (P.kry && P.kry_cap >= m_cap) return;
-    if (P.kry || P.d_kry) CUDA_CHECK(cudaStreamSynchronize(P.stream));
-    if (P.kry) { pool_free(P.desc.device, P.kry); P.kry = nullptr; }
-    if (P.d_kry) { pool_free(P.desc.device, P.d_kry); P.d_kry = nullptr; }
+    P.kry.release(); P.d_kry.release();
     // basis vectors V_0 .. V_{m_cap} and the two raw vectors of the fused recurrence
-    P.kry = (c2*)pool_alloc(P.desc.device, sizeof(c2) * (size_t)P.D * P.B * (m_cap + 3));
-    const size_t nd = (size_t)m_cap * P.B * 2 + (size_t)6 * P.B + P.B + (size_t)P.B * m_cap * 2;
-    P.d_kry = (double*)pool_alloc(P.desc.device, sizeof(double) * nd);
+    P.kry.reset(P, (size_t)P.D * P.B * (m_cap + 3));
+    P.d_kry.reset(P, (size_t)m_cap * P.B * 2 + (size_t)6 * P.B + P.B + (size_t)P.B * m_cap * 2);
     P.kry_cap = m_cap;
 }
 
@@ -858,7 +946,7 @@ static void krylov_exponential(Plan& P, const ExpParams& E, double tol, const st
     const int B = P.B;
     const long long D = P.D;
     const long long vstride = D * (long long)B;
-    double* d_alpha = P.d_kry;
+    double* d_alpha = P.d_kry.get();
     double* d_beta = d_alpha + (size_t)M * B;
     double* d_acc = d_beta + (size_t)M * B;   // [3][B][2]
     double* d_norm = d_acc + (size_t)6 * B;
@@ -870,7 +958,7 @@ static void krylov_exponential(Plan& P, const ExpParams& E, double tol, const st
     st.max_rho = std::max(st.max_rho, rh);
     if (!uniform) {
         ensure_table_capacity(P, host.size());
-        CUDA_CHECK(cudaMemcpyAsync(P.d_table, host.data(), host.size() * sizeof(double), cudaMemcpyHostToDevice, P.stream));
+        CUDA_CHECK(cudaMemcpyAsync(P.d_table.get(), host.data(), host.size() * sizeof(double), cudaMemcpyHostToDevice, P.stream));
     }
     UniformDrive ud{};
     ud.g = {E.g[0].real(), E.g[0].imag()}; ud.theta = E.th[0]; ud.w = E.w; ud.gamma = 0.0;
@@ -880,10 +968,10 @@ static void krylov_exponential(Plan& P, const ExpParams& E, double tol, const st
     // one launch per iteration: single-pass register-blocked d = 2 geometry, or the tiled d = 3 / 4 kernel
     const bool fused = (fused_dot && passes.size() == 1) || (!d2path && multilevel_eligible(P));
     if (fused) fused_dot = true;
-    c2* psi = P.buf[P.cur];
-    c2* outb = P.buf[(P.cur + 1) % 3];
-    c2* V = P.kry;                                  // V_j = V + j * vstride
-    c2* Rw[2] = {P.kry + (size_t)(M + 1) * vstride, P.kry + (size_t)(M + 2) * vstride};
+    c2* psi = P.buf[P.cur].get();
+    c2* outb = P.buf[(P.cur + 1) % 3].get();
+    c2* V = P.kry.get();                            // V_j = V + j * vstride
+    c2* Rw[2] = {V + (size_t)(M + 1) * vstride, V + (size_t)(M + 2) * vstride};
     auto acc = [&](int j) { return d_acc + (size_t)(((j % 3) + 3) % 3) * 2 * B; };
     const long long rblocks = std::min<long long>((D + 255) / 256, (long long)P.sm_count * 4);
     dim3 rgrid((unsigned)std::max<long long>(rblocks, 1), (unsigned)B);
@@ -901,7 +989,7 @@ static void krylov_exponential(Plan& P, const ExpParams& E, double tol, const st
         for (; j < m_check; ++j) {
             StageIO io{};
             io.coef = StageCoef{{0, 0}, {0, 0}, {1, 0}};
-            io.ud = ud; io.table = uniform ? nullptr : P.d_table; io.real_g = real_g;
+            io.ud = ud; io.table = uniform ? nullptr : P.d_table.get(); io.real_g = real_g;
             LanczosFuse lz{};
             if (fused) {
                 // stage j: raw r_j from raw r_{j-1} (j >= 1) or from v_0 (j = 0); materialises v_j
@@ -985,9 +1073,9 @@ static void krylov_exponential(Plan& P, const ExpParams& E, double tol, const st
 static void run_program_krylov(Plan& P, const Program& prog, const std::vector<PassGeom>& passes, pb200_run_stats& st) {
     long long launches = 0;
     for (size_t e = 0; e < prog.raw.size(); ++e) {
-        if (P.has_diss && prog.pre_diss[e] > 0.0) apply_dissipator(P, P.buf[P.cur], prog.pre_diss[e], launches);
+        if (P.has_diss && prog.pre_diss[e] > 0.0) apply_dissipator(P, P.buf[P.cur].get(), prog.pre_diss[e], launches);
         krylov_exponential(P, prog.raw[e], prog.ktol.empty() ? 1e-12 : prog.ktol[e], passes, st);
-        if (P.has_diss && prog.post_diss[e] > 0.0) apply_dissipator(P, P.buf[P.cur], prog.post_diss[e], launches);
+        if (P.has_diss && prog.post_diss[e] > 0.0) apply_dissipator(P, P.buf[P.cur].get(), prog.post_diss[e], launches);
     }
     st.n_launches += launches;
 }
@@ -998,12 +1086,12 @@ static void run_program(Plan& P, const Program& prog, const std::vector<PassGeom
     if (P.use_krylov) { run_program_krylov(P, prog, passes, st); return; }
     Chain ch;
     ch.prog = &prog;
-    ch.psi = P.buf[P.cur];
+    ch.psi = P.buf[P.cur].get();
     ch.psi_is_private = true;
-    for (int i = 0; i < 3; ++i) ch.pool[i] = P.buf[i];
+    for (int i = 0; i < 3; ++i) ch.pool[i] = P.buf[i].get();
     run_chains(P, &ch, 1, passes, st);
     for (int i = 0; i < 3; ++i)
-        if (P.buf[i] == ch.result()) P.cur = i;
+        if (P.buf[i].get() == ch.result()) P.cur = i;
 }
 
 // ---------------------------------------------------------------------------
@@ -1219,7 +1307,7 @@ static int jump_substeps(const Plan& P, double a, double b, double magnus_tol) {
 
 static void ensure_aux_buffers(Plan& P) {
     for (int i = 0; i < 6; ++i)
-        if (!P.aux[i]) P.aux[i] = (c2*)pool_alloc(P.desc.device, sizeof(c2) * (size_t)P.D * P.B);
+        if (!P.aux[i]) P.aux[i].reset(P, (size_t)P.D * P.B);
 }
 
 // ---- Monte-Carlo wave-function propagation (collapse operators without a density matrix) ------------------------
@@ -1247,17 +1335,13 @@ static void propagate_mcwf(Plan& P, double t_start, double t_stop, const pb200_r
     cudaEvent_t ev0 = evs.a, ev1 = evs.b;
     CUDA_CHECK(cudaEventRecord(ev0, P.stream));
     std::vector<double> norms(P.B), occ((size_t)P.dim * P.n);
-    double* d_occ = nullptr;
-    d_occ = (decltype(d_occ))pool_alloc(P.desc.device, sizeof(double) * P.n);
+    DevBuf<double> d_occ(P, (size_t)P.dim * P.n);   // populations [digit][qudit]
     std::uniform_real_distribution<double> uni(0.0, 1.0);
     auto norms2 = [&]() {
-        CUDA_CHECK(cudaMemsetAsync(P.d_scratch, 0, sizeof(double) * P.B, P.stream));
         const long long nb = std::min<long long>((P.D + 255) / 256, (long long)P.sm_count * 4);
         dim3 grid((unsigned)std::max<long long>(nb, 1), (unsigned)P.B);
-        norm2_kernel<<<grid, 256, 0, P.stream>>>(P.buf[P.cur], P.D, P.d_scratch);
-        CUDA_CHECK(cudaGetLastError());
-        CUDA_CHECK(cudaMemcpyAsync(norms.data(), P.d_scratch, sizeof(double) * P.B, cudaMemcpyDeviceToHost, P.stream));
-        CUDA_CHECK(cudaStreamSynchronize(P.stream));
+        device_sum(P, P.d_scratch.get(), P.B, norms.data(),
+                   [&] { norm2_kernel<<<grid, 256, 0, P.stream>>>(P.buf[P.cur].get(), P.D, P.d_scratch.get()); });
         st.n_launches += 1;
     };
     // K_tot = sum_c L_c^+ L_c (d x d): its norm bounds the jump rate per qudit
@@ -1275,7 +1359,7 @@ static void propagate_mcwf(Plan& P, double t_start, double t_stop, const pb200_r
     // d x d matrix exp(-tau K_tot) applied to each qudit in turn (general effective-noise operators)
     auto decay = [&](double tau) {
         if (P.jump_diag) {
-            mcwf_decay_kernel<<<bgrid, 256, 0, P.stream>>>(P.buf[P.cur], P.D, P.n, P.dim, tau, dt);
+            mcwf_decay_kernel<<<bgrid, 256, 0, P.stream>>>(P.buf[P.cur].get(), P.D, P.n, P.dim, tau, dt);
             st.n_launches += 1;
             return;
         }
@@ -1288,7 +1372,7 @@ static void propagate_mcwf(Plan& P, double t_start, double t_stop, const pb200_r
         long long stq = 1;
         for (int k = P.n - 1; k >= 0; --k) {  // qudit k has stride d^(n-1-k)
             qudit_op_kernel<<<dim3((unsigned)std::max<long long>(nb, 1), (unsigned)P.B), 256, 0, P.stream>>>(
-                P.buf[P.cur], P.D, d, stq, 1.0, qo);
+                P.buf[P.cur].get(), P.D, d, stq, 1.0, qo);
             stq *= d;
         }
         st.n_launches += P.n;
@@ -1322,7 +1406,7 @@ static void propagate_mcwf(Plan& P, double t_start, double t_stop, const pb200_r
         norms2();
         for (int tr = 0; tr < P.B; ++tr) {
             if (norms[tr] > P.thresholds[tr]) continue;
-            c2* psi = P.buf[P.cur] + (size_t)tr * P.D;
+            c2* psi = P.buf[P.cur].get() + (size_t)tr * P.D;
             std::vector<double> wts(P.jump_ops.size() * (size_t)P.n);
             double tot = 0.0;
             if (!P.jump_diag) {
@@ -1331,11 +1415,10 @@ static void propagate_mcwf(Plan& P, double t_start, double t_stop, const pb200_r
                 const long long nbq = std::min<long long>((P.D / d + 255) / 256, (long long)P.sm_count * 4);
                 long long stq = 1;
                 for (int k = P.n - 1; k >= 0; --k) {
-                    CUDA_CHECK(cudaMemsetAsync(P.d_scratch, 0, sizeof(double) * 2 * d * d, P.stream));
-                    reduced_density_kernel<<<(unsigned)std::max<long long>(nbq, 1), 256, 0, P.stream>>>(psi, P.D, d, stq, P.d_scratch);
-                    CUDA_CHECK(cudaGetLastError());
-                    CUDA_CHECK(cudaMemcpyAsync(hr.data(), P.d_scratch, sizeof(double) * 2 * d * d, cudaMemcpyDeviceToHost, P.stream));
-                    CUDA_CHECK(cudaStreamSynchronize(P.stream));
+                    device_sum(P, P.d_scratch.get(), hr.size(), hr.data(), [&] {
+                        reduced_density_kernel<<<(unsigned)std::max<long long>(nbq, 1), 256, 0, P.stream>>>(psi, P.D, d, stq,
+                                                                                                           P.d_scratch.get());
+                    });
                     for (size_t op = 0; op < P.jump_ops.size(); ++op) {
                         cplx tr_k = 0.0;
                         for (int a = 0; a < d; ++a)
@@ -1349,14 +1432,14 @@ static void propagate_mcwf(Plan& P, double t_start, double t_stop, const pb200_r
                 st.n_launches += P.n;
             }
             // populations of every digit on every qudit
-            for (int dgt = 0; P.jump_diag && dgt < P.dim; ++dgt) {
-                CUDA_CHECK(cudaMemsetAsync(d_occ, 0, sizeof(double) * P.n, P.stream));
+            if (P.jump_diag) {
                 const long long nb = std::min<long long>((P.D + 255) / 256, (long long)P.sm_count * 4);
-                occupation_kernel<<<(unsigned)std::max<long long>(nb, 1), 256, sizeof(double) * P.n, P.stream>>>(
-                    psi, d_occ, P.D, P.n, P.dim, dgt, 0LL);
-                CUDA_CHECK(cudaMemcpyAsync(occ.data() + (size_t)dgt * P.n, d_occ, sizeof(double) * P.n, cudaMemcpyDeviceToHost, P.stream));
+                device_sum(P, d_occ.get(), occ.size(), occ.data(), [&] {
+                    for (int dgt = 0; dgt < P.dim; ++dgt)
+                        occupation_kernel<<<(unsigned)std::max<long long>(nb, 1), 256, sizeof(double) * P.n, P.stream>>>(
+                            psi, d_occ.get() + (size_t)dgt * P.n, P.D, P.n, P.dim, dgt, 0LL);
+                });
             }
-            CUDA_CHECK(cudaStreamSynchronize(P.stream));
             // channel (op, qudit) with probability <L^+L>
             for (size_t op = 0; P.jump_diag && op < P.jump_ops.size(); ++op)
                 for (int k = 0; k < P.n; ++k) {
@@ -1387,12 +1470,11 @@ static void propagate_mcwf(Plan& P, double t_start, double t_stop, const pb200_r
     for (int tr = 0; tr < P.B; ++tr) {
         if (norms[tr] <= 0.0) continue;
         const double sc = 1.0 / std::sqrt(norms[tr]);
-        scale_kernel<<<(unsigned)std::max<long long>(blocks, 1), 256, 0, P.stream>>>(P.buf[P.cur] + (size_t)tr * P.D, P.D, sc);
+        scale_kernel<<<(unsigned)std::max<long long>(blocks, 1), 256, 0, P.stream>>>(P.buf[P.cur].get() + (size_t)tr * P.D, P.D, sc);
         P.thresholds[tr] /= norms[tr];  // the same decay continues from the rescaled state
         P.thresholds[tr] = std::min(P.thresholds[tr], 1.0);
     }
     CUDA_CHECK(cudaGetLastError());
-    pool_free(P.desc.device, d_occ);
     CUDA_CHECK(cudaEventRecord(ev1, P.stream));
     CUDA_CHECK(cudaEventSynchronize(ev1));
     float ms = 0.f;
@@ -1409,9 +1491,7 @@ static void propagate_taylor(Plan& P, double t_start, double t_stop, const pb200
 
 static void propagate(Plan& P, double t_start, double t_stop, const pb200_run_opts* o, pb200_run_stats* stats) {
     if (!P.state_set) fail(PB200_ERR_STATE, "pb200_propagate: no state set (call pb200_state_set first)");
-    for (int tr = 0; tr < P.B; ++tr)
-        for (int q = 0; q < P.n_drives; ++q)
-            if (!P.tabs_set[tr][q]) fail(PB200_ERR_STATE, "pb200_propagate: drive %d of trajectory %d not set", q, tr);
+    check_drives_set(P, "pb200_propagate");
     const double tlo = P.times.front(), thi = P.times.back();
     const double eps = 1e-12;
     if (t_start < tlo - eps || t_stop > thi + eps || t_stop < t_start)
@@ -1493,19 +1573,16 @@ static void propagate(Plan& P, double t_start, double t_stop, const pb200_run_op
     };
     const size_t flush_doubles = (size_t)8 << 20;  // 64 MiB of tables per chunk
     const size_t state_bytes = sizeof(c2) * (size_t)P.D * P.B;
-    auto copy_state = [&](c2* dst, const c2* src) {
-        CUDA_CHECK(cudaMemcpyAsync(dst, src, state_bytes, cudaMemcpyDeviceToDevice, P.stream));
+    auto copy_state = [&](const DevBuf<c2>& dst, const DevBuf<c2>& src) {
+        CUDA_CHECK(cudaMemcpyAsync(dst.get(), src.get(), state_bytes, cudaMemcpyDeviceToDevice, P.stream));
     };
-    auto max_diff2 = [&](const c2* x, const c2* y) {
+    auto max_diff2 = [&](const DevBuf<c2>& x, const DevBuf<c2>& y) {
         const int nb = std::min(P.B, 4096);
-        CUDA_CHECK(cudaMemsetAsync(P.d_scratch, 0, sizeof(double) * nb, P.stream));
         const long long blocks = std::min<long long>((P.D + 255) / 256, (long long)P.sm_count * 4);
         dim3 grid((unsigned)std::max<long long>(blocks, 1), (unsigned)nb);
-        diffnorm2_kernel<<<grid, 256, 0, P.stream>>>(x, y, P.D, P.d_scratch);
-        CUDA_CHECK(cudaGetLastError());
         std::vector<double> d2(nb);
-        CUDA_CHECK(cudaMemcpyAsync(d2.data(), P.d_scratch, sizeof(double) * nb, cudaMemcpyDeviceToHost, P.stream));
-        CUDA_CHECK(cudaStreamSynchronize(P.stream));
+        device_sum(P, P.d_scratch.get(), nb, d2.data(),
+                   [&] { diffnorm2_kernel<<<grid, 256, 0, P.stream>>>(x.get(), y.get(), P.D, P.d_scratch.get()); });
         st.n_launches += 1;
         double e = 0.0;
         for (double v : d2) e = std::max(e, v);
@@ -1558,10 +1635,10 @@ static void propagate(Plan& P, double t_start, double t_stop, const pb200_run_op
             add_step(P, big, a, b2, order, ctol);
             add_step(P, half, a, mid, order, ctol);
             add_step(P, half, mid, b2, order, ctol);
-            c2* X = P.buf[P.cur];
+            c2* X = P.buf[P.cur].get();
             c2* others[6]; int k = 0;
-            for (int i = 0; i < 3; ++i) if (i != P.cur) others[k++] = P.buf[i];
-            for (int i = 0; i < 4; ++i) others[k++] = P.aux[i];
+            for (int i = 0; i < 3; ++i) if (i != P.cur) others[k++] = P.buf[i].get();
+            for (int i = 0; i < 4; ++i) others[k++] = P.aux[i].get();
             Chain ch[2];
             ch[0].prog = &half; ch[0].psi = X; for (int i = 0; i < 3; ++i) ch[0].pool[i] = others[i];
             ch[1].prog = &big;  ch[1].psi = X; for (int i = 0; i < 3; ++i) ch[1].pool[i] = others[3 + i];
@@ -1570,11 +1647,11 @@ static void propagate(Plan& P, double t_start, double t_stop, const pb200_run_op
             axpby_kernel<<<(unsigned)nb, 256, 0, P.stream>>>(res, ch[1].result(), 1.0 + 1.0 / sc, -1.0 / sc, total);
             CUDA_CHECK(cudaGetLastError());
             st.n_launches += 1;
-            // make `res` the current state buffer (swap pointer slots if it lives in the aux set)
+            // make `res` the current state buffer (swap handles if it lives in the aux set)
             bool found = false;
-            for (int i = 0; i < 3; ++i) if (P.buf[i] == res) { P.cur = i; found = true; }
+            for (int i = 0; i < 3; ++i) if (P.buf[i].get() == res) { P.cur = i; found = true; }
             if (!found)
-                for (int i = 0; i < 4; ++i) if (P.aux[i] == res) { std::swap(P.aux[i], P.buf[P.cur]); break; }
+                for (int i = 0; i < 4; ++i) if (P.aux[i].get() == res) { std::swap(P.aux[i], P.buf[P.cur]); break; }
             if (!(is_d2path(P) && P.all_uniform() && P.B == 1))
                 CUDA_CHECK(cudaStreamSynchronize(P.stream));  // tables of big/half were uploaded from this scope
             return;
@@ -1587,7 +1664,7 @@ static void propagate(Plan& P, double t_start, double t_stop, const pb200_run_op
         add_step(P, prog, a, mid, order, ctol);
         add_step(P, prog, mid, b2, order, ctol);
         flush();
-        axpby_kernel<<<(unsigned)nb, 256, 0, P.stream>>>(P.buf[P.cur], P.aux[1], 1.0 + 1.0 / sc, -1.0 / sc, total);
+        axpby_kernel<<<(unsigned)nb, 256, 0, P.stream>>>(P.buf[P.cur].get(), P.aux[1].get(), 1.0 + 1.0 / sc, -1.0 / sc, total);
         CUDA_CHECK(cudaGetLastError());
         st.n_launches += 1;
     };
@@ -1899,9 +1976,8 @@ static bool taylor_prepare(Plan& P) {
                 t[2 * N + p] = C.c[(size_t)b * N + k];
             }
         }
-        if (C.d_tab) { CUDA_CHECK(cudaStreamSynchronize(P.stream)); pool_free(P.desc.device, C.d_tab); C.d_tab = nullptr; }
-        C.d_tab = (double*)pool_alloc(P.desc.device, C.tab_host.size() * sizeof(double));
-        CUDA_CHECK(cudaMemcpyAsync(C.d_tab, C.tab_host.data(), C.tab_host.size() * sizeof(double), cudaMemcpyHostToDevice,
+        C.d_tab.reset(P, C.tab_host.size());
+        CUDA_CHECK(cudaMemcpyAsync(C.d_tab.get(), C.tab_host.data(), C.tab_host.size() * sizeof(double), cudaMemcpyHostToDevice,
                                    P.stream));
     }
     C.w_knot.clear();
@@ -2320,19 +2396,19 @@ struct TaylorScheduler {
 // aux buffers too when the plan has them), then the plan's own Taylor work buffers, allocated on first need.
 struct TaylorRing {
     std::vector<c2*> chi, gr;
-    c2** acc_slot = nullptr;
+    DevBuf<c2>* acc_slot = nullptr;
 };
 
 static void taylor_grow_ring(Plan& P, int need) {
     int have = 2 + (P.aux[0] ? 6 : 0) + (int)P.tay_ws.size();
     while (have < need) {
-        P.tay_ws.push_back((c2*)pool_alloc(P.desc.device, sizeof(c2) * (size_t)P.D * P.B));
+        P.tay_ws.emplace_back(P, (size_t)P.D * P.B);
         ++have;
     }
 }
 
 static TaylorRing taylor_ring(Plan& P, const TaylorStep& s) {
-    std::vector<c2**> free_slots;
+    std::vector<DevBuf<c2>*> free_slots;
     for (int i = 0; i < 3; ++i) if (i != P.cur) free_slots.push_back(&P.buf[i]);
     if (P.aux[0]) for (int i = 0; i < 6; ++i) free_slots.push_back(&P.aux[i]);
     taylor_grow_ring(P, s.ring());
@@ -2340,9 +2416,9 @@ static TaylorRing taylor_ring(Plan& P, const TaylorStep& s) {
     TaylorRing R;
     R.chi.resize(s.n_chi); R.gr.resize(s.n_g);
     int fs = 0;
-    R.chi[0] = P.buf[P.cur];
-    for (int i = 1; i < s.n_chi; ++i) R.chi[i] = *free_slots[fs++];
-    for (int i = 0; i < s.n_g; ++i) R.gr[i] = *free_slots[fs++];
+    R.chi[0] = P.buf[P.cur].get();
+    for (int i = 1; i < s.n_chi; ++i) R.chi[i] = free_slots[fs++]->get();
+    for (int i = 0; i < s.n_g; ++i) R.gr[i] = free_slots[fs++]->get();
     R.acc_slot = free_slots[fs++];
     return R;
 }
@@ -2355,13 +2431,13 @@ static TaylorArgs taylor_args(const Plan& P, const PassGeom& geo, const TaylorSt
     TaylorArgs a{};
     a.v = R.chi[k % s.n_chi]; a.out = R.chi[(k + 1) % s.n_chi];
     a.g_out = (s.n_g && k + 1 < s.K) ? R.gr[k % s.n_g] : nullptr;
-    a.acc = *R.acc_slot;
-    a.dint = P.has_interaction ? P.dint : nullptr;
+    a.acc = R.acc_slot->get();
+    a.dint = P.has_interaction ? P.dint.get() : nullptr;
     a.dint_stride = P.dint_shared ? 0 : P.D;
     a.D = P.D;
     a.geo = geo;
     a.unit = C.unit;
-    a.table = C.uniform ? nullptr : C.d_tab;
+    a.table = C.uniform ? nullptr : C.d_tab.get();
     a.to_bit = P.desc.drives[0].state_to; a.from_is_one = P.desc.drives[0].state_from;
     a.th0 = s.th[0]; a.gam0 = s.gam[0]; a.om0 = s.om[0]; a.m0 = m_c(0);
     a.scale = {0.0, -s.h / (k + 1)};
@@ -2457,13 +2533,13 @@ static void apply_h_device(Plan& P, double t, const c2* in, c2* out, long long& 
         }
     }
     ensure_table_capacity(P, host.size());
-    CUDA_CHECK(cudaMemcpyAsync(P.d_table, host.data(), host.size() * sizeof(double), cudaMemcpyHostToDevice, P.stream));
+    CUDA_CHECK(cudaMemcpyAsync(P.d_table.get(), host.data(), host.size() * sizeof(double), cudaMemcpyHostToDevice, P.stream));
     CUDA_CHECK(cudaStreamSynchronize(P.stream));
     UniformDrive ud{};
     ud.g = {E.g[0].real(), E.g[0].imag()}; ud.theta = E.th[0]; ud.w = 1.0; ud.gamma = 0.0;
     StageCoef sc{{0, 0}, {0, 0}, {1, 0}};
     const std::vector<PassGeom> passes = plan_passes(P.n, kStageTileBits, kMaxExtraBits);
-    launch_stage(P, passes, in, nullptr, nullptr, out, sc, uniform, E.g[0].imag() == 0.0, ud, P.d_table, launches);
+    launch_stage(P, passes, in, nullptr, nullptr, out, sc, uniform, E.g[0].imag() == 0.0, ud, P.d_table.get(), launches);
     CUDA_CHECK(cudaGetLastError());
 }
 
@@ -2558,7 +2634,7 @@ static void shards_apply_h(const std::vector<Plan*>& G, double t, const std::vec
         Plan& P = *G[r];
         TaylorArgs a{};
         a.v = in[r]; a.out = out[r];
-        a.dint = P.has_interaction ? P.dint : nullptr;
+        a.dint = P.has_interaction ? P.dint.get() : nullptr;
         a.D = P.D; a.geo = geo; a.unit = P.tay.unit;
         a.to_bit = P.desc.drives[0].state_to; a.from_is_one = P.desc.drives[0].state_from;
         a.th0 = th; a.om0 = om;
@@ -2701,44 +2777,29 @@ static ExpHost exp_host(const pb200_op_terms* op, int n, int dim, int local_bits
     return dim == 2 ? exp_host_d2(op, n, local_bits) : exp_host_general(op, n, dim);
 }
 
-// the device copy of an ExpHost on one plan's device.  The pool buffer is released on every exit path, once the plan's
-// stream is idle: the pool is not stream-ordered, and on an error exit a kernel reading the table may still be queued
-struct ExpTable {
-    int dev = -1;
-    cudaStream_t stream = nullptr;
-    char* buf = nullptr;
-    ExpTable() = default;
-    ExpTable(const ExpTable&) = delete;
-    ExpTable& operator=(const ExpTable&) = delete;
-    ~ExpTable() {
-        if (!buf) return;
-        if (cudaStreamSynchronize(stream) != cudaSuccess) cudaGetLastError();
-        pool_free(dev, buf);
-    }
-    void upload(const ExpHost& H, const Plan& P) {
-        dev = P.desc.device;
-        stream = P.stream;
-        buf = (char*)pool_alloc(dev, H.img.size());
-        CUDA_CHECK(cudaMemcpyAsync(buf, H.img.data(), H.img.size(), cudaMemcpyHostToDevice, P.stream));
-    }
-};
+// the device copy of an ExpHost on one plan's device
+static DevBuf<char> upload_exp(const ExpHost& H, const Plan& P) {
+    DevBuf<char> X(P, H.img.size());
+    CUDA_CHECK(cudaMemcpyAsync(X.get(), H.img.data(), H.img.size(), cudaMemcpyHostToDevice, P.stream));
+    return X;
+}
 
-// acc[2 c] += <psi_c| op |psi_c> for `count` trajectories; src.p[src.shard] + c D is trajectory c (d = 2), psi (d > 2)
-static void launch_expect(const Plan& P, const ExpHost& H, const ExpTable& X, const ExpSrc& src, const c2* psi, int count,
+// acc[2 c] += <psi_c| op |psi_c> for `count` trajectories; src.p[src.shard] + c D is trajectory c (d = 2), psi (d > 2);
+// X = the device copy of H
+static void launch_expect(const Plan& P, const ExpHost& H, const char* X, const ExpSrc& src, const c2* psi, int count,
                           double* d_acc) {
     const long long blocks = std::min<long long>((P.D + 255) / 256, (long long)P.sm_count * 8);
     const dim3 grid((unsigned)std::max<long long>(blocks, 1), (unsigned)count);
-    const int* ct = reinterpret_cast<const int*>(X.buf + H.off_ct);
-    const int* cs = reinterpret_cast<const int*>(X.buf + H.off_cs);
+    const int* ct = reinterpret_cast<const int*>(X + H.off_ct);
+    const int* cs = reinterpret_cast<const int*>(X + H.off_cs);
     if (H.d2)
-        expect_terms_d2_kernel<<<grid, 256, 0, P.stream>>>(src, P.D, reinterpret_cast<const ExpD2Term*>(X.buf),
-                                                           reinterpret_cast<const ExpGenSite*>(X.buf + H.off_sites), ct, cs,
+        expect_terms_d2_kernel<<<grid, 256, 0, P.stream>>>(src, P.D, reinterpret_cast<const ExpD2Term*>(X),
+                                                           reinterpret_cast<const ExpGenSite*>(X + H.off_sites), ct, cs,
                                                            H.n_chunks, d_acc);
     else
-        expect_terms_kernel<<<grid, 256, 0, P.stream>>>(psi, P.D, P.dim, reinterpret_cast<const ExpTerm*>(X.buf),
-                                                        reinterpret_cast<const ExpSite*>(X.buf + H.off_sites), ct, cs,
+        expect_terms_kernel<<<grid, 256, 0, P.stream>>>(psi, P.D, P.dim, reinterpret_cast<const ExpTerm*>(X),
+                                                        reinterpret_cast<const ExpSite*>(X + H.off_sites), ct, cs,
                                                         H.n_chunks, d_acc);
-    CUDA_CHECK(cudaGetLastError());
 }
 
 #define PB200_TRY try {
@@ -2796,7 +2857,7 @@ static void create_plan(pb200_plan** out, const pb200_plan_desc* d, int shard_bi
     }
     if (d->device < 0 || d->device >= ndev) fail(PB200_ERR_INVALID, "device ordinal %d out of range", d->device);
     CUDA_CHECK(cudaSetDevice(d->device));
-    pb200_plan* h = new pb200_plan();
+    std::unique_ptr<pb200_plan> h(new pb200_plan());
     Plan& P = h->p;
     P.desc = *d;
     P.times.assign(d->sampling_times, d->sampling_times + d->n_times);
@@ -2808,19 +2869,14 @@ static void create_plan(pb200_plan** out, const pb200_plan_desc* d, int shard_bi
     P.D = D;
     P.shard_bits = shard_bits; P.shard = shard;
     P.sm_count = device_setup(d->device);
-    try {
-        CUDA_CHECK(cudaStreamCreateWithFlags(&P.stream, cudaStreamNonBlocking));
-        P.own_stream = true;
-        for (int i = 0; i < 3; ++i) P.buf[i] = (c2*)pool_alloc(d->device, sizeof(c2) * (size_t)D * P.B);
-        P.d_scratch = (double*)pool_alloc(d->device, sizeof(double) * 4096);
-    } catch (...) {
-        pb200_plan_destroy(h);
-        throw;
-    }
+    CUDA_CHECK(cudaStreamCreateWithFlags(&P.owned_stream.s, cudaStreamNonBlocking));
+    P.stream = P.owned_stream.s;
+    for (int i = 0; i < 3; ++i) P.buf[i].reset(P, (size_t)D * P.B);
+    P.d_scratch.reset(P, 4096);
     P.tabs.assign(P.B, std::vector<DriveTables>(P.n_drives));
     P.tabs_set.assign(P.B, std::vector<bool>(P.n_drives, false));
     P.has_interaction = false;
-    *out = h;
+    *out = h.release();
 }
 
 int pb200_plan_create(pb200_plan** out, const pb200_plan_desc* d) {
@@ -2857,24 +2913,10 @@ int pb200_plan_create_shard(pb200_plan** out, const pb200_plan_desc* d, int32_t 
 int pb200_plan_destroy(pb200_plan* h) {
     if (!h) return PB200_OK;
     Plan& P = h->p;
-    const int dev = P.desc.device;
     for (Plan* m : P.group)   // the other shards of a linked group are unlinked
         if (m != &P) m->group.clear();
-    cudaSetDevice(dev);
-    if (P.stream) cudaStreamSynchronize(P.stream);  // nothing may still be using the buffers that go back to the pool
-    for (int i = 0; i < 3; ++i) pool_free(dev, P.buf[i]);
-    for (int i = 0; i < 6; ++i) pool_free(dev, P.aux[i]);
-    pool_free(dev, P.d_xy);
-    pool_free(dev, P.dint2);
-    pool_free(dev, P.kry);
-    pool_free(dev, P.d_kry);
-    pool_free(dev, P.dint);
-    pool_free(dev, P.d_table);
-    pool_free(dev, P.d_scratch);
-    for (int i = 0; i < 2; ++i) pool_free(dev, P.wbuf[i]);
-    for (c2* w : P.tay_ws) pool_free(dev, w);
-    pool_free(dev, P.tay.d_tab);
-    if (P.own_stream && P.stream) cudaStreamDestroy(P.stream);
+    cudaSetDevice(P.desc.device);
+    if (P.stream) cudaStreamSynchronize(P.stream);  // once: every buffer then returns to the pool without waiting
     delete h;
     return PB200_OK;
 }
@@ -2884,8 +2926,8 @@ int pb200_plan_set_stream(pb200_plan* h, void* s) {
     if (!h) fail(PB200_ERR_INVALID, "null plan");
     Plan& P = h->p;
     if (s) {
-        if (P.own_stream && P.stream) { cudaStreamSynchronize(P.stream); cudaStreamDestroy(P.stream); }
-        P.stream = (cudaStream_t)s; P.own_stream = false;
+        P.owned_stream.reset();
+        P.stream = (cudaStream_t)s;
     }
     PB200_CATCH
 }
@@ -2898,27 +2940,24 @@ int pb200_plan_set_interaction(pb200_plan* h, int32_t traj0, int32_t count, cons
     Plan& P = h->p;
     if (P.desc.rydberg_state < 0) fail(PB200_ERR_INVALID, "plan has no interaction term (rydberg_state < 0)");
     if (shared && (count != 1 || traj0 != 0)) fail(PB200_ERR_INVALID, "shared interaction: traj0 = 0, count = 1");
-    if (!shared && (traj0 < 0 || count < 1 || traj0 + count > P.B)) fail(PB200_ERR_INVALID, "trajectory range");
+    if (!shared) check_traj_range(P, traj0, count, "pb200_plan_set_interaction");
     CUDA_CHECK(cudaSetDevice(P.desc.device));
     const int N = P.n;
     const bool want_shared = shared != 0;
-    if (P.dint && P.dint_shared != want_shared) { CUDA_CHECK(cudaStreamSynchronize(P.stream)); pool_free(P.desc.device, P.dint); P.dint = nullptr; }
-    if (!P.dint) {
-        P.dint = (decltype(P.dint))pool_alloc(P.desc.device, sizeof(double) * (size_t)P.D * (want_shared ? 1 : P.B));
-        if (!want_shared) CUDA_CHECK(cudaMemsetAsync(P.dint, 0, sizeof(double) * (size_t)P.D * P.B, P.stream));
+    if (!P.dint || P.dint_shared != want_shared) {
+        P.dint.reset(P, (size_t)P.D * (want_shared ? 1 : P.B));
+        if (!want_shared) CUDA_CHECK(cudaMemsetAsync(P.dint.get(), 0, sizeof(double) * (size_t)P.D * P.B, P.stream));
     }
     P.dint_shared = want_shared;
     P.dmin_traj.resize(want_shared ? 1 : P.B, 0.0);
     P.dmax_traj.resize(want_shared ? 1 : P.B, 0.0);
     if (P.has_slm) {
-        if (P.dint2) { CUDA_CHECK(cudaStreamSynchronize(P.stream)); pool_free(P.desc.device, P.dint2); P.dint2 = nullptr; }
-        P.dint2 = (decltype(P.dint2))pool_alloc(P.desc.device, sizeof(double) * (size_t)P.D * (want_shared ? 1 : P.B));
-        CUDA_CHECK(cudaMemsetAsync(P.dint2, 0, sizeof(double) * (size_t)P.D * (want_shared ? 1 : P.B), P.stream));
+        P.dint2.reset(P, (size_t)P.D * (want_shared ? 1 : P.B));
+        CUDA_CHECK(cudaMemsetAsync(P.dint2.get(), 0, sizeof(double) * (size_t)P.D * (want_shared ? 1 : P.B), P.stream));
         P.dmin2_traj.assign(want_shared ? 1 : P.B, 0.0);
         P.dmax2_traj.assign(want_shared ? 1 : P.B, 0.0);
     }
-    double* dU = nullptr;
-    dU = (decltype(dU))pool_alloc(P.desc.device, sizeof(double) * N * N);
+    DevBuf<double> dU(P, (size_t)N * N);
     std::vector<double> Uc((size_t)N * N);
     // part 0: pairs weighted by w (all pairs, or the pairs not touching the SLM mask); part 1: the pairs touching it
     for (int c = 0; c < count; ++c)
@@ -2935,22 +2974,24 @@ int pb200_plan_set_interaction(pb200_plan* h, int32_t traj0, int32_t count, cons
                 }
                 Uc[(size_t)i * N + j] = u;
             }
-        CUDA_CHECK(cudaMemcpyAsync(dU, Uc.data(), sizeof(double) * N * N, cudaMemcpyHostToDevice, P.stream));
-        double* dst = (part == 0 ? P.dint : P.dint2) + (want_shared ? 0 : (size_t)(traj0 + c) * P.D);
+        CUDA_CHECK(cudaMemcpyAsync(dU.get(), Uc.data(), sizeof(double) * N * N, cudaMemcpyHostToDevice, P.stream));
+        double* dst = (part == 0 ? P.dint : P.dint2).get() + (want_shared ? 0 : (size_t)(traj0 + c) * P.D);
         const int threads = 256;
         const long long blocks = std::min<long long>((P.D + threads - 1) / threads, (long long)P.sm_count * 16);
         dint_kernel<<<(unsigned)std::max<long long>(blocks, 1), threads, sizeof(double) * N * N, P.stream>>>(
-            dst, dU, N, P.dim, P.desc.rydberg_state, P.D, P.shard_offset());
+            dst, dU.get(), N, P.dim, P.desc.rydberg_state, P.D, P.shard_offset());
         CUDA_CHECK(cudaGetLastError());
         // bounds per |r>-count
         std::vector<double> mins(N + 1, 1e300), maxs(N + 1, -1e300);
-        CUDA_CHECK(cudaMemcpyAsync(P.d_scratch, mins.data(), sizeof(double) * (N + 1), cudaMemcpyHostToDevice, P.stream));
-        CUDA_CHECK(cudaMemcpyAsync(P.d_scratch + 64, maxs.data(), sizeof(double) * (N + 1), cudaMemcpyHostToDevice, P.stream));
+        double* d_mins = P.d_scratch.get();
+        double* d_maxs = d_mins + 64;
+        CUDA_CHECK(cudaMemcpyAsync(d_mins, mins.data(), sizeof(double) * (N + 1), cudaMemcpyHostToDevice, P.stream));
+        CUDA_CHECK(cudaMemcpyAsync(d_maxs, maxs.data(), sizeof(double) * (N + 1), cudaMemcpyHostToDevice, P.stream));
         dint_bounds_kernel<<<(unsigned)std::max<long long>(blocks, 1), threads, 0, P.stream>>>(
-            dst, N, P.dim, P.desc.rydberg_state, P.D, P.d_scratch, P.d_scratch + 64, P.shard_offset());
+            dst, N, P.dim, P.desc.rydberg_state, P.D, d_mins, d_maxs, P.shard_offset());
         CUDA_CHECK(cudaGetLastError());
-        CUDA_CHECK(cudaMemcpyAsync(mins.data(), P.d_scratch, sizeof(double) * (N + 1), cudaMemcpyDeviceToHost, P.stream));
-        CUDA_CHECK(cudaMemcpyAsync(maxs.data(), P.d_scratch + 64, sizeof(double) * (N + 1), cudaMemcpyDeviceToHost, P.stream));
+        CUDA_CHECK(cudaMemcpyAsync(mins.data(), d_mins, sizeof(double) * (N + 1), cudaMemcpyDeviceToHost, P.stream));
+        CUDA_CHECK(cudaMemcpyAsync(maxs.data(), d_maxs, sizeof(double) * (N + 1), cudaMemcpyDeviceToHost, P.stream));
         CUDA_CHECK(cudaStreamSynchronize(P.stream));
         double mn = 1e300, mx = -1e300;
         for (int k = 0; k <= N; ++k)
@@ -2963,7 +3004,6 @@ int pb200_plan_set_interaction(pb200_plan* h, int32_t traj0, int32_t count, cons
             P.dmin2_traj[slot] = mn; P.dmax2_traj[slot] = mx;
         }
       }
-    pool_free(P.desc.device, dU);
     P.has_interaction = true;
     P.tay.w_knot.clear();
     PB200_CATCH
@@ -2975,17 +3015,16 @@ int pb200_plan_set_xy(pb200_plan* h, int32_t traj0, int32_t count, const double*
     if (!h || !Uxy) fail(PB200_ERR_INVALID, "null argument");
     Plan& P = h->p;
     if (shared && (count != 1 || traj0 != 0)) fail(PB200_ERR_INVALID, "shared couplings: traj0 = 0, count = 1");
-    if (!shared && (traj0 < 0 || count < 1 || traj0 + count > P.B)) fail(PB200_ERR_INVALID, "trajectory range");
+    if (!shared) check_traj_range(P, traj0, count, "pb200_plan_set_xy");
     if (digit_u < 0 || digit_u >= P.dim || digit_d < 0 || digit_d >= P.dim || digit_u == digit_d)
         fail(PB200_ERR_INVALID, "bad eigenstate digits");
     if (P.n > 40) fail(PB200_ERR_UNSUPPORTED, "XY mode: at most 40 qudits");
     CUDA_CHECK(cudaSetDevice(P.desc.device));
     const int N = P.n;
     const bool want_shared = shared != 0;
-    if (P.d_xy && P.xy_shared != want_shared) { CUDA_CHECK(cudaStreamSynchronize(P.stream)); pool_free(P.desc.device, P.d_xy); P.d_xy = nullptr; }
-    if (!P.d_xy) {
-        P.d_xy = (decltype(P.d_xy))pool_alloc(P.desc.device, sizeof(double) * (size_t)N * N * (want_shared ? 1 : P.B));
-        CUDA_CHECK(cudaMemsetAsync(P.d_xy, 0, sizeof(double) * (size_t)N * N * (want_shared ? 1 : P.B), P.stream));
+    if (!P.d_xy || P.xy_shared != want_shared) {
+        P.d_xy.reset(P, (size_t)N * N * (want_shared ? 1 : P.B));
+        CUDA_CHECK(cudaMemsetAsync(P.d_xy.get(), 0, sizeof(double) * (size_t)N * N * (want_shared ? 1 : P.B), P.stream));
     }
     P.xy_shared = want_shared;
     P.xy_norm.resize(want_shared ? 1 : P.B, 0.0);
@@ -3004,7 +3043,7 @@ int pb200_plan_set_xy(pb200_plan* h, int32_t traj0, int32_t count, const double*
                 if (i < j) { if (touched) nrm2 += std::fabs(u); else nrm += std::fabs(u); }
             }
         const int slot = want_shared ? 0 : traj0 + c;
-        CUDA_CHECK(cudaMemcpyAsync(P.d_xy + (size_t)slot * N * N, Uc.data(), sizeof(double) * N * N, cudaMemcpyHostToDevice, P.stream));
+        CUDA_CHECK(cudaMemcpyAsync(P.d_xy.get() + (size_t)slot * N * N, Uc.data(), sizeof(double) * N * N, cudaMemcpyHostToDevice, P.stream));
         CUDA_CHECK(cudaStreamSynchronize(P.stream));
         P.xy_norm[slot] = nrm; P.xy_norm2[slot] = nrm2;
     }
@@ -3038,7 +3077,7 @@ int pb200_plan_set_drive(pb200_plan* h, int32_t drive, int32_t traj0, int32_t co
     if (!h || !coef || !det) fail(PB200_ERR_INVALID, "null argument");
     Plan& P = h->p;
     if (drive < 0 || drive >= P.n_drives) fail(PB200_ERR_INVALID, "drive index out of range");
-    if (traj0 < 0 || count < 1 || traj0 + count > P.B) fail(PB200_ERR_INVALID, "trajectory range");
+    check_traj_range(P, traj0, count, "pb200_plan_set_drive");
     const int rows = P.desc.drives[drive].uniform ? 1 : P.n;
     const int nt = (int)P.times.size();
     for (int c = 0; c < count; ++c) {
@@ -3127,9 +3166,9 @@ int pb200_state_set(pb200_plan* h, int32_t traj0, int32_t count, const double* p
     NvtxRange nvtx_range("pb200_state_set");
     if (!h) fail(PB200_ERR_INVALID, "null plan");
     Plan& P = h->p;
-    if (traj0 < 0 || count < 1 || traj0 + count > P.B) fail(PB200_ERR_INVALID, "trajectory range");
+    check_traj_range(P, traj0, count, "pb200_state_set");
     CUDA_CHECK(cudaSetDevice(P.desc.device));
-    c2* cur = P.buf[P.cur];
+    c2* cur = P.buf[P.cur].get();
     for (int c = 0; c < count; ++c) {
         c2* dst = cur + (size_t)(traj0 + c) * P.D;
         if (psi) {
@@ -3155,9 +3194,9 @@ int pb200_state_get(pb200_plan* h, int32_t traj0, int32_t count, double* psi) {
     NvtxRange nvtx_range("pb200_state_get");
     if (!h || !psi) fail(PB200_ERR_INVALID, "null argument");
     Plan& P = h->p;
-    if (traj0 < 0 || count < 1 || traj0 + count > P.B) fail(PB200_ERR_INVALID, "trajectory range");
+    check_traj_range(P, traj0, count, "pb200_state_get");
     CUDA_CHECK(cudaSetDevice(P.desc.device));
-    CUDA_CHECK(cudaMemcpyAsync(psi, P.buf[P.cur] + (size_t)traj0 * P.D, sizeof(c2) * (size_t)P.D * count,
+    CUDA_CHECK(cudaMemcpyAsync(psi, P.buf[P.cur].get() + (size_t)traj0 * P.D, sizeof(c2) * (size_t)P.D * count,
                                cudaMemcpyDeviceToHost, P.stream));
     CUDA_CHECK(cudaStreamSynchronize(P.stream));
     PB200_CATCH
@@ -3167,13 +3206,13 @@ int pb200_state_probabilities(pb200_plan* h, int32_t traj0, int32_t count, doubl
     PB200_TRY
     if (!h || !probs) fail(PB200_ERR_INVALID, "null argument");
     Plan& P = h->p;
-    if (traj0 < 0 || count < 1 || traj0 + count > P.B) fail(PB200_ERR_INVALID, "trajectory range");
+    check_traj_range(P, traj0, count, "pb200_state_probabilities");
     CUDA_CHECK(cudaSetDevice(P.desc.device));
     // reuse a scratch state buffer for the doubles
-    double* tmp = reinterpret_cast<double*>(P.buf[(P.cur + 1) % 3]);
+    double* tmp = reinterpret_cast<double*>(P.buf[(P.cur + 1) % 3].get());
     const long long total = P.D * count;
     const long long blocks = std::min<long long>((total + 255) / 256, (long long)P.sm_count * 16);
-    prob_kernel<<<(unsigned)blocks, 256, 0, P.stream>>>(P.buf[P.cur] + (size_t)traj0 * P.D, tmp, total);
+    prob_kernel<<<(unsigned)blocks, 256, 0, P.stream>>>(P.buf[P.cur].get() + (size_t)traj0 * P.D, tmp, total);
     CUDA_CHECK(cudaGetLastError());
     CUDA_CHECK(cudaMemcpyAsync(probs, tmp, sizeof(double) * (size_t)total, cudaMemcpyDeviceToHost, P.stream));
     CUDA_CHECK(cudaStreamSynchronize(P.stream));
@@ -3184,15 +3223,14 @@ int pb200_state_norm2(pb200_plan* h, int32_t traj0, int32_t count, double* norms
     PB200_TRY
     if (!h || !norms2) fail(PB200_ERR_INVALID, "null argument");
     Plan& P = h->p;
-    if (traj0 < 0 || count < 1 || traj0 + count > P.B || count > 4096) fail(PB200_ERR_INVALID, "trajectory range");
+    check_traj_range(P, traj0, count, "pb200_state_norm2");
+    if (count > 4096) fail(PB200_ERR_INVALID, "pb200_state_norm2: trajectory range: at most 4096 per call");
     CUDA_CHECK(cudaSetDevice(P.desc.device));
-    CUDA_CHECK(cudaMemsetAsync(P.d_scratch, 0, sizeof(double) * count, P.stream));
     const long long blocks = std::min<long long>((P.D + 255) / 256, (long long)P.sm_count * 4);
     dim3 grid((unsigned)std::max<long long>(blocks, 1), (unsigned)count);
-    norm2_kernel<<<grid, 256, 0, P.stream>>>(P.buf[P.cur] + (size_t)traj0 * P.D, P.D, P.d_scratch);
-    CUDA_CHECK(cudaGetLastError());
-    CUDA_CHECK(cudaMemcpyAsync(norms2, P.d_scratch, sizeof(double) * count, cudaMemcpyDeviceToHost, P.stream));
-    CUDA_CHECK(cudaStreamSynchronize(P.stream));
+    device_sum(P, P.d_scratch.get(), count, norms2, [&] {
+        norm2_kernel<<<grid, 256, 0, P.stream>>>(P.buf[P.cur].get() + (size_t)traj0 * P.D, P.D, P.d_scratch.get());
+    });
     PB200_CATCH
 }
 
@@ -3200,21 +3238,17 @@ int pb200_state_occupation(pb200_plan* h, int32_t traj0, int32_t count, int32_t 
     PB200_TRY
     if (!h || !occ) fail(PB200_ERR_INVALID, "null argument");
     Plan& P = h->p;
-    if (traj0 < 0 || count < 1 || traj0 + count > P.B) fail(PB200_ERR_INVALID, "trajectory range");
+    check_traj_range(P, traj0, count, "pb200_state_occupation");
     if (digit < 0 || digit >= P.dim) fail(PB200_ERR_INVALID, "digit out of range");
     CUDA_CHECK(cudaSetDevice(P.desc.device));
-    double* d_occ = nullptr;
-    d_occ = (decltype(d_occ))pool_alloc(P.desc.device, sizeof(double) * (size_t)count * P.n);
-    CUDA_CHECK(cudaMemsetAsync(d_occ, 0, sizeof(double) * (size_t)count * P.n, P.stream));
+    DevBuf<double> d_occ(P, (size_t)count * P.n);
     const long long blocks = std::min<long long>((P.D + 255) / 256, (long long)P.sm_count * 4);
     dim3 grid((unsigned)std::max<long long>(blocks, 1), (unsigned)count);
-    occupation_kernel<<<grid, 256, sizeof(double) * P.n, P.stream>>>(P.buf[P.cur] + (size_t)traj0 * P.D, d_occ, P.D, P.n,
-                                                                       P.dim, digit, P.shard_offset());
-    cudaError_t e = cudaGetLastError();
-    if (e == cudaSuccess) e = cudaMemcpyAsync(occ, d_occ, sizeof(double) * (size_t)count * P.n, cudaMemcpyDeviceToHost, P.stream);
-    if (e == cudaSuccess) e = cudaStreamSynchronize(P.stream);
-    pool_free(P.desc.device, d_occ);
-    if (e != cudaSuccess) fail(PB200_ERR_CUDA, "occupation: %s", cudaGetErrorString(e));
+    device_sum(P, d_occ.get(), d_occ.size(), occ, [&] {
+        occupation_kernel<<<grid, 256, sizeof(double) * P.n, P.stream>>>(P.buf[P.cur].get() + (size_t)traj0 * P.D,
+                                                                           d_occ.get(), P.D, P.n, P.dim, digit,
+                                                                           P.shard_offset());
+    });
     PB200_CATCH
 }
 
@@ -3222,23 +3256,18 @@ int pb200_state_correlation(pb200_plan* h, int32_t traj0, int32_t count, int32_t
     PB200_TRY
     if (!h || !corr) fail(PB200_ERR_INVALID, "null argument");
     Plan& P = h->p;
-    if (traj0 < 0 || count < 1 || traj0 + count > P.B) fail(PB200_ERR_INVALID, "trajectory range");
+    check_traj_range(P, traj0, count, "pb200_state_correlation");
     if (digit < 0 || digit >= P.dim) fail(PB200_ERR_INVALID, "digit out of range");
     if (P.n > 40) fail(PB200_ERR_UNSUPPORTED, "too many qudits for the correlation matrix");
     CUDA_CHECK(cudaSetDevice(P.desc.device));
     const size_t nn = (size_t)P.n * P.n;
-    double* d_c = nullptr;
-    d_c = (decltype(d_c))pool_alloc(P.desc.device, sizeof(double) * count * nn);
-    CUDA_CHECK(cudaMemsetAsync(d_c, 0, sizeof(double) * count * nn, P.stream));
+    DevBuf<double> d_c(P, count * nn);
     const long long blocks = std::min<long long>((P.D + 2047) / 2048, (long long)P.sm_count * 4);
     dim3 grid((unsigned)std::max<long long>(blocks, 1), (unsigned)count);
-    correlation_kernel<<<grid, 256, 0, P.stream>>>(P.buf[P.cur] + (size_t)traj0 * P.D, d_c, P.D, P.n, P.dim, digit,
-                                                   P.shard_offset());
-    cudaError_t e = cudaGetLastError();
-    if (e == cudaSuccess) e = cudaMemcpyAsync(corr, d_c, sizeof(double) * count * nn, cudaMemcpyDeviceToHost, P.stream);
-    if (e == cudaSuccess) e = cudaStreamSynchronize(P.stream);
-    pool_free(P.desc.device, d_c);
-    if (e != cudaSuccess) fail(PB200_ERR_CUDA, "correlation: %s", cudaGetErrorString(e));
+    device_sum(P, d_c.get(), d_c.size(), corr, [&] {
+        correlation_kernel<<<grid, 256, 0, P.stream>>>(P.buf[P.cur].get() + (size_t)traj0 * P.D, d_c.get(), P.D, P.n, P.dim,
+                                                       digit, P.shard_offset());
+    });
     for (int c = 0; c < count; ++c)  // the kernel fills i <= j
         for (int i = 0; i < P.n; ++i)
             for (int j = 0; j < i; ++j) corr[c * nn + (size_t)i * P.n + j] = corr[c * nn + (size_t)j * P.n + i];
@@ -3250,25 +3279,19 @@ int pb200_state_energy(pb200_plan* h, double t_us, double* energy, double* h2) {
     if (!h || !energy || !h2) fail(PB200_ERR_INVALID, "null argument");
     Plan& P = h->p;
     refuse_shard(P, "pb200_state_energy", "pb200_shards_energy");
-    for (int tr = 0; tr < P.B; ++tr)
-        for (int q = 0; q < P.n_drives; ++q)
-            if (!P.tabs_set[tr][q]) fail(PB200_ERR_STATE, "drive %d of trajectory %d not set", q, tr);
+    check_drives_set(P, "pb200_state_energy");
     CUDA_CHECK(cudaSetDevice(P.desc.device));
-    c2* hpsi = P.buf[(P.cur + 2) % 3];
+    c2* psi = P.buf[P.cur].get();
+    c2* hpsi = P.buf[(P.cur + 2) % 3].get();
     long long launches = 0;
-    apply_h_device(P, t_us, P.buf[P.cur], hpsi, launches);
-    double* d_acc = nullptr;
-    d_acc = (decltype(d_acc))pool_alloc(P.desc.device, sizeof(double) * 2 * P.B);
-    CUDA_CHECK(cudaMemsetAsync(d_acc, 0, sizeof(double) * 2 * P.B, P.stream));
+    apply_h_device(P, t_us, psi, hpsi, launches);
+    DevBuf<double> d_acc(P, 2 * (size_t)P.B);
     const long long blocks = std::min<long long>((P.D + 255) / 256, (long long)P.sm_count * 8);
     dim3 grid((unsigned)std::max<long long>(blocks, 1), (unsigned)P.B);
-    dot2_kernel<<<grid, 256, 0, P.stream>>>(P.buf[P.cur], hpsi, P.D, d_acc);  // Re<psi, H psi>, <H psi, H psi>
     std::vector<double> acc(2 * (size_t)P.B);
-    cudaError_t e = cudaGetLastError();
-    if (e == cudaSuccess) e = cudaMemcpyAsync(acc.data(), d_acc, sizeof(double) * 2 * P.B, cudaMemcpyDeviceToHost, P.stream);
-    if (e == cudaSuccess) e = cudaStreamSynchronize(P.stream);
-    pool_free(P.desc.device, d_acc);
-    if (e != cudaSuccess) fail(PB200_ERR_CUDA, "energy: %s", cudaGetErrorString(e));
+    device_sum(P, d_acc.get(), acc.size(), acc.data(), [&] {
+        dot2_kernel<<<grid, 256, 0, P.stream>>>(psi, hpsi, P.D, d_acc.get());  // Re<psi, H psi>, <H psi, H psi>
+    });
     for (int b = 0; b < P.B; ++b) { energy[b] = acc[2 * b]; h2[b] = acc[2 * b + 1]; }
     PB200_CATCH
 }
@@ -3277,21 +3300,16 @@ int pb200_state_overlap(pb200_plan* h, int32_t traj0, int32_t count, const doubl
     PB200_TRY
     if (!h || !phi || !out) fail(PB200_ERR_INVALID, "null argument");
     Plan& P = h->p;
-    if (traj0 < 0 || count < 1 || traj0 + count > P.B) fail(PB200_ERR_INVALID, "trajectory range");
+    check_traj_range(P, traj0, count, "pb200_state_overlap");
     CUDA_CHECK(cudaSetDevice(P.desc.device));
-    c2* d_phi = P.buf[(P.cur + 1) % 3];
+    c2* d_phi = P.buf[(P.cur + 1) % 3].get();
     CUDA_CHECK(cudaMemcpyAsync(d_phi, phi, sizeof(c2) * (size_t)P.D, cudaMemcpyHostToDevice, P.stream));
-    double* d_acc = nullptr;
-    d_acc = (decltype(d_acc))pool_alloc(P.desc.device, sizeof(double) * 2 * count);
-    CUDA_CHECK(cudaMemsetAsync(d_acc, 0, sizeof(double) * 2 * count, P.stream));
+    DevBuf<double> d_acc(P, 2 * (size_t)count);
     const long long blocks = std::min<long long>((P.D + 255) / 256, (long long)P.sm_count * 8);
     dim3 grid((unsigned)std::max<long long>(blocks, 1), (unsigned)count);
-    overlap_kernel<<<grid, 256, 0, P.stream>>>(d_phi, P.buf[P.cur] + (size_t)traj0 * P.D, P.D, d_acc);
-    cudaError_t e = cudaGetLastError();
-    if (e == cudaSuccess) e = cudaMemcpyAsync(out, d_acc, sizeof(double) * 2 * count, cudaMemcpyDeviceToHost, P.stream);
-    if (e == cudaSuccess) e = cudaStreamSynchronize(P.stream);
-    pool_free(P.desc.device, d_acc);
-    if (e != cudaSuccess) fail(PB200_ERR_CUDA, "overlap: %s", cudaGetErrorString(e));
+    device_sum(P, d_acc.get(), d_acc.size(), out, [&] {
+        overlap_kernel<<<grid, 256, 0, P.stream>>>(d_phi, P.buf[P.cur].get() + (size_t)traj0 * P.D, P.D, d_acc.get());
+    });
     PB200_CATCH
 }
 
@@ -3303,32 +3321,19 @@ int pb200_state_expect(pb200_plan* h, int32_t traj0, int32_t count, const pb200_
     refuse_shard(P, "pb200_state_expect", "pb200_shards_expect");
     if (P.has_diss)
         fail(PB200_ERR_UNSUPPORTED, "pb200_state_expect: the plan holds a vectorised density matrix, not state vectors");
-    if (traj0 < 0 || count < 1 || traj0 + count > P.B)
-        fail(PB200_ERR_INVALID, "pb200_state_expect: trajectories [%d, %d) outside [0, %d)", traj0, traj0 + count, P.B);
+    check_traj_range(P, traj0, count, "pb200_state_expect");
     check_op_terms(op, P.n, P.dim, "pb200_state_expect");
     if (!P.state_set) fail(PB200_ERR_STATE, "pb200_state_expect: no state set");
     std::fill(out, out + 2 * (size_t)count, 0.0);
     const ExpHost H = exp_host(op, P.n, P.dim, P.n);
     if (H.n_chunks == 0) return PB200_OK;
     CUDA_CHECK(cudaSetDevice(P.desc.device));
-    ExpTable X;
-    X.upload(H, P);
-    double* d_acc = (double*)pool_alloc(P.desc.device, sizeof(double) * 2 * count);
-    const c2* psi = P.buf[P.cur] + (size_t)traj0 * P.D;
+    const DevBuf<char> X = upload_exp(H, P);
+    DevBuf<double> d_acc(P, 2 * (size_t)count);
+    const c2* psi = P.buf[P.cur].get() + (size_t)traj0 * P.D;
     ExpSrc src{};
     src.p[0] = psi; src.shard = 0; src.local_bits = P.n;
-    cudaError_t e = cudaMemsetAsync(d_acc, 0, sizeof(double) * 2 * count, P.stream);
-    try {
-        if (e == cudaSuccess) launch_expect(P, H, X, src, psi, count, d_acc);
-    } catch (...) {
-        if (cudaStreamSynchronize(P.stream) != cudaSuccess) cudaGetLastError();  // the kernel no longer writes d_acc
-        pool_free(P.desc.device, d_acc);
-        throw;
-    }
-    if (e == cudaSuccess) e = cudaMemcpyAsync(out, d_acc, sizeof(double) * 2 * count, cudaMemcpyDeviceToHost, P.stream);
-    if (e == cudaSuccess) e = cudaStreamSynchronize(P.stream);
-    pool_free(P.desc.device, d_acc);
-    if (e != cudaSuccess) fail(PB200_ERR_CUDA, "pb200_state_expect: %s", cudaGetErrorString(e));
+    device_sum(P, d_acc.get(), d_acc.size(), out, [&] { launch_expect(P, H, X.get(), src, psi, count, d_acc.get()); });
     PB200_CATCH
 }
 
@@ -3345,33 +3350,22 @@ int pb200_state_sample(pb200_plan* h, int32_t traj, int32_t one_digit, const dou
     if (nbits > 30) fail(PB200_ERR_UNSUPPORTED, "bitstring sampling: at most 30 qudits (32-bit item count of the prefix scan)");
     CUDA_CHECK(cudaSetDevice(P.desc.device));
     const long long M = 1LL << nbits;
-    double *d_w = nullptr, *d_u = nullptr; long long* d_idx = nullptr; void* d_tmp = nullptr;
+    DevBuf<double> d_w(P, (size_t)M), d_u(P, (size_t)n_shots);
+    DevBuf<long long> d_idx(P, (size_t)n_shots);
+    CUDA_CHECK(cudaMemsetAsync(d_w.get(), 0, sizeof(double) * (size_t)M, P.stream));
+    CUDA_CHECK(cudaMemcpyAsync(d_u.get(), uniforms, sizeof(double) * (size_t)n_shots, cudaMemcpyHostToDevice, P.stream));
+    const long long blocks = std::min<long long>((P.D + 255) / 256, (long long)P.sm_count * 8);
+    bitstring_weights_kernel<<<(unsigned)std::max<long long>(blocks, 1), 256, 0, P.stream>>>(
+        P.buf[P.cur].get() + (size_t)traj * P.D, d_w.get(), P.D, P.n, P.dim, one_digit, P.shard_offset());
+    CUDA_CHECK(cudaGetLastError());
     size_t tmp_bytes = 0;
-    cudaError_t e = cudaSuccess;
-    auto cleanup = [&]() { pool_free(P.desc.device, d_w); pool_free(P.desc.device, d_u); pool_free(P.desc.device, d_idx); pool_free(P.desc.device, d_tmp); };
-    try {
-        d_w = (decltype(d_w))pool_alloc(P.desc.device, sizeof(double) * (size_t)M);
-        d_u = (decltype(d_u))pool_alloc(P.desc.device, sizeof(double) * (size_t)n_shots);
-        d_idx = (decltype(d_idx))pool_alloc(P.desc.device, sizeof(long long) * (size_t)n_shots);
-        CUDA_CHECK(cudaMemsetAsync(d_w, 0, sizeof(double) * (size_t)M, P.stream));
-        CUDA_CHECK(cudaMemcpyAsync(d_u, uniforms, sizeof(double) * (size_t)n_shots, cudaMemcpyHostToDevice, P.stream));
-        const long long blocks = std::min<long long>((P.D + 255) / 256, (long long)P.sm_count * 8);
-        bitstring_weights_kernel<<<(unsigned)std::max<long long>(blocks, 1), 256, 0, P.stream>>>(
-            P.buf[P.cur] + (size_t)traj * P.D, d_w, P.D, P.n, P.dim, one_digit, P.shard_offset());
-        CUDA_CHECK(cudaGetLastError());
-        CUDA_CHECK(cub::DeviceScan::InclusiveSum(nullptr, tmp_bytes, d_w, d_w, (int)M, P.stream));
-        d_tmp = (decltype(d_tmp))pool_alloc(P.desc.device, tmp_bytes);
-        CUDA_CHECK(cub::DeviceScan::InclusiveSum(d_tmp, tmp_bytes, d_w, d_w, (int)M, P.stream));
-        search_sorted_kernel<<<(n_shots + 255) / 256, 256, 0, P.stream>>>(d_w, M, d_u, d_idx, n_shots);
-        CUDA_CHECK(cudaGetLastError());
-        CUDA_CHECK(cudaMemcpyAsync(out, d_idx, sizeof(long long) * (size_t)n_shots, cudaMemcpyDeviceToHost, P.stream));
-        CUDA_CHECK(cudaStreamSynchronize(P.stream));
-    } catch (...) {
-        cleanup();
-        throw;
-    }
-    (void)e;
-    cleanup();
+    CUDA_CHECK(cub::DeviceScan::InclusiveSum(nullptr, tmp_bytes, d_w.get(), d_w.get(), (int)M, P.stream));
+    DevBuf<char> d_tmp(P, tmp_bytes);
+    CUDA_CHECK(cub::DeviceScan::InclusiveSum(d_tmp.get(), tmp_bytes, d_w.get(), d_w.get(), (int)M, P.stream));
+    search_sorted_kernel<<<(n_shots + 255) / 256, 256, 0, P.stream>>>(d_w.get(), M, d_u.get(), d_idx.get(), n_shots);
+    CUDA_CHECK(cudaGetLastError());
+    CUDA_CHECK(cudaMemcpyAsync(out, d_idx.get(), sizeof(long long) * (size_t)n_shots, cudaMemcpyDeviceToHost, P.stream));
+    CUDA_CHECK(cudaStreamSynchronize(P.stream));
     PB200_CATCH
 }
 
@@ -3388,7 +3382,7 @@ int pb200_state_copy(pb200_plan* dst, int32_t dst_traj, pb200_plan* src, int32_t
     if (A.B > 1 && !A.state_set) fail(PB200_ERR_STATE, "pb200_state_copy: set the other trajectories of the destination first");
     CUDA_CHECK(cudaSetDevice(A.desc.device));
     CUDA_CHECK(cudaStreamSynchronize(S.stream));  // the source state is complete
-    CUDA_CHECK(cudaMemcpyAsync(A.buf[A.cur] + (size_t)dst_traj * A.D, S.buf[S.cur] + (size_t)src_traj * S.D,
+    CUDA_CHECK(cudaMemcpyAsync(A.buf[A.cur].get() + (size_t)dst_traj * A.D, S.buf[S.cur].get() + (size_t)src_traj * S.D,
                                sizeof(c2) * (size_t)A.D, cudaMemcpyDeviceToDevice, A.stream));
     CUDA_CHECK(cudaStreamSynchronize(A.stream));
     A.state_set = true;
@@ -3398,7 +3392,7 @@ int pb200_state_copy(pb200_plan* dst, int32_t dst_traj, pb200_plan* src, int32_t
 int pb200_state_device_ptr(pb200_plan* h, void** dptr) {
     PB200_TRY
     if (!h || !dptr) fail(PB200_ERR_INVALID, "null argument");
-    *dptr = h->p.buf[h->p.cur];
+    *dptr = h->p.buf[h->p.cur].get();
     PB200_CATCH
 }
 
@@ -3419,12 +3413,10 @@ int pb200_apply_h(pb200_plan* h, int32_t traj, double t_us, const double* in, do
     Plan& P = h->p;
     refuse_shard(P, "pb200_apply_h", "pb200_shards_apply_h");
     if (traj < 0 || traj >= P.B) fail(PB200_ERR_INVALID, "trajectory out of range");
-    for (int tr = 0; tr < P.B; ++tr)
-        for (int q = 0; q < P.n_drives; ++q)
-            if (!P.tabs_set[tr][q]) fail(PB200_ERR_STATE, "drive %d of trajectory %d not set", q, tr);
+    check_drives_set(P, "pb200_apply_h");
     CUDA_CHECK(cudaSetDevice(P.desc.device));
-    c2* bin = P.buf[(P.cur + 1) % 3];
-    c2* bout = P.buf[(P.cur + 2) % 3];
+    c2* bin = P.buf[(P.cur + 1) % 3].get();
+    c2* bout = P.buf[(P.cur + 2) % 3].get();
     // the kernels run over the whole batch: zero the other trajectories' input
     CUDA_CHECK(cudaMemsetAsync(bin, 0, sizeof(c2) * (size_t)P.D * P.B, P.stream));
     CUDA_CHECK(cudaMemcpyAsync(bin + (size_t)traj * P.D, in, sizeof(c2) * (size_t)P.D, cudaMemcpyHostToDevice, P.stream));
@@ -3456,8 +3448,8 @@ int pb200_bench_apply(pb200_plan* h, double t_us, int32_t reps, double* ms_out, 
     refuse_shard(P, "pb200_bench_apply", "pb200_shards_apply_h");
     if (!P.state_set) fail(PB200_ERR_STATE, "no state set");
     CUDA_CHECK(cudaSetDevice(P.desc.device));
-    c2* in = P.buf[P.cur];
-    c2* outb = P.buf[(P.cur + 1) % 3];
+    c2* in = P.buf[P.cur].get();
+    c2* outb = P.buf[(P.cur + 1) % 3].get();
     long long launches = 0;
     apply_h_device(P, t_us, in, outb, launches);  // warm-up + table upload
     CUDA_CHECK(cudaStreamSynchronize(P.stream));
@@ -3473,7 +3465,7 @@ int pb200_bench_apply(pb200_plan* h, double t_us, int32_t reps, double* ms_out, 
     launches = 0;
     CUDA_CHECK(cudaEventRecord(e0, P.stream));
     for (int r = 0; r < reps; ++r)
-        launch_stage(P, passes, in, nullptr, nullptr, outb, sc, uniform, E.g[0].imag() == 0.0, ud, P.d_table, launches);
+        launch_stage(P, passes, in, nullptr, nullptr, outb, sc, uniform, E.g[0].imag() == 0.0, ud, P.d_table.get(), launches);
     CUDA_CHECK(cudaEventRecord(e1, P.stream));
     CUDA_CHECK(cudaEventSynchronize(e1));
     CUDA_CHECK(cudaGetLastError());
@@ -3633,7 +3625,7 @@ int pb200_shards_apply_h(pb200_plan** plans, int32_t count, double t_us, const d
     std::vector<c2*> bin(count), bout(count);
     for (int r = 0; r < count; ++r) {
         Plan& P = *G[r];
-        bin[r] = P.buf[(P.cur + 1) % 3]; bout[r] = P.buf[(P.cur + 2) % 3];
+        bin[r] = P.buf[(P.cur + 1) % 3].get(); bout[r] = P.buf[(P.cur + 2) % 3].get();
         CUDA_CHECK(cudaSetDevice(P.desc.device));
         CUDA_CHECK(cudaMemcpyAsync(bin[r], in + (size_t)2 * P.D * r, sizeof(c2) * (size_t)P.D, cudaMemcpyHostToDevice, P.stream));
     }
@@ -3655,7 +3647,7 @@ int pb200_shards_energy(pb200_plan** plans, int32_t count, double t_us, double* 
     std::vector<c2*> psi(count), hpsi(count);
     for (int r = 0; r < count; ++r) {
         if (!G[r]->state_set) fail(PB200_ERR_STATE, "pb200_shards_energy: no state set on shard %d", r);
-        psi[r] = G[r]->buf[G[r]->cur]; hpsi[r] = G[r]->buf[(G[r]->cur + 2) % 3];
+        psi[r] = G[r]->buf[G[r]->cur].get(); hpsi[r] = G[r]->buf[(G[r]->cur + 2) % 3].get();
     }
     shards_apply_h(G, t_us, psi, hpsi);
     // Re<psi, H psi> and <H psi, H psi>, summed over the shards
@@ -3663,13 +3655,12 @@ int pb200_shards_energy(pb200_plan** plans, int32_t count, double t_us, double* 
     for (int r = 0; r < count; ++r) {
         Plan& P = *G[r];
         CUDA_CHECK(cudaSetDevice(P.desc.device));
-        CUDA_CHECK(cudaMemsetAsync(P.d_scratch, 0, sizeof(double) * 2, P.stream));
         const long long blocks = std::min<long long>((P.D + 255) / 256, (long long)P.sm_count * 8);
-        dot2_kernel<<<dim3((unsigned)std::max<long long>(blocks, 1), 1), 256, 0, P.stream>>>(psi[r], hpsi[r], P.D, P.d_scratch);
-        CUDA_CHECK(cudaGetLastError());
         double acc[2];
-        CUDA_CHECK(cudaMemcpyAsync(acc, P.d_scratch, sizeof(double) * 2, cudaMemcpyDeviceToHost, P.stream));
-        CUDA_CHECK(cudaStreamSynchronize(P.stream));
+        device_sum(P, P.d_scratch.get(), 2, acc, [&] {
+            dot2_kernel<<<dim3((unsigned)std::max<long long>(blocks, 1), 1), 256, 0, P.stream>>>(psi[r], hpsi[r], P.D,
+                                                                                                 P.d_scratch.get());
+        });
         e += acc[0]; e2 += acc[1];
     }
     energy[0] = e; h2[0] = e2;
@@ -3709,40 +3700,33 @@ int pb200_shards_expect(pb200_plan** plans, int32_t count, const pb200_op_terms*
     }
     ExpSrc src{};
     src.local_bits = L;
-    for (int r = 0; r < count; ++r) src.p[r] = G[r]->buf[G[r]->cur];
-    std::vector<ExpTable> X(count);
-    std::vector<double*> acc(count, nullptr);
-    // every shard's kernel reads its peers' slices: all streams are idle before any accumulator returns to the pool
-    auto release = [&]() {
-        for (int r = 0; r < count; ++r)
-            if (cudaStreamSynchronize(G[r]->stream) != cudaSuccess) cudaGetLastError();
-        for (int r = 0; r < count; ++r) if (acc[r]) pool_free(G[r]->desc.device, acc[r]);
-    };
-    try {
-        shards_sync(G);  // every slice is complete before a shard reads a peer's
-        for (int r = 0; r < count; ++r) {
-            Plan& P = *G[r];
-            CUDA_CHECK(cudaSetDevice(P.desc.device));
-            X[r].upload(H, P);
-            acc[r] = (double*)pool_alloc(P.desc.device, sizeof(double) * 2);
-            CUDA_CHECK(cudaMemsetAsync(acc[r], 0, sizeof(double) * 2, P.stream));
-            src.shard = r;
-            launch_expect(P, H, X[r], src, nullptr, 1, acc[r]);
+    for (int r = 0; r < count; ++r) src.p[r] = G[r]->buf[G[r]->cur].get();
+    std::vector<DevBuf<char>> X(count);
+    std::vector<DevBuf<double>> acc(count);
+    // every shard's kernel reads its peers' slices: all streams are idle before any buffer of the group is released
+    struct GroupIdle {
+        const std::vector<Plan*>& G;
+        ~GroupIdle() {
+            for (Plan* P : G)
+                if (cudaStreamSynchronize(P->stream) != cudaSuccess) cudaGetLastError();
         }
-        for (int r = 0; r < count; ++r) {
-            Plan& P = *G[r];
-            double a[2];
-            CUDA_CHECK(cudaSetDevice(P.desc.device));
-            CUDA_CHECK(cudaMemcpyAsync(a, acc[r], sizeof(double) * 2, cudaMemcpyDeviceToHost, P.stream));
-            CUDA_CHECK(cudaStreamSynchronize(P.stream));
-            out[0] += a[0]; out[1] += a[1];
-        }
-        shards_sync(G);  // no shard still reads a peer's slice
-    } catch (...) {
-        release();
-        throw;
+    } idle{G};
+    shards_sync(G);  // every slice is complete before a shard reads a peer's
+    for (int r = 0; r < count; ++r) {
+        Plan& P = *G[r];
+        CUDA_CHECK(cudaSetDevice(P.desc.device));
+        X[r] = upload_exp(H, P);
+        acc[r].reset(P, 2);
+        src.shard = r;
+        sum_launch(P, acc[r].get(), 2, [&] { launch_expect(P, H, X[r].get(), src, nullptr, 1, acc[r].get()); });
     }
-    release();
+    for (int r = 0; r < count; ++r) {
+        double a[2];
+        CUDA_CHECK(cudaSetDevice(G[r]->desc.device));
+        sum_fetch(*G[r], acc[r].get(), 2, a);
+        out[0] += a[0]; out[1] += a[1];
+    }
+    shards_sync(G);  // no shard still reads a peer's slice
     PB200_CATCH
 }
 
