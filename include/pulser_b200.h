@@ -363,6 +363,21 @@ int pb200_host_taylor_separable(const double* coef, const double* det,
                                 int32_t n_traj, int32_t n_qudits,
                                 int32_t n_times, int32_t* separable,
                                 double* a_out, double* c_out, double* m_out);
+/* Separable structure with several detuning time shapes (what lets detuning-map
+ * sequences, masks and their noisy batches run on integrator 3): same tables
+ * and drive factors as pb200_host_taylor_separable, with
+ * det_{b,k} = det_{0,0} + sum_{s < S} c_{b,k,s} * m_s, each max |m_s| = 1, to
+ * 2e-13 of the largest sample, S <= max_shapes <= 4.  Pulser's detuning map
+ * modulator adds -w_k eps(t) n_k to every atom k
+ * (pulser-core/pulser/sampler/samples.py:560-601): one shape per map.
+ * *n_shapes = S, or -1 when the drive rows are not multiples of one row or the
+ * detuning needs more than max_shapes shapes; then a_out[n_traj][n_qudits]
+ * (re,im), c_out[n_traj][n_qudits][max_shapes], m_out[max_shapes][n_times]
+ * (unused shapes 0; any may be NULL). */
+int pb200_host_taylor_shapes(const double* coef, const double* det,
+                             int32_t n_traj, int32_t n_qudits, int32_t n_times,
+                             int32_t max_shapes, int32_t* n_shapes,
+                             double* a_out, double* c_out, double* m_out);
 /* Order K of the Taylor series of a step of length h whose generator obeys
  * |H_j| <= m[j] (j = 0..p): smallest K with remainder bound *tail_out <= tol. */
 int pb200_host_taylor_order(double h, const double* m, int32_t p, double tol,

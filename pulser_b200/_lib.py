@@ -149,6 +149,8 @@ def _load() -> C.CDLL:
             C.c_int, [dp, dp, C.c_int32, C.c_int32, C.c_double, C.c_double, C.c_int32, dp, dp]),
         "pb200_host_taylor_separable": (
             C.c_int, [dp, dp, C.c_int32, C.c_int32, C.c_int32, C.POINTER(C.c_int32), dp, dp, dp]),
+        "pb200_host_taylor_shapes": (
+            C.c_int, [dp, dp, C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.POINTER(C.c_int32), dp, dp, dp]),
         "pb200_host_taylor_order": (
             C.c_int, [C.c_double, dp, C.c_int32, C.c_double, C.POINTER(C.c_int32), dp]),
     }
@@ -168,6 +170,7 @@ EXPORTED_SYMBOLS = [
     "pb200_state_occupation", "pb200_state_correlation", "pb200_state_energy", "pb200_state_overlap", "pb200_state_expect", "pb200_state_sample", "pb200_state_copy", "pb200_state_device_ptr", "pb200_propagate", "pb200_apply_h",
     "pb200_coefficients_at", "pb200_bench_apply", "pb200_host_interpolate",
     "pb200_host_moments", "pb200_host_chebyshev", "pb200_host_taylor_fit", "pb200_host_taylor_order", "pb200_host_taylor_separable",
+    "pb200_host_taylor_shapes",
     "pb200_plan_create_shard", "pb200_shards_link", "pb200_shards_propagate", "pb200_shards_apply_h", "pb200_shards_energy",
     "pb200_shards_expect",
 ]

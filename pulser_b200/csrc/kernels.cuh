@@ -11,6 +11,7 @@
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>
+#include <type_traits>
 
 namespace pb200 {
 
@@ -756,6 +757,11 @@ __global__ void __launch_bounds__(1 << (TBITS - RB), 2) stage_d2_fwd_kernel(cons
 // static factors from a per-trajectory table (TaylorArgs::table) -- the trajectory loop's solves (simulation.py:885-915).
 #define PB200_TAYLOR_PMAX 8
 #define PB200_MAX_SHARD_BITS 3
+#define PB200_TAYLOR_SMAX 4   // detuning time shapes with static per-qubit weights (detuning maps, masks, noise)
+// table of a plan whose detuning has several shapes, or one shape on a uniform drive, per trajectory:
+//   tab[0 .. 2N)              a unit (re, im) per BIT position p (the unit itself for a uniform drive)
+//   tab[2N + s N + p]         weight c_s of bit position p, s < S
+__host__ __device__ inline int taylor_table_stride(int n, int s) { return 2 * n + s * n; }
 struct TaylorArgs {
     const c2* v;       // chi_k, gather source [B][D]
     c2* out;           // chi_{k+1}
@@ -768,15 +774,19 @@ struct TaylorArgs {
     c2 unit;           // uniform drive: e^{-i phi}, the constant phase
     // separable per-qubit drives (trajectory batches with static noise): coef_{b,k}(t) = a_{b,k} unit omega(t),
     // det_{b,k}(t) = theta(t) + c_{b,k} M(t).  table[b][0 .. 2N) = a unit per BIT position (re, im),
-    // table[b][2N .. 3N) = c per bit position (layout of d2_table_stride); nullptr in the uniform case
+    // table[b][2N .. 3N) = c per bit position (layout of d2_table_stride); nullptr in the uniform case.
+    // Several shapes, det_{b,k}(t) = theta(t) + sum_s c_{b,k,s} M_s(t): layout of taylor_table_stride(N, tab_shapes)
     const double* table;
+    int tab_shapes;    // 0: d2_table_stride layout (one shape), else PB200_TAYLOR_SMAX (unused shapes have c = m = 0)
     int to_bit, from_is_one;
-    double th0, gam0, om0, m0;  // H_0 = Dint - th0 n_from - m0 sum_k c_k n_k - gam0 + om0 X
+    double th0, gam0, om0;  // H_0 = Dint - th0 n_from - sum_s m0[s] sum_k c_{k,s} n_k - gam0 + om0 X
+    double m0[PB200_TAYLOR_SMAX];
     c2 scale;          // -i h / (k+1)
     int nh;            // history terms j = 1 .. nh
     const c2* hchi[PB200_TAYLOR_PMAX];   // chi_{k-j}   (nullptr when th_j = m_j = gam_j = 0)
     const c2* hg[PB200_TAYLOR_PMAX];     // G_{k-j}     (nullptr when om_j = 0)
-    double hth[PB200_TAYLOR_PMAX], hgam[PB200_TAYLOR_PMAX], hom[PB200_TAYLOR_PMAX], hm[PB200_TAYLOR_PMAX];
+    double hth[PB200_TAYLOR_PMAX], hgam[PB200_TAYLOR_PMAX], hom[PB200_TAYLOR_PMAX];
+    double hm[PB200_TAYLOR_SMAX][PB200_TAYLOR_PMAX];   // hm[s][j]: shape s, history j
     int acc_read;      // 1: acc is read before it is updated (0: first write of the step)
     int acc_add_v;     // 1: chi_k joins the update (even orders), 0: chi_{k+1} alone
     int acc_on;        // 0: this order leaves the accumulator alone
@@ -788,14 +798,17 @@ struct TaylorArgs {
     int shard_bits, shard;
 };
 
-// epilogue of one amplitude block: everything after the partner sums.  `off[r]` = sum_k c_k [digit_k == from] of the
-// amplitude (0 for uniform drives); idx is the index inside the trajectory, voff the trajectory's offset.
-// The own-element operands are loaded H amplitudes at a time.  SHARD: idx is local, the excitation count is that of the
-// global index (the shard index holds its top bits).
-template <int R, int H = (R >= 4) ? R / 2 : R, bool SHARD = false>
+// epilogue of one amplitude block: everything after the partner sums.  idx is the index inside the trajectory, voff
+// the trajectory's offset.  The own-element operands are loaded H amplitudes at a time.  SHARD: idx is local, the
+// excitation count is that of the global index (the shard index holds its top bits).  The local detuning of amplitude
+// r is either `off[r]` = sum_k c_k [digit_k == from] of the one shape (0 for uniform drives), or, with several shapes,
+// a functor off(r, J) = sum_s m_{s,J} sum_k c_{k,s} [digit_k == from] with the shapes' order-0 coefficients (J = 0)
+// or those of history term J - 1.
+template <int R, int H = (R >= 4) ? R / 2 : R, bool SHARD = false, class Off>
 __device__ __forceinline__ void taylor_epilogue(const TaylorArgs& a, const long long (&idx)[R], const c2 (&v)[R],
-                                                const double (&gx)[R], const double (&gy)[R], const double (&off)[R],
+                                                const double (&gx)[R], const double (&gy)[R], const Off& off,
                                                 long long voff, const double* __restrict__ dsrc) {
+    constexpr bool SHAPES = !std::is_array<Off>::value;
     const int nb = a.geo.n_bits;
     const int ones_hi = SHARD ? __popc(a.shard) : 0;
 #pragma unroll
@@ -809,7 +822,9 @@ __device__ __forceinline__ void taylor_epilogue(const TaylorArgs& a, const long 
             for (int r = 0; r < H; ++r) {
                 const int ones = __popcll((unsigned long long)idx[h0 + r]) + ones_hi;
                 cn[r] = (double)(a.from_is_one ? ones : (nb - ones));
-                const double diag = fma(-a.th0, cn[r], fma(-a.m0, off[h0 + r], dv[r] - a.gam0));
+                double diag;
+                if constexpr (SHAPES) diag = fma(-a.th0, cn[r], dv[r] - a.gam0 - off(h0 + r, 0));
+                else diag = fma(-a.th0, cn[r], fma(-a.m0[0], off[h0 + r], dv[r] - a.gam0));
                 sx[r] = fma(diag, v[h0 + r].x, a.om0 * gx[h0 + r]);
                 sy[r] = fma(diag, v[h0 + r].y, a.om0 * gy[h0 + r]);
             }
@@ -821,7 +836,9 @@ __device__ __forceinline__ void taylor_epilogue(const TaylorArgs& a, const long 
                 for (int r = 0; r < H; ++r) c[r] = ld_own(a.hchi[j] + voff + idx[h0 + r]);
 #pragma unroll
                 for (int r = 0; r < H; ++r) {
-                    const double d = -fma(a.hth[j], cn[r], fma(a.hm[j], off[h0 + r], a.hgam[j]));
+                    double d;
+                    if constexpr (SHAPES) d = -fma(a.hth[j], cn[r], a.hgam[j] + off(h0 + r, j + 1));
+                    else d = -fma(a.hth[j], cn[r], fma(a.hm[0][j], off[h0 + r], a.hgam[j]));
                     sx[r] = fma(d, c[r].x, sx[r]); sy[r] = fma(d, c[r].y, sy[r]);
                 }
             }
@@ -865,11 +882,18 @@ __device__ __forceinline__ void taylor_epilogue(const TaylorArgs& a, const long 
 // what lets 16 amplitudes per thread fit in 128 registers; the first chunk's partner loads overlap the tile copy.
 // SHARD (uniform drives): the launch works on one shard of the state (TaylorArgs::peer); a flip of shard bit q is one
 // more coalesced load from the peer's chi_k at the same local index, issued with the other out-of-tile partners.
-template <bool UNIFORM, bool REAL_G, int TBITS, int RB, bool SHARD = false>
+// NS: detuning shapes with per-bit weights.  0 (uniform) and 1 (batch) read the one-shape table of d2_table_stride;
+// PB200_TAYLOR_SMAX reads taylor_table_stride(N, PB200_TAYLOR_SMAX), with a uniform drive too (detuning maps).  Only
+// the combinations sum_s m_{s,J} off_s of the order's coefficients enter the diagonal, so they are formed once per
+// launch in shared memory (per thread for the bits of base + tid, per register-bit pattern for the rest) and an
+// amplitude reads two of them per history term instead of holding S offsets in registers.
+template <bool UNIFORM, bool REAL_G, int TBITS, int RB, bool SHARD = false, int NS = (UNIFORM ? 0 : 1)>
 __global__ void __launch_bounds__(1 << (TBITS - RB), (65536 / ((1 << (TBITS - RB)) * (RB >= 3 ? 128 : 64))))
 stage_d2_taylor_kernel(const __grid_constant__ TaylorArgs a) {
     static_assert(RB >= 3, "chunks of 8 amplitudes per thread");
     static_assert(UNIFORM || !SHARD, "shards carry one state with a uniform drive");
+    static_assert(NS == (UNIFORM ? 0 : 1) || NS == PB200_TAYLOR_SMAX, "one-shape table, or PB200_TAYLOR_SMAX shapes");
+    constexpr bool SHAPES = NS == PB200_TAYLOR_SMAX;
     constexpr int NT = 1 << (TBITS - RB);
     constexpr int TSIZE = 1 << TBITS;
     constexpr int RC = 8;                   // amplitudes per chunk
@@ -898,13 +922,36 @@ stage_d2_taylor_kernel(const __grid_constant__ TaylorArgs a) {
         tma_load_1d(tile, vsrc + base, (uint32_t)TSIZE * 16u, &mbar);
     }
     double* tab = reinterpret_cast<double*>(tile + TSIZE);
-    if (TAB) {   // the table is written behind the tile copy
-        if (UNIFORM) {
+    // SHAPES, for J = 0 (order-0 coefficients m0) and J = 1 + history j (hm[s][j]) up to nh, behind the per-bit table:
+    //   bl[J][i]   = sum_s m_{s,J} x (shape s's weights of the register bits i, relative to i = 0), the same for all
+    //   at[J][tid] = sum_s m_{s,J} x (shape s's weights of the bits of base + tid, shard bits included)
+    // so that the local detuning of amplitude (c RC + r) in history J is at[J][tid] + bl[J][c RC + r]
+    double* bl = tab + (SHAPES ? taylor_table_stride(g.n_bits, NS) : 0);
+    double* at = bl + ((PB200_TAYLOR_PMAX + 1) << RB);
+    auto shape_coef = [&](int J, int s) { return J == 0 ? a.m0[s] : a.hm[s][J - 1]; };
+    if (TAB || SHAPES) {   // the table is written behind the tile copy
+        if (UNIFORM && !SHAPES) {
             for (int i = tid; i < 2 * g.n_bits; i += NT) tab[i] = (i & 1) ? a.unit.y : a.unit.x;
         } else {
-            const int stride = d2_table_stride(g.n_bits);
+            const int stride = SHAPES ? taylor_table_stride(g.n_bits, NS) : d2_table_stride(g.n_bits);
             const double* src = a.table + traj * stride;
             for (int i = tid; i < stride; i += NT) tab[i] = src[i];
+            if (SHAPES) {
+                for (int i = tid; i < ((a.nh + 1) << RB); i += NT) {
+                    const int J = i >> RB;
+                    double acc = 0.0;
+                    for (int s = 0; s < NS; ++s) {
+                        const double* w = src + 2 * g.n_bits + s * g.n_bits + (TBITS - RB);
+                        double l = 0.0;
+                        for (int q = 0; q < RB; ++q) {
+                            const int bit = (i >> q) & 1;
+                            l += ((bit == a.from_is_one) ? w[q] : 0.0) - ((0 == a.from_is_one) ? w[q] : 0.0);
+                        }
+                        acc = fma(shape_coef(J, s), l, acc);
+                    }
+                    bl[i] = acc;
+                }
+            }
         }
         __syncthreads();
     }
@@ -912,10 +959,29 @@ stage_d2_taylor_kernel(const __grid_constant__ TaylorArgs a) {
     const int nb = g.n_bits;
     // static per-qubit detuning weights: sum over (bits of base) + (bits of tid) + (register bits)
     double common = 0.0;
-    if (!UNIFORM) {
+    if (!UNIFORM && !SHAPES) {
         for (int p = 0; p < nb; ++p) {
             const int bit = (int)(((base + tid) >> p) & 1);
             common += (bit == a.from_is_one) ? tab[2 * nb + p] : 0.0;
+        }
+    }
+    if (SHAPES) {   // a shard's global bits N - shard_bits + q are the bits of the shard index
+        double cs[NS > 0 ? NS : 1];
+#pragma unroll
+        for (int s = 0; s < NS; ++s) cs[s] = 0.0;
+        for (int p = 0; p < nb; ++p) {
+            int bit = (int)(((base + tid) >> p) & 1);
+            if (SHARD && p >= nb - a.shard_bits) bit = (a.shard >> (p - (nb - a.shard_bits))) & 1;
+            if (bit == a.from_is_one) {
+#pragma unroll
+                for (int s = 0; s < NS; ++s) cs[s] += tab[2 * nb + s * nb + p];
+            }
+        }
+        for (int J = 0; J <= a.nh; ++J) {
+            double acc = 0.0;
+#pragma unroll
+            for (int s = 0; s < NS; ++s) acc = fma(shape_coef(J, s), cs[s], acc);
+            at[J * NT + tid] = acc;   // read by this thread only
         }
     }
     const double* dsrc = a.dint ? a.dint + traj * a.dint_stride : nullptr;
@@ -1002,7 +1068,7 @@ stage_d2_taylor_kernel(const __grid_constant__ TaylorArgs a) {
             idx[r] = i0 + r * NT;
             if (!TAB) { pr[r] *= a.unit.x; pi[r] *= a.unit.x; }   // G = ux P for a real unit
             double acc = common;
-            if (!UNIFORM) {
+            if (!UNIFORM && !SHAPES) {
 #pragma unroll
                 for (int q = 0; q < RB; ++q) {
                     const double th = tab[2 * nb + TBITS - RB + q];
@@ -1013,7 +1079,14 @@ stage_d2_taylor_kernel(const __grid_constant__ TaylorArgs a) {
             off[r] = acc;
         }
         // per-qubit factors (off != 0) leave the registers for 2 amplitudes' operands at a time, not 4
-        taylor_epilogue<RC, UNIFORM ? RC / 2 : RC / 4, SHARD>(a, idx, v, pr, pi, off, voff, dsrc);
+        if constexpr (SHAPES) {
+            const double* lc = bl + c * RC;
+            const double* lt = at + tid;
+            taylor_epilogue<RC, RC / 4, SHARD>(
+                a, idx, v, pr, pi, [&](int r, int J) { return lt[J * NT] + lc[(J << RB) + r]; }, voff, dsrc);
+        } else {
+            taylor_epilogue<RC, UNIFORM ? RC / 2 : RC / 4, SHARD>(a, idx, v, pr, pi, off, voff, dsrc);
+        }
     }
 }
 
@@ -1024,8 +1097,11 @@ __global__ void __launch_bounds__(256) stage_d2_taylor_small_kernel(const __grid
     const int nb = a.geo.n_bits;
     const long long traj = blockIdx.y;
     const long long voff = traj * a.D;
-    const double* tab = a.table ? a.table + traj * d2_table_stride(nb) : nullptr;
-    double gxs = 0.0, gys = 0.0, offv = 0.0;
+    const int ns = a.tab_shapes ? a.tab_shapes : 1;
+    const double* tab = a.table ? a.table + traj * (a.tab_shapes ? taylor_table_stride(nb, ns) : d2_table_stride(nb)) : nullptr;
+    double gxs = 0.0, gys = 0.0, offv[PB200_TAYLOR_SMAX];
+#pragma unroll
+    for (int q = 0; q < PB200_TAYLOR_SMAX; ++q) offv[q] = 0.0;
     if (tab) {
         for (int p = 0; p < nb; ++p) {
             const double2 raw = __ldg(reinterpret_cast<const double2*>(a.v + voff + (s ^ (1LL << p))));
@@ -1033,7 +1109,11 @@ __global__ void __launch_bounds__(256) stage_d2_taylor_small_kernel(const __grid
             const double gx = tab[2 * p], gy = (bit == a.to_bit) ? tab[2 * p + 1] : -tab[2 * p + 1];
             gxs = fma(gx, raw.x, gxs); gxs = fma(-gy, raw.y, gxs);
             gys = fma(gx, raw.y, gys); gys = fma(gy, raw.x, gys);
-            offv += (bit == a.from_is_one) ? tab[2 * nb + p] : 0.0;
+            if (bit == a.from_is_one) {
+#pragma unroll
+                for (int q = 0; q < PB200_TAYLOR_SMAX; ++q)
+                    if (q < ns) offv[q] += tab[2 * nb + q * nb + p];
+            }
         }
     } else {
         double pr = 0.0, pi = 0.0, qr = 0.0, qi = 0.0;
@@ -1048,8 +1128,15 @@ __global__ void __launch_bounds__(256) stage_d2_taylor_small_kernel(const __grid
     const long long idx[1] = {s};
     const double2 own = __ldg(reinterpret_cast<const double2*>(a.v + voff + s));
     const c2 v[1] = {{own.x, own.y}};
-    const double gx[1] = {gxs}, gy[1] = {gys}, off[1] = {offv};
-    taylor_epilogue<1>(a, idx, v, gx, gy, off, voff, a.dint ? a.dint + traj * a.dint_stride : nullptr);
+    const double gx[1] = {gxs}, gy[1] = {gys}, offv1[1] = {offv[0]};
+    auto local = [&](int, int J) {
+        double acc = 0.0;
+#pragma unroll
+        for (int q = 0; q < PB200_TAYLOR_SMAX; ++q) acc = fma(J == 0 ? a.m0[q] : a.hm[q][J - 1], offv[q], acc);
+        return acc;
+    };
+    if (a.tab_shapes) taylor_epilogue<1>(a, idx, v, gx, gy, local, voff, a.dint ? a.dint + traj * a.dint_stride : nullptr);
+    else taylor_epilogue<1>(a, idx, v, gx, gy, offv1, voff, a.dint ? a.dint + traj * a.dint_stride : nullptr);
 }
 
 // ---- generic-d stage kernel (any dim, several drives; global gathers) -------

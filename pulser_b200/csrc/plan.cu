@@ -195,6 +195,13 @@ class DevBuf {
 // store of chi_{k+1} (DESIGN.md section 8).
 constexpr int kTaylorTileBits = 13;
 constexpr int kTaylorRegBits = 4;
+// shared memory of the Taylor stage with several detuning shapes: the tile, the per-bit table, and the shapes' sums of
+// every order's coefficients per register-bit pattern and per thread (stage_d2_taylor_kernel<..., PB200_TAYLOR_SMAX>)
+static size_t taylor_shapes_smem(int n) {
+    return ((size_t)16 << kTaylorTileBits) +
+           (size_t)(taylor_table_stride(n, PB200_TAYLOR_SMAX) +
+                    (PB200_TAYLOR_PMAX + 1) * ((1 << kTaylorRegBits) + (1 << (kTaylorTileBits - kTaylorRegBits)))) * 8;
+}
 // tile of the Chebyshev / Lanczos stage kernels (stage_d2_rb_kernel, stage_d2_fwd_kernel): 2^11 amplitudes, 8 per thread
 constexpr int kStageTileBits = 11;
 constexpr int kStageRegBits = 3;
@@ -226,6 +233,13 @@ static int device_setup(int dev) {
     CUDA_CHECK(cudaFuncSetAttribute(stage_d2_taylor_kernel<false, false, kTaylorTileBits, kTaylorRegBits>, cudaFuncAttributeMaxDynamicSharedMemorySize, taylor_smem));
     CUDA_CHECK(cudaFuncSetAttribute(stage_d2_taylor_kernel<true, true, kTaylorTileBits, kTaylorRegBits, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, taylor_smem));
     CUDA_CHECK(cudaFuncSetAttribute(stage_d2_taylor_kernel<true, false, kTaylorTileBits, kTaylorRegBits, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, taylor_smem));
+    const int shapes_smem = (int)taylor_shapes_smem(64);   // several detuning shapes, N <= 64
+    constexpr int SM = PB200_TAYLOR_SMAX;
+    CUDA_CHECK(cudaFuncSetAttribute(stage_d2_taylor_kernel<true, true, kTaylorTileBits, kTaylorRegBits, false, SM>, cudaFuncAttributeMaxDynamicSharedMemorySize, shapes_smem));
+    CUDA_CHECK(cudaFuncSetAttribute(stage_d2_taylor_kernel<true, false, kTaylorTileBits, kTaylorRegBits, false, SM>, cudaFuncAttributeMaxDynamicSharedMemorySize, shapes_smem));
+    CUDA_CHECK(cudaFuncSetAttribute(stage_d2_taylor_kernel<false, false, kTaylorTileBits, kTaylorRegBits, false, SM>, cudaFuncAttributeMaxDynamicSharedMemorySize, shapes_smem));
+    CUDA_CHECK(cudaFuncSetAttribute(stage_d2_taylor_kernel<true, true, kTaylorTileBits, kTaylorRegBits, true, SM>, cudaFuncAttributeMaxDynamicSharedMemorySize, shapes_smem));
+    CUDA_CHECK(cudaFuncSetAttribute(stage_d2_taylor_kernel<true, false, kTaylorTileBits, kTaylorRegBits, true, SM>, cudaFuncAttributeMaxDynamicSharedMemorySize, shapes_smem));
     CUDA_CHECK(cudaFuncSetAttribute(stage_d2_fwd_kernel<true, TB, RB>, cudaFuncAttributeMaxDynamicSharedMemorySize, 2 * 2048 * 16 + 256));
     CUDA_CHECK(cudaFuncSetAttribute(stage_d2_fwd_kernel<false, TB, RB>, cudaFuncAttributeMaxDynamicSharedMemorySize, 2 * 2048 * 16 + 256));
     if (dev >= 0 && dev < PB200_MAX_DEVICES) sm_count[dev] = sms;
@@ -313,17 +327,23 @@ struct Plan {
     // extra ring buffers (beyond buf / aux) for polynomial degrees > 2
     struct TaylorCache {
         bool valid = false, ok = false;
+        const char* why = "";              // why not, once valid
         c2 unit{1.0, 0.0};
         PiecewiseCubic<double> om;         // omega(t): the drive along its constant phase (reference row)
         std::vector<double> w_knot;        // spectral half-width of H at the sampling times
-        // separable per-(trajectory, qubit) drives: coef = a unit omega(t), det = theta(t) + c M(t)
+        // separable per-(trajectory, qubit) drives: coef = a unit omega(t), det = theta(t) + sum_s c_s M_s(t)
         bool uniform = true;               // one state, one coefficient for every qubit (a = 1, c = 0)
-        bool has_m = false;                // some c != 0
-        PiecewiseCubic<double> mshape;     // M(t)
+        bool drive_uniform = true;         // one state, a = 1 (the detuning may have shapes)
+        int ns = 0;                        // detuning shapes, <= PB200_TAYLOR_SMAX
+        PiecewiseCubic<double> shape[PB200_TAYLOR_SMAX];   // M_s(t)
         std::vector<cplx> a;               // [B][N] per qubit
-        std::vector<double> c;             // [B][N]
-        double a_sum_max = 0.0, c_sum_max = 0.0;   // max over trajectories of sum_k |a|, sum_k |c|
-        std::vector<double> tab_host;      // [B][3N+2] device table image
+        std::vector<double> c;             // [B][N][ns]
+        double a_sum_max = 0.0;            // max over trajectories of sum_k |a|
+        double c_sum_max[PB200_TAYLOR_SMAX] = {};   // max over trajectories of sum_k |c_s|
+        // 0: [B][3N+2] device table of one shape (d2_table_stride); PB200_TAYLOR_SMAX: [B][taylor_table_stride(N, SMAX)]
+        // (several shapes, or shapes on a uniform drive)
+        int tab_shapes = 0;
+        std::vector<double> tab_host;      // device table image
         DevBuf<double> d_tab;
     } tay;
     std::vector<DevBuf<c2>> tay_ws;
@@ -1519,7 +1539,8 @@ static void propagate(Plan& P, double t_start, double t_stop, const pb200_run_op
             if (env_int("PB200_TAYLOR_LOG", 0)) fprintf(stderr, "taylor not taken: %s\n", g_taylor_why);
             if (req == 3)
                 fail(PB200_ERR_UNSUPPORTED, "integrator 3 (Taylor) needs a d = 2 register whose drive is one time shape of constant phase "
-                                            "(per-qubit static factors / detuning offsets allowed), no collapse operators / SLM mask");
+                                            "(per-qubit static factors / detuning offsets allowed), no collapse operators / SLM mask: %s",
+                     g_taylor_why);
         }
     }
     const double gtol = (o && o->tol != 0.0) ? o->tol : (P.has_diss ? 1e-6 : 1e-8);
@@ -1827,22 +1848,64 @@ static void propagate(Plan& P, double t_start, double t_stop, const pb200_run_op
 // so a run never synchronises with the host.
 
 // Separable structure of a batch of drive tables, read off the samples (the interpolants are linear in the samples and
-// share their knots):  coef_{b,k}[i] = a_{b,k} * coef_ref[i]  and  det_{b,k}[i] = det_{0,0}[i] + c_{b,k} * m[i]  with ONE
-// reference drive row (the largest one) and ONE common shape m (max |m| = 1).  cs(b,k,i) / ds(b,k,i) return the samples.
-// Least-squares factors with extended-precision sums (4001 same-sign terms: a plain double sum is only good to ~1e-13,
-// which is the size of the residual being tested).  Host only; also reachable through pb200_host_taylor_separable.
+// share their knots):  coef_{b,k}[i] = a_{b,k} * coef_ref[i]  and  det_{b,k}[i] = det_{0,0}[i] + sum_s c_{b,k,s} m_s[i]
+// with ONE reference drive row (the largest one) and at most max_shapes common shapes m_s (max |m_s| = 1): detuning
+// maps, masks and doppler noise each add one.  Greedy: the difference row with the largest residual becomes the next
+// shape, normalised at that sample, and every row is fitted again on all shapes.  cs(b,k,i) / ds(b,k,i) return the
+// samples.  Least-squares factors with extended-precision sums (4001 same-sign terms: a plain double sum is only good
+// to ~1e-13, which is the size of the residual being tested).  Host only; also reachable through
+// pb200_host_taylor_separable (one shape) and pb200_host_taylor_shapes.
 struct SeparableFit {
     bool ok = false;
     const char* why = "";
     int ref_b = 0, ref_k = 0;       // reference drive row
     cplx big = 0.0; double scale = 0.0;
     std::vector<cplx> a;            // [B][N]
-    std::vector<double> c, m;       // [B][N], [nt]
-    bool has_m = false;
+    int ns = 0;                     // shapes
+    std::vector<double> c;          // [B][N][ns]
+    std::vector<std::vector<double>> m;   // [ns][nt]
 };
 
+// least-squares factors of every difference row on the shapes F.m (normal equations in extended precision; the greedy
+// shapes are residuals of the earlier fit, so the system is close to diagonal); max |residual| and where it is
+template <class DS>
+static double taylor_shape_factors(int B, int N, int nt, DS ds, SeparableFit& F, int& rb, int& rk, int& ri) {
+    typedef long double ld;
+    const int S = F.ns;
+    std::vector<ld> G((size_t)S * S, 0.0L);
+    for (int s = 0; s < S; ++s)
+        for (int u = 0; u < S; ++u)
+            for (int i = 0; i < nt; ++i) G[(size_t)s * S + u] += (ld)F.m[s][i] * F.m[u][i];
+    F.c.assign((size_t)B * N * S, 0.0);
+    double emax = -1.0;
+    for (int b = 0; b < B; ++b)
+        for (int k = 0; k < N; ++k) {
+            std::vector<ld> A(G), x(S, 0.0L);
+            for (int s = 0; s < S; ++s)
+                for (int i = 0; i < nt; ++i) x[s] += (ld)(ds(b, k, i) - ds(0, 0, i)) * F.m[s][i];
+            for (int s = 0; s < S; ++s)   // Gaussian elimination (symmetric positive definite: no pivoting)
+                for (int u = s + 1; u < S; ++u) {
+                    const ld f = A[(size_t)u * S + s] / A[(size_t)s * S + s];
+                    for (int w = s; w < S; ++w) A[(size_t)u * S + w] -= f * A[(size_t)s * S + w];
+                    x[u] -= f * x[s];
+                }
+            for (int s = S - 1; s >= 0; --s) {
+                for (int w = s + 1; w < S; ++w) x[s] -= A[(size_t)s * S + w] * x[w];
+                x[s] /= A[(size_t)s * S + s];
+            }
+            double* cc = F.c.data() + ((size_t)b * N + k) * S;
+            for (int s = 0; s < S; ++s) cc[s] = (double)x[s];
+            for (int i = 0; i < nt; ++i) {
+                double r = ds(b, k, i) - ds(0, 0, i);
+                for (int s = 0; s < S; ++s) r -= cc[s] * F.m[s][i];
+                if (std::fabs(r) > emax) { emax = std::fabs(r); rb = b; rk = k; ri = i; }
+            }
+        }
+    return emax;
+}
+
 template <class CS, class DS>
-static SeparableFit taylor_separable(int B, int N, int nt, CS cs, DS ds) {
+static SeparableFit taylor_separable(int B, int N, int nt, CS cs, DS ds, int max_shapes = 1) {
     SeparableFit F;
     for (int b = 0; b < B; ++b)
         for (int k = 0; k < N; ++k)
@@ -1872,7 +1935,7 @@ static SeparableFit taylor_separable(int B, int N, int nt, CS cs, DS ds) {
                 }
             F.a[(size_t)b * N + k] = (ref2 > 0.0L) ? aa : cplx(0.0, 0.0);
         }
-    // every detuning row = the reference row (trajectory 0, qubit 0) + c x one common shape m
+    // every detuning row = the reference row (trajectory 0, qubit 0) + sum_s c_s x common shape m_s
     double dscale = 0.0;
     for (int b = 0; b < B; ++b)
         for (int k = 0; k < N; ++k)
@@ -1884,28 +1947,28 @@ static SeparableFit taylor_separable(int B, int N, int nt, CS cs, DS ds) {
                 const double e = std::fabs(ds(b, k, i) - ds(0, 0, i));
                 if (e > emax) { emax = e; mb = b; mk = k; mi = i; }
             }
-    F.c.assign((size_t)B * N, 0.0);
-    F.m.assign(nt, 0.0);
-    F.has_m = emax > 1e-13 * std::max(dscale, 1e-300);
-    if (F.has_m) {
-        const double norm = ds(mb, mk, mi) - ds(0, 0, mi);
-        long double m2 = 0.0L;
-        for (int i = 0; i < nt; ++i) {
-            F.m[i] = (ds(mb, mk, i) - ds(0, 0, i)) / norm;
-            m2 += (long double)F.m[i] * F.m[i];
-        }
-        for (int b = 0; b < B; ++b)
-            for (int k = 0; k < N; ++k) {
-                long double acc = 0.0L;
-                for (int i = 0; i < nt; ++i) acc += (long double)(ds(b, k, i) - ds(0, 0, i)) * F.m[i];
-                const double cc = (double)(acc / m2);
-                for (int i = 0; i < nt; ++i)
-                    if (std::fabs(ds(b, k, i) - ds(0, 0, i) - cc * F.m[i]) > 2e-13 * std::max(dscale, 1e-300)) {
-                        F.why = "a detuning row is not the reference row plus a multiple of the common shape";
-                        return F;
-                    }
-                F.c[(size_t)b * N + k] = cc;
+    F.c.clear();
+    F.m.clear();
+    if (emax > 1e-13 * std::max(dscale, 1e-300)) {
+        for (;;) {
+            if (F.ns == max_shapes) {
+                F.why = max_shapes == 1 ? "a detuning row is not the reference row plus a multiple of the common shape"
+                                        : "the detuning rows need more than 4 time shapes (detuning maps, masks, noise)";
+                return F;
             }
+            // the residual row (mb, mk) of the fit so far, normalised at its largest sample, is the next shape
+            std::vector<double> row(nt);
+            for (int i = 0; i < nt; ++i) {
+                double r = ds(mb, mk, i) - ds(0, 0, i);
+                for (int s = 0; s < F.ns; ++s) r -= F.c[((size_t)mb * N + mk) * F.ns + s] * F.m[s][i];
+                row[i] = r;
+            }
+            const double norm = row[mi];
+            for (int i = 0; i < nt; ++i) row[i] /= norm;
+            F.m.push_back(std::move(row));
+            ++F.ns;
+            if (taylor_shape_factors(B, N, nt, ds, F, mb, mk, mi) <= 2e-13 * std::max(dscale, 1e-300)) break;
+        }
     }
     F.ok = true;
     return F;
@@ -1918,7 +1981,7 @@ static bool taylor_prepare(Plan& P) {
     if (!is_d2path(P)) return false;
     if (P.has_diss || P.has_collapse || P.has_slm) return false;
     if (P.desc.interp_order != 3 && P.desc.interp_order != 1) return false;
-    if (C.valid) { if (C.ok) g_taylor_why = ""; return C.ok; }
+    if (C.valid) { g_taylor_why = C.ok ? "" : C.why; return C.ok; }
     C.valid = true; C.ok = false;
     const int N = P.n, B = P.B, nt = (int)P.times.size();
     auto rows_of = [&](int b) { return (int)P.tabs[b][0].coef.size(); };
@@ -1933,8 +1996,9 @@ static bool taylor_prepare(Plan& P) {
     const SeparableFit F = taylor_separable(
         B, N, nt,
         [&](int b, int k, int i) { const PiecewiseCubic<cplx>* pc = crow[(size_t)b * N + k]; return i < npc ? pc->c0[i] : pc->y_last; },
-        [&](int b, int k, int i) { const PiecewiseCubic<double>* pc = drow[(size_t)b * N + k]; return i < npc ? pc->c0[i] : pc->y_last; });
-    if (!F.ok) { g_taylor_why = F.why; return false; }
+        [&](int b, int k, int i) { const PiecewiseCubic<double>* pc = drow[(size_t)b * N + k]; return i < npc ? pc->c0[i] : pc->y_last; },
+        PB200_TAYLOR_SMAX);
+    if (!F.ok) { g_taylor_why = C.why = F.why; return false; }
     const double scale = F.scale;
     const cplx unit = scale > 0.0 ? F.big / scale : cplx(1.0, 0.0);
     const cplx cu = std::conj(unit);
@@ -1947,25 +2011,31 @@ static bool taylor_prepare(Plan& P) {
         const cplx v0 = ref.c0[i] * cu, v1 = ref.c1[i] * cu, v2 = ref.c2[i] * cu, v3 = ref.c3[i] * cu;
         const double im = std::max(std::max(std::fabs(v0.imag()), std::fabs(v1.imag()) * hi),
                                    std::max(std::fabs(v2.imag()) * hi * hi, std::fabs(v3.imag()) * hi * hi * hi));
-        if (im > 1e-13 * scale) { g_taylor_why = "the drive phase moves in time"; return false; }
+        if (im > 1e-13 * scale) { g_taylor_why = C.why = "the drive phase moves in time"; return false; }
         C.om.c0[i] = v0.real(); C.om.c1[i] = v1.real(); C.om.c2[i] = v2.real(); C.om.c3[i] = v3.real();
     }
     C.om.y_last = (ref.y_last * cu).real();
     C.unit = {unit.real(), unit.imag()};
-    C.a = F.a; C.c = F.c; C.has_m = F.has_m;
-    if (C.has_m) C.mshape = make_interpolant<double>(P.times.data(), F.m.data(), nt, P.desc.interp_order);
-    C.uniform = (B == 1) && !C.has_m;
-    C.a_sum_max = 0.0; C.c_sum_max = 0.0;
+    C.a = F.a; C.c = F.c; C.ns = F.ns;
+    for (int s = 0; s < C.ns; ++s) C.shape[s] = make_interpolant<double>(P.times.data(), F.m[s].data(), nt, P.desc.interp_order);
+    C.drive_uniform = B == 1;
+    C.a_sum_max = 0.0;
+    for (int s = 0; s < PB200_TAYLOR_SMAX; ++s) C.c_sum_max[s] = 0.0;
     for (int b = 0; b < B; ++b) {
-        double sa = 0.0, sc = 0.0;
+        double sa = 0.0, sc[PB200_TAYLOR_SMAX] = {};
         for (int k = 0; k < N; ++k) {
-            sa += std::abs(C.a[(size_t)b * N + k]); sc += std::fabs(C.c[(size_t)b * N + k]);
-            if (std::abs(C.a[(size_t)b * N + k] - cplx(1.0, 0.0)) > 0.0) C.uniform = false;
+            sa += std::abs(C.a[(size_t)b * N + k]);
+            for (int s = 0; s < C.ns; ++s) sc[s] += std::fabs(C.c[((size_t)b * N + k) * C.ns + s]);
+            if (std::abs(C.a[(size_t)b * N + k] - cplx(1.0, 0.0)) > 0.0) C.drive_uniform = false;
         }
-        C.a_sum_max = std::max(C.a_sum_max, sa); C.c_sum_max = std::max(C.c_sum_max, sc);
+        C.a_sum_max = std::max(C.a_sum_max, sa);
+        for (int s = 0; s < C.ns; ++s) C.c_sum_max[s] = std::max(C.c_sum_max[s], sc[s]);
     }
-    if (!C.uniform) {   // static device table: a unit per BIT position (re, im), c per bit position
-        const int stride = d2_table_stride(N);
+    C.uniform = C.drive_uniform && C.ns == 0;
+    // a uniform drive keeps its gather with local detuning (stage_d2_taylor_kernel<true, ..., PB200_TAYLOR_SMAX>)
+    C.tab_shapes = (C.ns > 1 || (C.drive_uniform && C.ns == 1)) ? PB200_TAYLOR_SMAX : 0;
+    if (!C.uniform) {   // static device table: a unit per BIT position (re, im), c per (shape,) bit position
+        const int stride = C.tab_shapes ? taylor_table_stride(N, C.tab_shapes) : d2_table_stride(N);
         C.tab_host.assign((size_t)B * stride, 0.0);
         for (int b = 0; b < B; ++b) {
             double* t = C.tab_host.data() + (size_t)b * stride;
@@ -1973,7 +2043,7 @@ static bool taylor_prepare(Plan& P) {
                 const int p = N - 1 - k;
                 const cplx g = C.a[(size_t)b * N + k] * unit;
                 t[2 * p] = g.real(); t[2 * p + 1] = g.imag();
-                t[2 * N + p] = C.c[(size_t)b * N + k];
+                for (int s = 0; s < C.ns; ++s) t[2 * N + s * N + p] = C.c[((size_t)b * N + k) * C.ns + s];
             }
         }
         C.d_tab.reset(P, C.tab_host.size());
@@ -1985,21 +2055,31 @@ static bool taylor_prepare(Plan& P) {
     return true;
 }
 
-// centre and half-width of  Dint - th n_from - mv sum_k c_k n_k + om X  over the batch: the rigorous bounds build_tables
-// gives the Chebyshev path (per-excitation-number bounds of the shared Dint where they exist), without its tables
-static void taylor_bounds(const Plan& P, double om, double th, double mv, double& centre, double& half) {
+// centre and half-width of  Dint - th n_from - sum_s mv_s sum_k c_{k,s} n_k + om X  over the batch: the rigorous bounds
+// build_tables gives the Chebyshev path (per-excitation-number bounds of the shared Dint where they exist), without its
+// tables.  With local detuning e_k = sum_s mv_s c_{k,s} on a uniform drive, the local term of the excitation-count-c
+// states lies between minus the sums of the c largest and of the c smallest e_k.
+static void taylor_bounds(const Plan& P, double om, double th, const double* mv, double& centre, double& half) {
     const int N = P.n;
     const Plan::TaylorCache& C = P.tay;
     double lo = 1e300, hi = -1e300;
-    const bool caseA = C.uniform && P.has_interaction && P.dint_shared &&
+    const bool caseA = C.drive_uniform && P.has_interaction && P.dint_shared &&
                        P.desc.drives[0].state_from == P.desc.rydberg_state && !P.dmin_cnt.empty();
     if (caseA) {
         const double dr = std::fabs(om) * N;
+        std::vector<double> small(N + 1, 0.0), large(N + 1, 0.0);   // sums of the c smallest / largest e_k
+        if (C.ns) {
+            std::vector<double> e(N, 0.0);
+            for (int k = 0; k < N; ++k)
+                for (int s = 0; s < C.ns; ++s) e[k] += C.c[(size_t)k * C.ns + s] * mv[s];
+            std::sort(e.begin(), e.end());
+            for (int c = 1; c <= N; ++c) { small[c] = small[c - 1] + e[c - 1]; large[c] = large[c - 1] + e[N - c]; }
+        }
         double dlo = 1e300, dhi = -1e300;
         for (int c = 0; c <= N; ++c) {
             if (P.dmin_cnt[c] > P.dmax_cnt[c]) continue;  // empty bin
-            dlo = std::min(dlo, P.dmin_cnt[c] - th * c);
-            dhi = std::max(dhi, P.dmax_cnt[c] - th * c);
+            dlo = std::min(dlo, P.dmin_cnt[c] - th * c - large[c]);
+            dhi = std::max(dhi, P.dmax_cnt[c] - th * c - small[c]);
         }
         lo = dlo - dr; hi = dhi + dr;
     } else {
@@ -2012,7 +2092,9 @@ static void taylor_bounds(const Plan& P, double om, double th, double mv, double
             }
             for (int k = 0; k < N; ++k) {
                 dr += std::abs(C.a[(size_t)b * N + k]);
-                const double val = -(th + C.c[(size_t)b * N + k] * mv);   // diagonal of a qubit in |from>, 0 otherwise
+                double e = 0.0;
+                for (int s = 0; s < C.ns; ++s) e += C.c[((size_t)b * N + k) * C.ns + s] * mv[s];
+                const double val = -(th + e);   // diagonal of a qubit in |from>, 0 otherwise
                 dlo += std::min(0.0, val); dhi += std::max(0.0, val);
             }
             dr *= std::fabs(om);
@@ -2032,9 +2114,9 @@ static void taylor_knot_widths(Plan& P) {
     const PiecewiseCubic<double>& th_pc = P.tabs[0][0].det[0];
     C.w_knot.resize(nt);
     for (int i = 0; i < nt; ++i) {
-        double c, hw;
-        taylor_bounds(P, eval_at(C.om, P.times, P.times[i], order), eval_at(th_pc, P.times, P.times[i], order),
-                      C.has_m ? eval_at(C.mshape, P.times, P.times[i], order) : 0.0, c, hw);
+        double c, hw, mv[PB200_TAYLOR_SMAX] = {};
+        for (int s = 0; s < C.ns; ++s) mv[s] = eval_at(C.shape[s], P.times, P.times[i], order);
+        taylor_bounds(P, eval_at(C.om, P.times, P.times[i], order), eval_at(th_pc, P.times, P.times[i], order), mv, c, hw);
         C.w_knot[i] = hw;
     }
 }
@@ -2051,7 +2133,7 @@ static bool taylor_worthwhile(Plan& P, double gtol) {
     const double rate = gtol / std::max(P.times.back() - P.times.front(), 1e-30);
     const double allow = 0.25 * rate / P.n;
     std::vector<const PiecewiseCubic<double>*> pcs = {&P.tay.om, &P.tabs[0][0].det[0]};
-    if (P.tay.has_m) pcs.push_back(&P.tay.mshape);
+    for (int s = 0; s < P.tay.ns; ++s) pcs.push_back(&P.tay.shape[s]);
     std::vector<char> rough(nt, 0);
     for (const PiecewiseCubic<double>* pc : pcs) {
         const int np = pc->pieces();
@@ -2156,12 +2238,17 @@ static int taylor_order(double h, const std::vector<double>& mj, double tol, dou
 static void launch_taylor_stage(Plan& P, const PassGeom* geo, const TaylorArgs& a, long long& launches) {
     const bool uniform = a.table == nullptr;
     if (geo) {
-        constexpr int TB = kTaylorTileBits, RB = kTaylorRegBits;
+        constexpr int TB = kTaylorTileBits, RB = kTaylorRegBits, SM = PB200_TAYLOR_SMAX;
         const bool real_g = a.unit.y == 0.0;
-        dim3 grid((unsigned)(P.D >> TB), (unsigned)(uniform ? 1 : P.B)), block(1 << (TB - RB));
+        const bool local = a.tab_shapes && P.tay.drive_uniform;   // uniform drive, detuning shapes: one state
+        dim3 grid((unsigned)(P.D >> TB), (unsigned)(uniform || local ? 1 : P.B)), block(1 << (TB - RB));
         // the kernel keeps a per-bit table behind the tile unless the drive is uniform and real
-        const size_t smem = ((size_t)16 << TB) + (uniform && real_g ? 0 : (size_t)d2_table_stride(P.n) * 8);
-        if (!uniform) launch_k(stage_d2_taylor_kernel<false, false, TB, RB>, grid, block, smem, P.stream, true, a);
+        const size_t smem = a.tab_shapes ? taylor_shapes_smem(P.n)
+                                         : ((size_t)16 << TB) + (uniform && real_g ? 0 : (size_t)d2_table_stride(P.n) * 8);
+        if (local && real_g) launch_k(stage_d2_taylor_kernel<true, true, TB, RB, false, SM>, grid, block, smem, P.stream, true, a);
+        else if (local) launch_k(stage_d2_taylor_kernel<true, false, TB, RB, false, SM>, grid, block, smem, P.stream, true, a);
+        else if (a.tab_shapes) launch_k(stage_d2_taylor_kernel<false, false, TB, RB, false, SM>, grid, block, smem, P.stream, true, a);
+        else if (!uniform) launch_k(stage_d2_taylor_kernel<false, false, TB, RB>, grid, block, smem, P.stream, true, a);
         else if (real_g) launch_k(stage_d2_taylor_kernel<true, true, TB, RB>, grid, block, smem, P.stream, true, a);
         else launch_k(stage_d2_taylor_kernel<true, false, TB, RB>, grid, block, smem, P.stream, true, a);
     } else {
@@ -2183,7 +2270,8 @@ static bool taylor_geometry(const Plan& P, std::vector<PassGeom>& passes, bool& 
 // the ring it needs.  Everything here is decided a priori, before any launch of the step.
 struct TaylorStep {
     double t = 0.0, h = 0.0;
-    std::vector<double> om, th, m;   // monomial coefficients in u of omega, theta, M (trailing zeros trimmed)
+    std::vector<double> om, th;      // monomial coefficients in u of omega, theta, M_s (trailing zeros trimmed)
+    std::vector<double> m[PB200_TAYLOR_SMAX];
     int p_om = 0, p_th = 0, p = 0;
     std::vector<double> gam;         // centres of H_j
     int K = 0;
@@ -2198,11 +2286,11 @@ struct TaylorStep {
 struct TaylorScheduler {
     Plan& P;
     double t_stop, eps = 1e-12, gtol, rate, rho_target, fit_total, fit_spent = 0.0, round2 = 0.0;
-    double t, steps_len = 0.0, t_retry_len = 0.0, A_sum, C_sum, kRoundUnit = 0.05 * 1.1102230246251565e-16;
-    int order, N, nt;
+    double t, steps_len = 0.0, t_retry_len = 0.0, A_sum, C_sum[PB200_TAYLOR_SMAX], kRoundUnit = 0.05 * 1.1102230246251565e-16;
+    int order, N, nt, ns;
     bool log_steps;
     pb200_run_stats st{};
-    struct Fit { TaylorPoly om, th, m; bool ok; };
+    struct Fit { TaylorPoly om, th, m[PB200_TAYLOR_SMAX]; bool ok; };
 
     TaylorScheduler(Plan& P_, double t_start, double t_stop_, const pb200_run_opts* o) : P(P_), t_stop(t_stop_), t(t_start) {
         const double tlo = P.times.front(), thi = P.times.back();
@@ -2227,7 +2315,9 @@ struct TaylorScheduler {
                 rho_target = std::min(kTaylorRhoMax, std::max(4.0, std::log(0.2 * gtol / (kRoundUnit * std::sqrt(n_est)))));
             }
         }
-        A_sum = std::max(C.a_sum_max, 1e-300); C_sum = std::max(C.c_sum_max, 1e-300);
+        A_sum = std::max(C.a_sum_max, 1e-300);
+        ns = C.ns;
+        for (int s = 0; s < PB200_TAYLOR_SMAX; ++s) C_sum[s] = std::max(C.c_sum_max[s], 1e-300);
         // The fit error is budgeted over the call: 50 % of its share of the tolerance (10 % goes to the Taylor remainders).
         fit_total = 0.5 * rate * (t_stop - t_start);
         log_steps = env_int("PB200_TAYLOR_LOG", 0) != 0;
@@ -2241,7 +2331,8 @@ struct TaylorScheduler {
         const Plan::TaylorCache& C = P.tay;
         Fit F; F.ok = false;
         const double budget = std::max(0.5 * rate * h, 0.02 * std::max(fit_total - fit_spent, 0.0));
-        // |dH| <= r_om sum|a| + r_th N + r_M sum|c| : a third of the step's allowance each
+        // |dH| <= r_om sum|a| + r_th N + sum_s r_Ms sum|c_s| : a third of the step's allowance each, the shapes' third
+        // shared equally
         const double third = budget / (3.0 * h);
         // smallest passing degree; a candidate that spans several intervals is first tried at the highest degree so
         // that a step across a non-smooth sample is refused after one fit instead of PB200_TAYLOR_PMAX + 1
@@ -2258,8 +2349,8 @@ struct TaylorScheduler {
             return true;
         };
         F.ok = one(C.om, F.om, third / A_sum) && one(P.tabs[0][0].det[0], F.th, third / N);
-        if (F.ok && C.has_m) F.ok = one(C.mshape, F.m, third / C_sum);
-        if (!C.has_m) { F.m.c.assign(1, 0.0); F.m.resid = 0.0; }
+        for (int s = 0; s < ns && F.ok; ++s) F.ok = one(C.shape[s], F.m[s], third / ns / C_sum[s]);
+        for (int s = ns; s < PB200_TAYLOR_SMAX; ++s) { F.m[s].c.assign(1, 0.0); F.m[s].resid = 0.0; }
         return F;
     }
 
@@ -2315,28 +2406,37 @@ struct TaylorScheduler {
             auto trim = [](std::vector<double>& c, double scale) {
                 while (c.size() > 1 && std::fabs(c.back()) <= 1e-15 * scale) c.pop_back();
             };
+            int p_m = 0;
             {
-                double so = 0.0, sh = 0.0, sm = 0.0;
+                double so = 0.0, sh = 0.0;
                 for (double v : F.om.c) so = std::max(so, std::fabs(v));
                 for (double v : F.th.c) sh = std::max(sh, std::fabs(v));
-                for (double v : F.m.c) sm = std::max(sm, std::fabs(v));
-                trim(F.om.c, std::max(so, 1e-300)); trim(F.th.c, std::max(sh, 1e-300)); trim(F.m.c, std::max(sm, 1e-300));
+                trim(F.om.c, std::max(so, 1e-300)); trim(F.th.c, std::max(sh, 1e-300));
+                for (int q = 0; q < PB200_TAYLOR_SMAX; ++q) {
+                    double sm = 0.0;
+                    for (double v : F.m[q].c) sm = std::max(sm, std::fabs(v));
+                    trim(F.m[q].c, std::max(sm, 1e-300));
+                    p_m = std::max(p_m, (int)F.m[q].c.size() - 1);
+                }
             }
-            const int p_om = (int)F.om.c.size() - 1, p_m = (int)F.m.c.size() - 1;
+            const int p_om = (int)F.om.c.size() - 1;
             const int p_th = std::max((int)F.th.c.size() - 1, p_m);   // degree of the diagonal (own-element) history
             const int p = std::max(p_om, p_th);
             auto th_c = [&](int j) { return j < (int)F.th.c.size() ? F.th.c[j] : 0.0; };
-            auto m_c = [&](int j) { return j < (int)F.m.c.size() ? F.m.c[j] : 0.0; };
+            auto m_c = [&](int q, int j) { return j < (int)F.m[q].c.size() ? F.m[q].c[j] : 0.0; };
             // centres and norm bounds of H_j
             std::vector<double> gam(p + 1, 0.0), mj(p + 1, 0.0);
             {
-                double c0, hw0;
-                taylor_bounds(P, F.om.c[0], F.th.c[0], m_c(0), c0, hw0);
+                double c0, hw0, mv[PB200_TAYLOR_SMAX];
+                for (int q = 0; q < PB200_TAYLOR_SMAX; ++q) mv[q] = m_c(q, 0);
+                taylor_bounds(P, F.om.c[0], F.th.c[0], mv, c0, hw0);
                 gam[0] = c0; mj[0] = hw0;
                 for (int j = 1; j <= p; ++j) {
                     const double thj = th_c(j), omj = j <= p_om ? F.om.c[j] : 0.0;
                     gam[j] = -thj * 0.5 * N;
-                    mj[j] = std::fabs(thj) * 0.5 * N + std::fabs(m_c(j)) * C_sum + std::fabs(omj) * A_sum;
+                    double mm = 0.0;
+                    for (int q = 0; q < ns; ++q) mm += std::fabs(m_c(q, j)) * C_sum[q];
+                    mj[j] = std::fabs(thj) * 0.5 * N + mm + std::fabs(omj) * A_sum;
                 }
             }
             {   // the fp64 cancellation of the series grows like e^rho: a step whose majorant exponent overshoots the
@@ -2352,7 +2452,8 @@ struct TaylorScheduler {
             double trunc_bound = 0.0;
             const int K = taylor_order(h, mj, std::max(1e-15, 0.1 * rate * h), trunc_bound);
             s.t = t; s.h = h;
-            s.om = F.om.c; s.th = F.th.c; s.m = F.m.c;
+            s.om = F.om.c; s.th = F.th.c;
+            for (int q = 0; q < PB200_TAYLOR_SMAX; ++q) s.m[q] = F.m[q].c;
             s.p_om = p_om; s.p_th = p_th; s.p = p;
             s.gam = gam; s.K = K;
             s.n_chi = p_th + 2;
@@ -2364,11 +2465,13 @@ struct TaylorScheduler {
             st.n_applies += K; st.n_exponentials += 1; ++st.n_steps;
             if (log_steps)
                 fprintf(stderr, "taylor step t=%.6f h_ns=%.3f p_om=%d p_th=%d p_m=%d K=%d ring=%d rho=%.3f resid=%.2e/%.2e/%.2e\n", t,
-                        h * 1e3, p_om, p_th, p_m, K, s.ring() + 1, mj[0] * h, F.om.resid, F.th.resid, F.m.resid);
+                        h * 1e3, p_om, p_th, p_m, K, s.ring() + 1, mj[0] * h, F.om.resid, F.th.resid, F.m[0].resid);
             double rho_eff = 0.0;
             for (int j = 0; j <= p; ++j) rho_eff += mj[j] / (j + 1);
             st.max_rho = std::max(st.max_rho, rho_eff * h);
-            const double fit_err = h * (A_sum * F.om.resid + N * F.th.resid + C_sum * F.m.resid);
+            double fit_m = 0.0;
+            for (int q = 0; q < ns; ++q) fit_m += C_sum[q] * F.m[q].resid;
+            const double fit_err = h * (A_sum * F.om.resid + N * F.th.resid + fit_m);
             st.err_estimate += trunc_bound + fit_err;
             fit_spent += fit_err;
             { const double r = kRoundUnit * std::exp(std::min(rho_eff * h, 40.0)); round2 += r * r; }
@@ -2427,7 +2530,7 @@ static TaylorRing taylor_ring(Plan& P, const TaylorStep& s) {
 static TaylorArgs taylor_args(const Plan& P, const PassGeom& geo, const TaylorStep& s, const TaylorRing& R, int k) {
     const Plan::TaylorCache& C = P.tay;
     auto th_c = [&](int j) { return j < (int)s.th.size() ? s.th[j] : 0.0; };
-    auto m_c = [&](int j) { return j < (int)s.m.size() ? s.m[j] : 0.0; };
+    auto m_c = [&](int q, int j) { return j < (int)s.m[q].size() ? s.m[q][j] : 0.0; };
     TaylorArgs a{};
     a.v = R.chi[k % s.n_chi]; a.out = R.chi[(k + 1) % s.n_chi];
     a.g_out = (s.n_g && k + 1 < s.K) ? R.gr[k % s.n_g] : nullptr;
@@ -2438,14 +2541,18 @@ static TaylorArgs taylor_args(const Plan& P, const PassGeom& geo, const TaylorSt
     a.geo = geo;
     a.unit = C.unit;
     a.table = C.uniform ? nullptr : C.d_tab.get();
+    a.tab_shapes = C.tab_shapes;
     a.to_bit = P.desc.drives[0].state_to; a.from_is_one = P.desc.drives[0].state_from;
-    a.th0 = s.th[0]; a.gam0 = s.gam[0]; a.om0 = s.om[0]; a.m0 = m_c(0);
+    a.th0 = s.th[0]; a.gam0 = s.gam[0]; a.om0 = s.om[0];
+    for (int q = 0; q < PB200_TAYLOR_SMAX; ++q) a.m0[q] = m_c(q, 0);
     a.scale = {0.0, -s.h / (k + 1)};
     a.nh = std::min(s.p, k);
     for (int j = 1; j <= a.nh; ++j) {
-        const double thj = th_c(j), mjv = m_c(j), omj = j <= s.p_om ? s.om[j] : 0.0;
-        a.hth[j - 1] = thj; a.hgam[j - 1] = s.gam[j]; a.hom[j - 1] = omj; a.hm[j - 1] = mjv;
-        a.hchi[j - 1] = (thj != 0.0 || mjv != 0.0 || s.gam[j] != 0.0) ? R.chi[(k - j) % s.n_chi] : nullptr;
+        const double thj = th_c(j), omj = j <= s.p_om ? s.om[j] : 0.0;
+        bool any_m = false;
+        for (int q = 0; q < PB200_TAYLOR_SMAX; ++q) { a.hm[q][j - 1] = m_c(q, j); any_m = any_m || a.hm[q][j - 1] != 0.0; }
+        a.hth[j - 1] = thj; a.hgam[j - 1] = s.gam[j]; a.hom[j - 1] = omj;
+        a.hchi[j - 1] = (thj != 0.0 || any_m || s.gam[j] != 0.0) ? R.chi[(k - j) % s.n_chi] : nullptr;
         a.hg[j - 1] = (omj != 0.0) ? R.gr[(k - j) % s.n_g] : nullptr;
     }
     const bool last = (k + 1 == s.K);
@@ -2578,9 +2685,15 @@ static PassGeom shard_geometry(const Plan& P) {
 
 // one order on one shard; no programmatic dependent launch: an order waits for its peers through events
 static void launch_taylor_shard(Plan& P, const TaylorArgs& a) {
-    constexpr int TB = kTaylorTileBits, RB = kTaylorRegBits;
+    constexpr int TB = kTaylorTileBits, RB = kTaylorRegBits, SM = PB200_TAYLOR_SMAX;
     const bool real_g = a.unit.y == 0.0;
     dim3 grid((unsigned)(P.D >> TB)), block(1 << (TB - RB));
+    if (a.table) {   // detuning shapes (the drive of a shard is uniform: pb200_shards_link)
+        const size_t smem = taylor_shapes_smem(P.n);
+        if (real_g) launch_k(stage_d2_taylor_kernel<true, true, TB, RB, true, SM>, grid, block, smem, P.stream, false, a);
+        else launch_k(stage_d2_taylor_kernel<true, false, TB, RB, true, SM>, grid, block, smem, P.stream, false, a);
+        return;
+    }
     const size_t smem = ((size_t)16 << TB) + (real_g ? 0 : (size_t)d2_table_stride(P.n) * 8);
     if (real_g) launch_k(stage_d2_taylor_kernel<true, true, TB, RB, true>, grid, block, smem, P.stream, false, a);
     else launch_k(stage_d2_taylor_kernel<true, false, TB, RB, true>, grid, block, smem, P.stream, false, a);
@@ -2636,6 +2749,9 @@ static void shards_apply_h(const std::vector<Plan*>& G, double t, const std::vec
         a.v = in[r]; a.out = out[r];
         a.dint = P.has_interaction ? P.dint.get() : nullptr;
         a.D = P.D; a.geo = geo; a.unit = P.tay.unit;
+        a.table = P.tay.uniform ? nullptr : P.tay.d_tab.get();
+        a.tab_shapes = P.tay.tab_shapes;
+        for (int s = 0; s < P.tay.ns; ++s) a.m0[s] = eval_at(P.tay.shape[s], P.times, t, order);
         a.to_bit = P.desc.drives[0].state_to; a.from_is_one = P.desc.drives[0].state_from;
         a.th0 = th; a.om0 = om;
         a.scale = {1.0, 0.0};
@@ -3496,8 +3612,9 @@ int pb200_shards_link(pb200_plan** plans, int32_t count) {
             fail(PB200_ERR_INVALID, "pb200_shards_link: every shard needs the same (shared) interaction");
         if (!P.tabs_set[0][0]) fail(PB200_ERR_STATE, "pb200_shards_link: the drive of shard %d is not set", i);
         if (!taylor_prepare(P)) fail(PB200_ERR_UNSUPPORTED, "pb200_shards_link: no Taylor propagator for this sequence: %s", g_taylor_why);
-        if (!P.tay.uniform)
-            fail(PB200_ERR_UNSUPPORTED, "pb200_shards_link: shards need one drive coefficient for every qubit (per-qubit factors are not sharded)");
+        if (!P.tay.drive_uniform)
+            fail(PB200_ERR_UNSUPPORTED, "pb200_shards_link: shards need one drive coefficient for every qubit (per-qubit drive "
+                                        "amplitudes are not sharded; per-qubit detuning is)");
     }
     // peer access between distinct devices of neighbouring shards (a flip of one shard bit)
     for (int i = 0; i < count; ++i)
@@ -3780,8 +3897,33 @@ int pb200_host_taylor_separable(const double* coef, const double* det, int32_t n
         // the factors refer to the reference row: report them scaled by its phase so that coef = a x |ref row| shape
         if (a_out)
             for (size_t x = 0; x < F.a.size(); ++x) { a_out[2 * x] = F.a[x].real(); a_out[2 * x + 1] = F.a[x].imag(); }
-        if (c_out) for (size_t x = 0; x < F.c.size(); ++x) c_out[x] = F.c[x];
-        if (m_out) for (size_t i = 0; i < F.m.size(); ++i) m_out[i] = F.m[i];
+        if (c_out) for (size_t x = 0; x < (size_t)n_traj * N; ++x) c_out[x] = F.ns ? F.c[x] : 0.0;
+        if (m_out) for (size_t i = 0; i < nt; ++i) m_out[i] = F.ns ? F.m[0][i] : 0.0;
+    }
+    PB200_CATCH
+}
+
+int pb200_host_taylor_shapes(const double* coef, const double* det, int32_t n_traj, int32_t n_qudits, int32_t n_times,
+                             int32_t max_shapes, int32_t* n_shapes, double* a_out, double* c_out, double* m_out) {
+    PB200_TRY
+    if (!coef || !det || !n_shapes || n_traj < 1 || n_qudits < 1 || n_times < 2 || max_shapes < 0 ||
+        max_shapes > PB200_TAYLOR_SMAX)
+        fail(PB200_ERR_INVALID, "bad argument");
+    const cplx* y = reinterpret_cast<const cplx*>(coef);
+    const size_t nt = (size_t)n_times, N = (size_t)n_qudits, S = (size_t)max_shapes;
+    const SeparableFit F = taylor_separable(
+        n_traj, n_qudits, n_times, [&](int b, int k, int i) { return y[((size_t)b * N + k) * nt + i]; },
+        [&](int b, int k, int i) { return det[((size_t)b * N + k) * nt + i]; }, max_shapes);
+    *n_shapes = F.ok ? F.ns : -1;
+    if (F.ok) {
+        if (a_out)
+            for (size_t x = 0; x < F.a.size(); ++x) { a_out[2 * x] = F.a[x].real(); a_out[2 * x + 1] = F.a[x].imag(); }
+        if (c_out)
+            for (size_t x = 0; x < (size_t)n_traj * N; ++x)
+                for (size_t s = 0; s < S; ++s) c_out[x * S + s] = (int)s < F.ns ? F.c[x * F.ns + s] : 0.0;
+        if (m_out)
+            for (size_t s = 0; s < S; ++s)
+                for (size_t i = 0; i < nt; ++i) m_out[s * nt + i] = (int)s < F.ns ? F.m[s][i] : 0.0;
     }
     PB200_CATCH
 }

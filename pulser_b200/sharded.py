@@ -7,8 +7,8 @@ an ordinary plan on ``devices[i]`` (several shards may share a device), and one 
 them all: ``pb200_shards_propagate`` runs every order of the time-dependent Taylor series on every
 shard, whose partners across the shard bits are read from the peers' slices.
 
-Scope: what the Taylor propagator takes with one state -- d = 2, one global drive of constant
-phase, Ising interaction.  The methods mirror the single-state methods of ``DevicePlan`` that
+Scope: what the Taylor propagator takes with one state -- d = 2, one global drive amplitude of
+constant phase, per-qubit detuning of up to 4 time shapes (detuning maps), Ising interaction.  The methods mirror the single-state methods of ``DevicePlan`` that
 ``B200Backend._stream``, ``DeviceStateView`` and ``DeviceHamiltonian`` call, with the same shapes
 (a leading trajectory axis of 1).
 """
@@ -102,9 +102,12 @@ class ShardedPlan:
                 f"{self.G} shards of a {self.n}-qubit state hold 2^{self.L} amplitudes each; a shard holds "
                 f"2^{MIN_LOCAL_BITS} to 2^{MAX_LOCAL_BITS}"
             )
-        if spec.interaction_type == "XY" or len(spec.drives) != 1 or not spec.drives[0].uniform:
+        # per-qubit detuning (detuning maps) is the library's to accept or refuse; drive amplitudes must be global
+        coef = np.asarray(spec.drives[0].coef) if len(spec.drives) == 1 else None
+        if spec.interaction_type == "XY" or coef is None or not (coef == coef[:1]).all():
             raise NotImplementedError(
-                "state-vector shards need one global drive (no XY interaction, per-qubit drives or several bases)"
+                "state-vector shards need one global drive (no XY interaction, per-qubit drive amplitudes or several "
+                "bases)"
             )
         self.D = spec.hilbert_dim
         self.Dl = 1 << self.L

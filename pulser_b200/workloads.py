@@ -224,6 +224,25 @@ def noisy_trajectory_spec(base: HamiltonianSpec, coords: np.ndarray, doppler: np
     return spec
 
 
+def detuning_map_spec(base: HamiltonianSpec, maps) -> HamiltonianSpec:
+    """Detuning maps on a ground-rydberg sequence: ``maps`` is a list of ``(weights, waveform)``, one per detuning map
+    modulator (``Sequence.config_detuning_map`` + ``add_dmm_detuning``); atom k's detuning gains
+    ``sum weights[k] * waveform(t)``, as the reference samples it (``samples.py:560-601``: det += cs.det * weight).
+    A waveform has one sample per ns; the zero-padded extra sample gets 0.  All samples become Local."""
+    import copy
+
+    d0 = base.drives[0]
+    nt = d0.det.shape[1]
+    det = np.array(d0.det, dtype=float)
+    for weights, waveform in maps:
+        wf = np.zeros(nt)
+        wf[: len(waveform)] = waveform
+        det = det + np.outer(np.asarray(weights, dtype=float), wf)
+    spec = copy.copy(base)
+    spec.drives = [DriveTable(d0.basis, np.array(d0.coef), det, False)]
+    return spec
+
+
 def config_c4_stream(n_traj: int = 1024, seed: int = 4, side: int = 4, temperature: float = 50.0,
                      amp_sigma: float = 0.05, laser_waist: float = 175.0, keep=None):
     """Generator over the C4 trajectories in order: yields ``(j, spec)``; with ``keep`` (a set of indices) the other
