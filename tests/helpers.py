@@ -80,6 +80,37 @@ def open_spec(
     )
 
 
+def curved_spec(n: int, T: int = 300, phase: float = 0.0, seed: int = 3, radius: float = 20.0,
+                min_dist: float = 6.0, swing: float = 14.0) -> HamiltonianSpec:
+    """Global drive with a Blackman amplitude (peak ~8 rad/us whatever T) and a sin^2 detuning of amplitude ``swing``:
+    smooth curved waveforms, so that a polynomial of degree above 3 spans several sampling intervals"""
+    t = np.arange(T)
+    amp = W.blackman(T, 2.2 * np.pi * T / 600)
+    det = -6.0 + swing * np.sin(1.3 * np.pi * t / T) ** 2
+    coords = W.disc_register(n, radius, min_dist, seed)
+    return W.ising_global_spec(coords, W.C6_LEVEL_60, amp, det, phase=phase)
+
+
+def dmm_waveforms(T: int) -> list[np.ndarray]:
+    """four detuning-map waveforms of different time shapes (negative, as a DMM allows)"""
+    t = np.arange(T)
+    return [
+        -4.0 * np.sin(np.pi * t / T) ** 2,
+        -np.concatenate([np.linspace(0.0, 5.0, T // 2), np.full(T - T // 2, 5.0)]),
+        -2.0 * (1.0 + np.sin(5.0 * np.pi * t / T)),
+        -1.5 * np.cos(3.0 * np.pi * t / T) ** 2,
+    ]
+
+
+def with_dmm(base: HamiltonianSpec, n_maps: int, seed: int = 0) -> HamiltonianSpec:
+    """``base`` plus ``n_maps`` detuning maps with random weights on different subsets of the atoms"""
+    n = base.n_qudits
+    rng = np.random.default_rng(seed)
+    wfs = dmm_waveforms(base.total_duration_ns)
+    maps = [(rng.uniform(0.2, 1.0, n) * (np.arange(n) % (s + 2) != 0), wfs[s]) for s in range(n_maps)]
+    return W.detuning_map_spec(base, maps)
+
+
 def random_state(D: int, seed: int = 0) -> np.ndarray:
     rng = np.random.default_rng(seed)
     v = rng.normal(size=D) + 1j * rng.normal(size=D)
