@@ -95,8 +95,9 @@ typedef struct pb200_run_opts {
                                  order); -1: plain 4th-order steps */
     int32_t integrator;       /* 1 Chebyshev-Clenshaw / 2 Lanczos (Krylov) exponentials of
                                  Richardson-CF4 Magnus steps; 3 time-dependent Taylor
-                                 series (one global drive of constant phase, d = 2, one
-                                 state: no Magnus error, ~1 H-apply per ns on C2);
+                                 series (one global drive, its phase constant or
+                                 moving, d = 2, one state: no Magnus error, ~1
+                                 H-apply per ns on C2);
                                  0 auto: 3 where it applies, else 2 for strongly
                                  blockaded / HBM-resident registers, else 1 */
 } pb200_run_opts;
@@ -307,7 +308,7 @@ int pb200_bench_apply(pb200_plan* plan, double t_us, int32_t reps,
 int pb200_plan_create_shard(pb200_plan** out, const pb200_plan_desc* desc,
                             int32_t shard_bits, int32_t shard_index);
 /* Link the G shards plans[i] = shard i (after their uploads): checks N, sampling
- * times and the Taylor structure (global drive of constant phase), merges the
+ * times and the Taylor structure (one global drive, of any phase), merges the
  * interaction bounds so that every shard schedules exactly like the unsharded
  * plan, enables peer access between distinct devices (PB200_ERR_UNSUPPORTED
  * where it is impossible). */

@@ -313,14 +313,26 @@ __device__ __forceinline__ c2 ld_own(const c2* p) {
     return {r.x, r.y};
 }
 
+// one partner of a complex-drive Taylor stage: z = f chi (f = gx + i gy, the factor of the partner's transition),
+// p += z, q += sg z
+__device__ __forceinline__ void taylor_signed_add(double gx, double gy, double sg, double x, double y, double& pr, double& pi,
+                                                  double& qr, double& qi) {
+    const double zx = fma(gx, x, -gy * y), zy = fma(gx, y, gy * x);
+    pr += zx; pi += zy;
+    qr = fma(sg, zx, qr); qi = fma(sg, zy, qi);
+}
+
 // In-tile partner sums of the R = 2^RB amplitudes a thread owns (tile index t = tid + r*NT): flips of the
 // register-block bits (tile bits TBITS-RB .. TBITS-1) are register moves, flips of the tile bits
 // [jstart, TBITS-RB) are independent LDS.128 from `tile`.
-template <bool UNIFORM, bool REAL_G, int TBITS, int RB>
+// SIGNED (per-bit table only): q also receives the signed sum  sum_k sg_k f_k chi_k,  sg_k = +1 where the amplitude's bit
+// k is to_bit, with f_k the factor p receives (the complex-drive Taylor stage).
+template <bool UNIFORM, bool REAL_G, int TBITS, int RB, bool SIGNED = false>
 __device__ __forceinline__ void rb_tile_gather(const PassGeom& g, const c2* tile, const double* __restrict__ tab, int tid,
                                                int to_bit, int jstart, bool skip_smem, const c2 (&v)[1 << RB],
                                                double (&pr)[1 << RB], double (&pi)[1 << RB], double (&qr)[1 << RB],
                                                double (&qi)[1 << RB]) {
+    static_assert(!SIGNED || !UNIFORM, "signed sums of the per-bit table gather");
     constexpr int R = 1 << RB;
     constexpr int NT = 1 << (TBITS - RB);
     // --- flips inside the register block (tile bits TBITS-RB .. TBITS-1) ---
@@ -341,6 +353,9 @@ __device__ __forceinline__ void rb_tile_gather(const PassGeom& g, const c2* tile
                 if (!REAL_G) {
                     if (bit == to_bit) { qr[r] += pv.x; qi[r] += pv.y; } else { qr[r] -= pv.x; qi[r] -= pv.y; }
                 }
+            } else if constexpr (SIGNED) {
+                const double gy = (bit == to_bit) ? gyt : -gyt;
+                taylor_signed_add(gx, gy, bit == to_bit ? 1.0 : -1.0, pv.x, pv.y, pr[r], pi[r], qr[r], qi[r]);
             } else {
                 const double gy = (bit == to_bit) ? gyt : -gyt;
                 pr[r] = fma(gx, pv.x, pr[r]); pr[r] = fma(-gy, pv.y, pr[r]);
@@ -367,6 +382,8 @@ __device__ __forceinline__ void rb_tile_gather(const PassGeom& g, const c2* tile
                 if (UNIFORM) {
                     pr[r] += pv.x; pi[r] += pv.y;
                     if (!REAL_G) { qr[r] = fma(sg, pv.x, qr[r]); qi[r] = fma(sg, pv.y, qi[r]); }
+                } else if constexpr (SIGNED) {
+                    taylor_signed_add(gx, gy, sg, pv.x, pv.y, pr[r], pi[r], qr[r], qi[r]);
                 } else {
                     pr[r] = fma(gx, pv.x, pr[r]); pr[r] = fma(-gy, pv.y, pr[r]);
                     pi[r] = fma(gx, pv.y, pi[r]); pi[r] = fma(gy, pv.x, pi[r]);
@@ -744,7 +761,7 @@ __global__ void __launch_bounds__(1 << (TBITS - RB), 2) stage_d2_fwd_kernel(cons
     }
 }
 
-// ---- d = 2 stage kernel of the time-dependent Taylor propagator (one drive time shape of constant phase) ---------
+// ---- d = 2 stage kernel of the time-dependent Taylor propagator (one drive time shape, its phase constant or moving) -
 // On a step [a, a+h] the interpolated coefficients (QobjEvo's cubic splines, hamiltonian.py:436) are polynomials in
 // u = (t-a)/h:  H(u) = sum_j H_j u^j,  H_0 = Dint - th_0 n_from - gam_0 + om_0 X,  H_j = -th_j n_from - gam_j + om_j X
 // with X = sum_k (unit |to><from|_k + h.c.).  psi(u) = sum_k chi_k u^k solves psi' = -i h H(u) psi exactly when
@@ -753,7 +770,8 @@ __global__ void __launch_bounds__(1 << (TBITS - RB), 2) stage_d2_fwd_kernel(cons
 // products, no host synchronisation; the step length is bounded by the spectral width (rho = h W, fp64
 // cancellation: rho <= 14) and by the polynomial fit of the splines only.  The stage computes chi_{k+1} from the tile of chi_k,
 // optionally stores G_k for later orders and folds chi_k + chi_{k+1} into the accumulator of psi(1) on every other
-// order.  Replaces qutip.sesolve (simulation.py:729-735) for global drives of constant phase, and -- with per-qubit
+// order.  Replaces qutip.sesolve (simulation.py:729-735) for global drives (a phase that moves inside a step: the CPLX
+// instantiations, two gathers per order), and -- with per-qubit
 // static factors from a per-trajectory table (TaylorArgs::table) -- the trajectory loop's solves (simulation.py:885-915).
 #define PB200_TAYLOR_PMAX 8
 #define PB200_MAX_SHARD_BITS 3
@@ -771,7 +789,7 @@ struct TaylorArgs {
     long long dint_stride;  // 0: Dint shared by the trajectories
     long long D;
     PassGeom geo;
-    c2 unit;           // uniform drive: e^{-i phi}, the constant phase
+    c2 unit;           // uniform drive: e^{-i phi}, the drive's phase on the step (TaylorStep::unit)
     // separable per-qubit drives (trajectory batches with static noise): coef_{b,k}(t) = a_{b,k} unit omega(t),
     // det_{b,k}(t) = theta(t) + c_{b,k} M(t).  table[b][0 .. 2N) = a unit per BIT position (re, im),
     // table[b][2N .. 3N) = c per bit position (layout of d2_table_stride); nullptr in the uniform case.
@@ -796,6 +814,13 @@ struct TaylorArgs {
     // of shard (shard ^ 1 << q): a flip of shard bit q leaves the local index unchanged
     const c2* peer[PB200_MAX_SHARD_BITS];
     int shard_bits, shard;
+    // complex drive on the step (stage kernels with CPLX = true): omega_j = om_j + i omi_j, so the drive part of H_j
+    // chi is om_j G + omi_j G', G' = X' chi the gather with factors i unit (X' = sum_k (i unit |to><from|_k + h.c.)).
+    // Both come from the same partner loads: G = P + Q, G' = i (P - Q) with P, Q the to-side and from-side sums.
+    c2* g2_out;        // G'_k (nullptr: nobody reads it later)
+    double om0i;
+    const c2* hg2[PB200_TAYLOR_PMAX];    // G'_{k-j}   (nullptr when omi_j = 0)
+    double homi[PB200_TAYLOR_PMAX];
 };
 
 // epilogue of one amplitude block: everything after the partner sums.  idx is the index inside the trajectory, voff
@@ -804,10 +829,12 @@ struct TaylorArgs {
 // r is either `off[r]` = sum_k c_k [digit_k == from] of the one shape (0 for uniform drives), or, with several shapes,
 // a functor off(r, J) = sum_s m_{s,J} sum_k c_{k,s} [digit_k == from] with the shapes' order-0 coefficients (J = 0)
 // or those of history term J - 1.
-template <int R, int H = (R >= 4) ? R / 2 : R, bool SHARD = false, class Off>
+// CPLX: (qx, qy) is G' of the complex-drive step.
+template <int R, int H = (R >= 4) ? R / 2 : R, bool SHARD = false, bool CPLX = false, class Off>
 __device__ __forceinline__ void taylor_epilogue(const TaylorArgs& a, const long long (&idx)[R], const c2 (&v)[R],
                                                 const double (&gx)[R], const double (&gy)[R], const Off& off,
-                                                long long voff, const double* __restrict__ dsrc) {
+                                                long long voff, const double* __restrict__ dsrc,
+                                                const double* qx = nullptr, const double* qy = nullptr) {
     constexpr bool SHAPES = !std::is_array<Off>::value;
     const int nb = a.geo.n_bits;
     const int ones_hi = SHARD ? __popc(a.shard) : 0;
@@ -827,6 +854,7 @@ __device__ __forceinline__ void taylor_epilogue(const TaylorArgs& a, const long 
                 else diag = fma(-a.th0, cn[r], fma(-a.m0[0], off[h0 + r], dv[r] - a.gam0));
                 sx[r] = fma(diag, v[h0 + r].x, a.om0 * gx[h0 + r]);
                 sy[r] = fma(diag, v[h0 + r].y, a.om0 * gy[h0 + r]);
+                if constexpr (CPLX) { sx[r] = fma(a.om0i, qx[h0 + r], sx[r]); sy[r] = fma(a.om0i, qy[h0 + r], sy[r]); }
             }
         }
         for (int j = 0; j < a.nh; ++j) {
@@ -849,6 +877,15 @@ __device__ __forceinline__ void taylor_epilogue(const TaylorArgs& a, const long 
 #pragma unroll
                 for (int r = 0; r < H; ++r) { sx[r] = fma(a.hom[j], c[r].x, sx[r]); sy[r] = fma(a.hom[j], c[r].y, sy[r]); }
             }
+            if constexpr (CPLX) {
+                if (a.hg2[j]) {
+                    c2 c[H];
+#pragma unroll
+                    for (int r = 0; r < H; ++r) c[r] = ld_own(a.hg2[j] + voff + idx[h0 + r]);
+#pragma unroll
+                    for (int r = 0; r < H; ++r) { sx[r] = fma(a.homi[j], c[r].x, sx[r]); sy[r] = fma(a.homi[j], c[r].y, sy[r]); }
+                }
+            }
         }
         c2 res[H];
 #pragma unroll
@@ -858,6 +895,7 @@ __device__ __forceinline__ void taylor_epilogue(const TaylorArgs& a, const long 
             // (C2 on H100: the ring is twice the 50 MB L2; 42.9 against 44.1 us per order, DESIGN.md section 8)
             st_c2_evict_last(a.out + voff + idx[h0 + r], res[r]);
             if (a.g_out) st_c2(a.g_out + voff + idx[h0 + r], c2{gx[h0 + r], gy[h0 + r]});
+            if constexpr (CPLX) { if (a.g2_out) st_c2(a.g2_out + voff + idx[h0 + r], c2{qx[h0 + r], qy[h0 + r]}); }
         }
         if (a.acc_on) {
             c2 ac[H];
@@ -887,12 +925,17 @@ __device__ __forceinline__ void taylor_epilogue(const TaylorArgs& a, const long 
 // the combinations sum_s m_{s,J} off_s of the order's coefficients enter the diagonal, so they are formed once per
 // launch in shared memory (per thread for the bits of base + tid, per register-bit pattern for the rest) and an
 // amplitude reads two of them per history term instead of holding S offsets in registers.
-template <bool UNIFORM, bool REAL_G, int TBITS, int RB, bool SHARD = false, int NS = (UNIFORM ? 0 : 1)>
-__global__ void __launch_bounds__(1 << (TBITS - RB), (65536 / ((1 << (TBITS - RB)) * (RB >= 3 ? 128 : 64))))
+// CPLX: the drive's phase moves inside the step (TaylorArgs::om0i, hg2, g2_out): the per-bit table gather also forms
+// the signed sum P - Q of the same partner loads, i.e. G' as well as G.  The two sums of a chunk do not fit in 128
+// registers; these launches use fewer threads with more chunks each (kTaylorCplxRegBits) and one CTA's worth of
+// registers per SM.
+template <bool UNIFORM, bool REAL_G, int TBITS, int RB, bool SHARD = false, int NS = (UNIFORM ? 0 : 1), bool CPLX = false>
+__global__ void __launch_bounds__(1 << (TBITS - RB), CPLX ? 1 : (65536 / ((1 << (TBITS - RB)) * (RB >= 3 ? 128 : 64))))
 stage_d2_taylor_kernel(const __grid_constant__ TaylorArgs a) {
     static_assert(RB >= 3, "chunks of 8 amplitudes per thread");
     static_assert(UNIFORM || !SHARD, "shards carry one state with a uniform drive");
     static_assert(NS == (UNIFORM ? 0 : 1) || NS == PB200_TAYLOR_SMAX, "one-shape table, or PB200_TAYLOR_SMAX shapes");
+    static_assert(!CPLX || !REAL_G, "a complex drive gathers through the per-bit table");
     constexpr bool SHAPES = NS == PB200_TAYLOR_SMAX;
     constexpr int NT = 1 << (TBITS - RB);
     constexpr int TSIZE = 1 << TBITS;
@@ -989,8 +1032,9 @@ stage_d2_taylor_kernel(const __grid_constant__ TaylorArgs a) {
     for (int c = 0; c < (1 << CB); ++c) {
         const long long i0 = base + tid + c * RC * NT;   // index of the chunk's first amplitude; the r-th is i0 + r*NT
         double pr[RC], pi[RC];
+        double dr[RC], di[RC];   // CPLX: signed sums P - Q
 #pragma unroll
-        for (int r = 0; r < RC; ++r) { pr[r] = 0.0; pi[r] = 0.0; }
+        for (int r = 0; r < RC; ++r) { pr[r] = 0.0; pi[r] = 0.0; dr[r] = 0.0; di[r] = 0.0; }
         // partners across the bits outside the tile: coalesced loads (for the first chunk, while the tile is in flight)
         for (unsigned long long m = g.extra_mask; m; m &= m - 1) {
             const int p = __ffsll((long long)m) - 1;
@@ -1003,7 +1047,9 @@ stage_d2_taylor_kernel(const __grid_constant__ TaylorArgs a) {
             for (int r = 0; r < RC; ++r) raw[r] = __ldg(reinterpret_cast<const double2*>(src + r * NT));
 #pragma unroll
             for (int r = 0; r < RC; ++r) {
-                if (!TAB) {
+                if constexpr (CPLX) {
+                    taylor_signed_add(gx, gy, bit == to_bit ? 1.0 : -1.0, raw[r].x, raw[r].y, pr[r], pi[r], dr[r], di[r]);
+                } else if (!TAB) {
                     pr[r] += raw[r].x; pi[r] += raw[r].y;
                 } else {
                     pr[r] = fma(gx, raw[r].x, pr[r]); pr[r] = fma(-gy, raw[r].y, pr[r]);
@@ -1027,7 +1073,9 @@ stage_d2_taylor_kernel(const __grid_constant__ TaylorArgs a) {
                 for (int r = 0; r < RC; ++r) raw[r] = *reinterpret_cast<const double2*>(src + r * NT);
 #pragma unroll
                 for (int r = 0; r < RC; ++r) {
-                    if (!TAB) {
+                    if constexpr (CPLX) {
+                        taylor_signed_add(gx, gy, bit == to_bit ? 1.0 : -1.0, raw[r].x, raw[r].y, pr[r], pi[r], dr[r], di[r]);
+                    } else if (!TAB) {
                         pr[r] += raw[r].x; pi[r] += raw[r].y;
                     } else {
                         pr[r] = fma(gx, raw[r].x, pr[r]); pr[r] = fma(-gy, raw[r].y, pr[r]);
@@ -1042,7 +1090,8 @@ stage_d2_taylor_kernel(const __grid_constant__ TaylorArgs a) {
         double qd[RC];   // the Q sums of rb_tile_gather: not used by the two instantiations below
 #pragma unroll
         for (int r = 0; r < RC; ++r) v[r] = sub[tid + r * NT];
-        rb_tile_gather<!TAB, !TAB, STB, 3>(g, sub, tab, tid, to_bit, 0, false, v, pr, pi, qd, qd);
+        if constexpr (CPLX) rb_tile_gather<false, false, STB, 3, true>(g, sub, tab, tid, to_bit, 0, false, v, pr, pi, dr, di);
+        else rb_tile_gather<!TAB, !TAB, STB, 3>(g, sub, tab, tid, to_bit, 0, false, v, pr, pi, qd, qd);
 #pragma unroll
         for (int q = 0; q < CB; ++q) {   // flips of the chunk bits
             const int p = STB + q;
@@ -1053,7 +1102,9 @@ stage_d2_taylor_kernel(const __grid_constant__ TaylorArgs a) {
 #pragma unroll
             for (int r = 0; r < RC; ++r) {
                 const c2 pv = other[tid + r * NT];
-                if (!TAB) {
+                if constexpr (CPLX) {
+                    taylor_signed_add(gx, gy, bit == to_bit ? 1.0 : -1.0, pv.x, pv.y, pr[r], pi[r], dr[r], di[r]);
+                } else if (!TAB) {
                     pr[r] += pv.x; pi[r] += pv.y;
                 } else {
                     pr[r] = fma(gx, pv.x, pr[r]); pr[r] = fma(-gy, pv.y, pr[r]);
@@ -1079,7 +1130,19 @@ stage_d2_taylor_kernel(const __grid_constant__ TaylorArgs a) {
             off[r] = acc;
         }
         // per-qubit factors (off != 0) leave the registers for 2 amplitudes' operands at a time, not 4
-        if constexpr (SHAPES) {
+        if constexpr (CPLX) {
+            double qx[RC], qy[RC];   // G' = i (P - Q)
+#pragma unroll
+            for (int r = 0; r < RC; ++r) { qx[r] = -di[r]; qy[r] = dr[r]; }
+            if constexpr (SHAPES) {
+                const double* lc = bl + c * RC;
+                const double* lt = at + tid;
+                taylor_epilogue<RC, RC / 4, SHARD, true>(
+                    a, idx, v, pr, pi, [&](int r, int J) { return lt[J * NT] + lc[(J << RB) + r]; }, voff, dsrc, qx, qy);
+            } else {
+                taylor_epilogue<RC, RC / 4, SHARD, true>(a, idx, v, pr, pi, off, voff, dsrc, qx, qy);
+            }
+        } else if constexpr (SHAPES) {
             const double* lc = bl + c * RC;
             const double* lt = at + tid;
             taylor_epilogue<RC, RC / 4, SHARD>(
@@ -1090,7 +1153,9 @@ stage_d2_taylor_kernel(const __grid_constant__ TaylorArgs a) {
     }
 }
 
-// any register size (N < 13 in particular): one thread per amplitude, partners through global loads
+// any register size (N < 13 in particular): one thread per amplitude, partners through global loads.  CPLX: the
+// complex-drive step, G' = i (P - Q) as well (stage_d2_taylor_kernel)
+template <bool CPLX = false>
 __global__ void __launch_bounds__(256) stage_d2_taylor_small_kernel(const __grid_constant__ TaylorArgs a) {
     const long long s = (long long)blockIdx.x * blockDim.x + threadIdx.x;
     if (s >= a.D) return;
@@ -1100,21 +1165,28 @@ __global__ void __launch_bounds__(256) stage_d2_taylor_small_kernel(const __grid
     const int ns = a.tab_shapes ? a.tab_shapes : 1;
     const double* tab = a.table ? a.table + traj * (a.tab_shapes ? taylor_table_stride(nb, ns) : d2_table_stride(nb)) : nullptr;
     double gxs = 0.0, gys = 0.0, offv[PB200_TAYLOR_SMAX];
+    double q2x = 0.0, q2y = 0.0;   // CPLX: G'
 #pragma unroll
     for (int q = 0; q < PB200_TAYLOR_SMAX; ++q) offv[q] = 0.0;
     if (tab) {
+        double dx = 0.0, dy = 0.0;
         for (int p = 0; p < nb; ++p) {
             const double2 raw = __ldg(reinterpret_cast<const double2*>(a.v + voff + (s ^ (1LL << p))));
             const int bit = (int)((s >> p) & 1);
             const double gx = tab[2 * p], gy = (bit == a.to_bit) ? tab[2 * p + 1] : -tab[2 * p + 1];
-            gxs = fma(gx, raw.x, gxs); gxs = fma(-gy, raw.y, gxs);
-            gys = fma(gx, raw.y, gys); gys = fma(gy, raw.x, gys);
+            if constexpr (CPLX) {
+                taylor_signed_add(gx, gy, bit == a.to_bit ? 1.0 : -1.0, raw.x, raw.y, gxs, gys, dx, dy);
+            } else {
+                gxs = fma(gx, raw.x, gxs); gxs = fma(-gy, raw.y, gxs);
+                gys = fma(gx, raw.y, gys); gys = fma(gy, raw.x, gys);
+            }
             if (bit == a.from_is_one) {
 #pragma unroll
                 for (int q = 0; q < PB200_TAYLOR_SMAX; ++q)
                     if (q < ns) offv[q] += tab[2 * nb + q * nb + p];
             }
         }
+        q2x = -dy; q2y = dx;
     } else {
         double pr = 0.0, pi = 0.0, qr = 0.0, qi = 0.0;
         for (int p = 0; p < nb; ++p) {
@@ -1124,19 +1196,24 @@ __global__ void __launch_bounds__(256) stage_d2_taylor_small_kernel(const __grid
         }
         gxs = fma(-a.unit.y, qi, a.unit.x * pr);
         gys = fma(a.unit.y, qr, a.unit.x * pi);
+        // P - Q = ux Q + i uy P in these sums (Q here is the signed sum)
+        q2x = -fma(a.unit.x, qi, a.unit.y * pr);
+        q2y = fma(a.unit.x, qr, -a.unit.y * pi);
     }
     const long long idx[1] = {s};
     const double2 own = __ldg(reinterpret_cast<const double2*>(a.v + voff + s));
     const c2 v[1] = {{own.x, own.y}};
     const double gx[1] = {gxs}, gy[1] = {gys}, offv1[1] = {offv[0]};
+    const double qx[1] = {q2x}, qy[1] = {q2y};
     auto local = [&](int, int J) {
         double acc = 0.0;
 #pragma unroll
         for (int q = 0; q < PB200_TAYLOR_SMAX; ++q) acc = fma(J == 0 ? a.m0[q] : a.hm[q][J - 1], offv[q], acc);
         return acc;
     };
-    if (a.tab_shapes) taylor_epilogue<1>(a, idx, v, gx, gy, local, voff, a.dint ? a.dint + traj * a.dint_stride : nullptr);
-    else taylor_epilogue<1>(a, idx, v, gx, gy, offv1, voff, a.dint ? a.dint + traj * a.dint_stride : nullptr);
+    const double* dsrc = a.dint ? a.dint + traj * a.dint_stride : nullptr;
+    if (a.tab_shapes) taylor_epilogue<1, 1, false, CPLX>(a, idx, v, gx, gy, local, voff, dsrc, qx, qy);
+    else taylor_epilogue<1, 1, false, CPLX>(a, idx, v, gx, gy, offv1, voff, dsrc, qx, qy);
 }
 
 // ---- generic-d stage kernel (any dim, several drives; global gathers) -------

@@ -11,6 +11,7 @@
 #include <cuda_runtime.h>
 
 #include <algorithm>
+#include <deque>
 #include <map>
 #include <memory>
 #include <mutex>
@@ -195,6 +196,8 @@ class DevBuf {
 // store of chi_{k+1} (DESIGN.md section 8).
 constexpr int kTaylorTileBits = 13;
 constexpr int kTaylorRegBits = 4;
+// complex-drive steps (stage_d2_taylor_kernel<..., CPLX = true>): the same tile, 256 threads of 32 amplitudes
+constexpr int kTaylorCplxRegBits = 5;
 // shared memory of the Taylor stage with several detuning shapes: the tile, the per-bit table, and the shapes' sums of
 // every order's coefficients per register-bit pattern and per thread (stage_d2_taylor_kernel<..., PB200_TAYLOR_SMAX>)
 static size_t taylor_shapes_smem(int n) {
@@ -240,6 +243,13 @@ static int device_setup(int dev) {
     CUDA_CHECK(cudaFuncSetAttribute(stage_d2_taylor_kernel<false, false, kTaylorTileBits, kTaylorRegBits, false, SM>, cudaFuncAttributeMaxDynamicSharedMemorySize, shapes_smem));
     CUDA_CHECK(cudaFuncSetAttribute(stage_d2_taylor_kernel<true, true, kTaylorTileBits, kTaylorRegBits, true, SM>, cudaFuncAttributeMaxDynamicSharedMemorySize, shapes_smem));
     CUDA_CHECK(cudaFuncSetAttribute(stage_d2_taylor_kernel<true, false, kTaylorTileBits, kTaylorRegBits, true, SM>, cudaFuncAttributeMaxDynamicSharedMemorySize, shapes_smem));
+    // complex-drive steps (the drive's phase moves inside the step)
+    CUDA_CHECK(cudaFuncSetAttribute(stage_d2_taylor_kernel<true, false, kTaylorTileBits, kTaylorCplxRegBits, false, 0, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, taylor_smem));
+    CUDA_CHECK(cudaFuncSetAttribute(stage_d2_taylor_kernel<true, false, kTaylorTileBits, kTaylorCplxRegBits, true, 0, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, taylor_smem));
+    CUDA_CHECK(cudaFuncSetAttribute(stage_d2_taylor_kernel<false, false, kTaylorTileBits, kTaylorCplxRegBits, false, 1, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, taylor_smem));
+    CUDA_CHECK(cudaFuncSetAttribute(stage_d2_taylor_kernel<true, false, kTaylorTileBits, kTaylorCplxRegBits, false, SM, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, shapes_smem));
+    CUDA_CHECK(cudaFuncSetAttribute(stage_d2_taylor_kernel<false, false, kTaylorTileBits, kTaylorCplxRegBits, false, SM, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, shapes_smem));
+    CUDA_CHECK(cudaFuncSetAttribute(stage_d2_taylor_kernel<true, false, kTaylorTileBits, kTaylorCplxRegBits, true, SM, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, shapes_smem));
     CUDA_CHECK(cudaFuncSetAttribute(stage_d2_fwd_kernel<true, TB, RB>, cudaFuncAttributeMaxDynamicSharedMemorySize, 2 * 2048 * 16 + 256));
     CUDA_CHECK(cudaFuncSetAttribute(stage_d2_fwd_kernel<false, TB, RB>, cudaFuncAttributeMaxDynamicSharedMemorySize, 2 * 2048 * 16 + 256));
     if (dev >= 0 && dev < PB200_MAX_DEVICES) sm_count[dev] = sms;
@@ -323,13 +333,15 @@ struct Plan {
     bool fwd_now = false;           // decided per propagate call
     PassGeom fwd_geo[3];
     DevBuf<c2> wbuf[2];
-    // time-dependent Taylor propagator: drive projected on its constant phase, half-width of H at the sampling times,
-    // extra ring buffers (beyond buf / aux) for polynomial degrees > 2
+    // time-dependent Taylor propagator: the drive relative to the phase of its largest sample, half-width of H at the
+    // sampling times, extra ring buffers (beyond buf / aux) for polynomial degrees > 2
     struct TaylorCache {
         bool valid = false, ok = false;
         const char* why = "";              // why not, once valid
-        c2 unit{1.0, 0.0};
-        PiecewiseCubic<double> om;         // omega(t): the drive along its constant phase (reference row)
+        c2 unit{1.0, 0.0};                 // phase of the reference row's largest sample
+        PiecewiseCubic<double> om;         // Re omega(t), omega = reference row x conj(unit)
+        PiecewiseCubic<double> om_im;      // Im omega(t) (phase_moves only)
+        bool phase_moves = false;          // omega is not real: the steps are classified (TaylorStep::drive)
         std::vector<double> w_knot;        // spectral half-width of H at the sampling times
         // separable per-(trajectory, qubit) drives: coef = a unit omega(t), det = theta(t) + sum_s c_s M_s(t)
         bool uniform = true;               // one state, one coefficient for every qubit (a = 1, c = 0)
@@ -343,8 +355,9 @@ struct Plan {
         // 0: [B][3N+2] device table of one shape (d2_table_stride); PB200_TAYLOR_SMAX: [B][taylor_table_stride(N, SMAX)]
         // (several shapes, or shapes on a uniform drive)
         int tab_shapes = 0;
-        std::vector<double> tab_host;      // device table image
+        std::vector<double> tab_host;      // device table image with `unit`
         DevBuf<double> d_tab;
+        c2 tab_unit{1.0, 0.0};             // the unit d_tab holds now (steps of one rotated phase upload their own)
     } tay;
     std::vector<DevBuf<c2>> tay_ws;
     // state-vector shard (pb200_plan_create_shard): the top shard_bits qubits of the global index equal `shard`; n is
@@ -1518,8 +1531,8 @@ static void propagate(Plan& P, double t_start, double t_stop, const pb200_run_op
         fail(PB200_ERR_INVALID, "pb200_propagate: [%g, %g] outside sampling times [%g, %g]", t_start, t_stop, tlo, thi);
     t_start = std::max(t_start, tlo); t_stop = std::min(t_stop, thi);
     if (P.has_collapse) { propagate_mcwf(P, t_start, t_stop, o, stats); return; }
-    {   // integrator 3 / auto: the time-dependent Taylor propagator wherever it applies (global drive of constant
-        // phase, d = 2, one state) unless the caller steers the Magnus controller explicitly
+    {   // integrator 3 / auto: the time-dependent Taylor propagator wherever it applies (global drive of any phase,
+        // d = 2, one state) unless the caller steers the Magnus controller explicitly
         const int req = o ? o->integrator : 0;
         if (req < 0 || req > 3) fail(PB200_ERR_INVALID, "integrator must be 0 (auto), 1, 2 or 3");
         bool want = req == 3;
@@ -1538,7 +1551,7 @@ static void propagate(Plan& P, double t_start, double t_stop, const pb200_run_op
             if (ok) { propagate_taylor(P, t_start, t_stop, o, stats); return; }
             if (env_int("PB200_TAYLOR_LOG", 0)) fprintf(stderr, "taylor not taken: %s\n", g_taylor_why);
             if (req == 3)
-                fail(PB200_ERR_UNSUPPORTED, "integrator 3 (Taylor) needs a d = 2 register whose drive is one time shape of constant phase "
+                fail(PB200_ERR_UNSUPPORTED, "integrator 3 (Taylor) needs a d = 2 register whose drive rows are multiples of one row "
                                             "(per-qubit static factors / detuning offsets allowed), no collapse operators / SLM mask: %s",
                      g_taylor_why);
         }
@@ -1838,7 +1851,7 @@ static void propagate(Plan& P, double t_start, double t_stop, const pb200_run_op
     if (stats) *stats = st;
 }
 
-// ---- time-dependent Taylor propagator (one drive time shape of constant phase, d = 2) -----------------------------
+// ---- time-dependent Taylor propagator (one drive time shape, its phase constant or moving, d = 2) -----------------
 // Replaces the whole Magnus / exponential machinery above where it applies (C2, C5; C4 batches through per-qubit static
 // factors, taylor_separable): the interpolated coefficients
 // are polynomials in u = (t-a)/h on a step, the solution is the Taylor series in u (kernels.cuh,
@@ -1974,7 +1987,26 @@ static SeparableFit taylor_separable(int B, int N, int nt, CS cs, DS ds, int max
     return F;
 }
 
-// real part of the drive along its constant phase, per-(trajectory, qubit) static factors, device table
+// per-trajectory device table image (a unit per BIT position, c per (shape,) bit position) with drive unit `unit`
+static std::vector<double> taylor_table(const Plan& P, cplx unit) {
+    const Plan::TaylorCache& C = P.tay;
+    const int N = P.n, B = P.B;
+    const int stride = C.tab_shapes ? taylor_table_stride(N, C.tab_shapes) : d2_table_stride(N);
+    std::vector<double> tab((size_t)B * stride, 0.0);
+    for (int b = 0; b < B; ++b) {
+        double* t = tab.data() + (size_t)b * stride;
+        for (int k = 0; k < N; ++k) {
+            const int p = N - 1 - k;
+            const cplx g = C.a[(size_t)b * N + k] * unit;
+            t[2 * p] = g.real(); t[2 * p + 1] = g.imag();
+            for (int s = 0; s < C.ns; ++s) t[2 * N + s * N + p] = C.c[((size_t)b * N + k) * C.ns + s];
+        }
+    }
+    return tab;
+}
+
+// the drive relative to the phase of its largest sample (real and imaginary parts), per-(trajectory, qubit) static
+// factors, device table
 static bool taylor_prepare(Plan& P) {
     Plan::TaylorCache& C = P.tay;
     g_taylor_why = "structure (d, drives, collapse / dissipator / mask, interpolation order)";
@@ -2006,15 +2038,20 @@ static bool taylor_prepare(Plan& P) {
     const int np = ref.pieces();
     C.om = PiecewiseCubic<double>();
     C.om.c0.resize(np); C.om.c1.resize(np); C.om.c2.resize(np); C.om.c3.resize(np);
+    C.om_im = C.om;
+    C.phase_moves = false;
     for (int i = 0; i < np; ++i) {
         const double hi = P.times[i + 1] - P.times[i];
         const cplx v0 = ref.c0[i] * cu, v1 = ref.c1[i] * cu, v2 = ref.c2[i] * cu, v3 = ref.c3[i] * cu;
         const double im = std::max(std::max(std::fabs(v0.imag()), std::fabs(v1.imag()) * hi),
                                    std::max(std::fabs(v2.imag()) * hi * hi, std::fabs(v3.imag()) * hi * hi * hi));
-        if (im > 1e-13 * scale) { g_taylor_why = C.why = "the drive phase moves in time"; return false; }
+        if (im > 1e-13 * scale) C.phase_moves = true;
         C.om.c0[i] = v0.real(); C.om.c1[i] = v1.real(); C.om.c2[i] = v2.real(); C.om.c3[i] = v3.real();
+        C.om_im.c0[i] = v0.imag(); C.om_im.c1[i] = v1.imag(); C.om_im.c2[i] = v2.imag(); C.om_im.c3[i] = v3.imag();
     }
     C.om.y_last = (ref.y_last * cu).real();
+    C.om_im.y_last = (ref.y_last * cu).imag();
+    if (!C.phase_moves) C.om_im = PiecewiseCubic<double>();   // constant phase: the real drive of before, exactly
     C.unit = {unit.real(), unit.imag()};
     C.a = F.a; C.c = F.c; C.ns = F.ns;
     for (int s = 0; s < C.ns; ++s) C.shape[s] = make_interpolant<double>(P.times.data(), F.m[s].data(), nt, P.desc.interp_order);
@@ -2035,24 +2072,27 @@ static bool taylor_prepare(Plan& P) {
     // a uniform drive keeps its gather with local detuning (stage_d2_taylor_kernel<true, ..., PB200_TAYLOR_SMAX>)
     C.tab_shapes = (C.ns > 1 || (C.drive_uniform && C.ns == 1)) ? PB200_TAYLOR_SMAX : 0;
     if (!C.uniform) {   // static device table: a unit per BIT position (re, im), c per (shape,) bit position
-        const int stride = C.tab_shapes ? taylor_table_stride(N, C.tab_shapes) : d2_table_stride(N);
-        C.tab_host.assign((size_t)B * stride, 0.0);
-        for (int b = 0; b < B; ++b) {
-            double* t = C.tab_host.data() + (size_t)b * stride;
-            for (int k = 0; k < N; ++k) {
-                const int p = N - 1 - k;
-                const cplx g = C.a[(size_t)b * N + k] * unit;
-                t[2 * p] = g.real(); t[2 * p + 1] = g.imag();
-                for (int s = 0; s < C.ns; ++s) t[2 * N + s * N + p] = C.c[((size_t)b * N + k) * C.ns + s];
-            }
-        }
+        C.tab_host = taylor_table(P, unit);
         C.d_tab.reset(P, C.tab_host.size());
         CUDA_CHECK(cudaMemcpyAsync(C.d_tab.get(), C.tab_host.data(), C.tab_host.size() * sizeof(double), cudaMemcpyHostToDevice,
                                    P.stream));
+        C.tab_unit = C.unit;
     }
     C.w_knot.clear();
     C.ok = true;
     return true;
+}
+
+// Before a step whose drive unit differs from the one the device table holds (a step of one phase other than the
+// reference's, TaylorStep::drive == 1): upload the table with that unit.  The host image goes into `keep`, which the
+// caller holds until its stream has run the copy.
+static void taylor_table_unit(Plan& P, c2 unit, std::deque<std::vector<double>>& keep) {
+    Plan::TaylorCache& C = P.tay;
+    if (C.uniform || (unit.x == C.tab_unit.x && unit.y == C.tab_unit.y)) return;
+    keep.push_back(taylor_table(P, cplx(unit.x, unit.y)));
+    CUDA_CHECK(cudaMemcpyAsync(C.d_tab.get(), keep.back().data(), keep.back().size() * sizeof(double), cudaMemcpyHostToDevice,
+                               P.stream));
+    C.tab_unit = unit;
 }
 
 // centre and half-width of  Dint - th n_from - sum_s mv_s sum_k c_{k,s} n_k + om X  over the batch: the rigorous bounds
@@ -2116,7 +2156,10 @@ static void taylor_knot_widths(Plan& P) {
     for (int i = 0; i < nt; ++i) {
         double c, hw, mv[PB200_TAYLOR_SMAX] = {};
         for (int s = 0; s < C.ns; ++s) mv[s] = eval_at(C.shape[s], P.times, P.times[i], order);
-        taylor_bounds(P, eval_at(C.om, P.times, P.times[i], order), eval_at(th_pc, P.times, P.times[i], order), mv, c, hw);
+        // the spectrum of omega X does not depend on the phase of omega: |omega| bounds it
+        double om = eval_at(C.om, P.times, P.times[i], order);
+        if (C.phase_moves) om = std::hypot(om, eval_at(C.om_im, P.times, P.times[i], order));
+        taylor_bounds(P, om, eval_at(th_pc, P.times, P.times[i], order), mv, c, hw);
         C.w_knot[i] = hw;
     }
 }
@@ -2133,6 +2176,7 @@ static bool taylor_worthwhile(Plan& P, double gtol) {
     const double rate = gtol / std::max(P.times.back() - P.times.front(), 1e-30);
     const double allow = 0.25 * rate / P.n;
     std::vector<const PiecewiseCubic<double>*> pcs = {&P.tay.om, &P.tabs[0][0].det[0]};
+    if (P.tay.phase_moves) pcs.push_back(&P.tay.om_im);   // a phase jump under amplitude is a kink of both parts
     for (int s = 0; s < P.tay.ns; ++s) pcs.push_back(&P.tay.shape[s]);
     std::vector<char> rough(nt, 0);
     for (const PiecewiseCubic<double>* pc : pcs) {
@@ -2235,17 +2279,23 @@ static int taylor_order(double h, const std::vector<double>& mj, double tol, dou
     return std::max(kk, 1);
 }
 
-static void launch_taylor_stage(Plan& P, const PassGeom* geo, const TaylorArgs& a, long long& launches) {
+// cplx: a step whose drive phase moves inside it (the CPLX instantiations)
+static void launch_taylor_stage(Plan& P, const PassGeom* geo, const TaylorArgs& a, bool cplx, long long& launches) {
     const bool uniform = a.table == nullptr;
     if (geo) {
-        constexpr int TB = kTaylorTileBits, RB = kTaylorRegBits, SM = PB200_TAYLOR_SMAX;
-        const bool real_g = a.unit.y == 0.0;
+        constexpr int TB = kTaylorTileBits, RB = kTaylorRegBits, RBC = kTaylorCplxRegBits, SM = PB200_TAYLOR_SMAX;
+        const bool real_g = a.unit.y == 0.0 && !cplx;
         const bool local = a.tab_shapes && P.tay.drive_uniform;   // uniform drive, detuning shapes: one state
-        dim3 grid((unsigned)(P.D >> TB), (unsigned)(uniform || local ? 1 : P.B)), block(1 << (TB - RB));
+        dim3 grid((unsigned)(P.D >> TB), (unsigned)(uniform || local ? 1 : P.B)), block(1 << (TB - (cplx ? RBC : RB)));
         // the kernel keeps a per-bit table behind the tile unless the drive is uniform and real
         const size_t smem = a.tab_shapes ? taylor_shapes_smem(P.n)
                                          : ((size_t)16 << TB) + (uniform && real_g ? 0 : (size_t)d2_table_stride(P.n) * 8);
-        if (local && real_g) launch_k(stage_d2_taylor_kernel<true, true, TB, RB, false, SM>, grid, block, smem, P.stream, true, a);
+        if (cplx) {
+            if (local) launch_k(stage_d2_taylor_kernel<true, false, TB, RBC, false, SM, true>, grid, block, smem, P.stream, true, a);
+            else if (a.tab_shapes) launch_k(stage_d2_taylor_kernel<false, false, TB, RBC, false, SM, true>, grid, block, smem, P.stream, true, a);
+            else if (!uniform) launch_k(stage_d2_taylor_kernel<false, false, TB, RBC, false, 1, true>, grid, block, smem, P.stream, true, a);
+            else launch_k(stage_d2_taylor_kernel<true, false, TB, RBC, false, 0, true>, grid, block, smem, P.stream, true, a);
+        } else if (local && real_g) launch_k(stage_d2_taylor_kernel<true, true, TB, RB, false, SM>, grid, block, smem, P.stream, true, a);
         else if (local) launch_k(stage_d2_taylor_kernel<true, false, TB, RB, false, SM>, grid, block, smem, P.stream, true, a);
         else if (a.tab_shapes) launch_k(stage_d2_taylor_kernel<false, false, TB, RB, false, SM>, grid, block, smem, P.stream, true, a);
         else if (!uniform) launch_k(stage_d2_taylor_kernel<false, false, TB, RB>, grid, block, smem, P.stream, true, a);
@@ -2253,7 +2303,8 @@ static void launch_taylor_stage(Plan& P, const PassGeom* geo, const TaylorArgs& 
         else launch_k(stage_d2_taylor_kernel<true, false, TB, RB>, grid, block, smem, P.stream, true, a);
     } else {
         dim3 grid((unsigned)((P.D + 255) / 256), (unsigned)P.B);
-        stage_d2_taylor_small_kernel<<<grid, 256, 0, P.stream>>>(a);
+        if (cplx) stage_d2_taylor_small_kernel<true><<<grid, 256, 0, P.stream>>>(a);
+        else stage_d2_taylor_small_kernel<false><<<grid, 256, 0, P.stream>>>(a);
     }
     ++launches;
 }
@@ -2276,8 +2327,13 @@ struct TaylorStep {
     std::vector<double> gam;         // centres of H_j
     int K = 0;
     double phi = 0.0;                // phase of the scalar centre over the step
-    int n_chi = 0, n_g = 0;          // chi ring (slot 0 = the current state), G ring
-    int ring() const { return (n_chi - 1) + n_g + 1; }   // state-sized buffers beyond the state itself
+    int n_chi = 0, n_g = 0;          // chi ring (slot 0 = the current state), G ring (and G' ring of a complex step)
+    // drive of the step: 0 real along the plan's unit; 1 real along its own unit (one phase over the step, the existing
+    // kernels); 2 complex, omega = om + i omi along the plan's unit (the CPLX kernels, two gathers per order)
+    int drive = 0;
+    c2 unit{1.0, 0.0};
+    std::vector<double> omi;
+    int ring() const { return (n_chi - 1) + n_g * (drive == 2 ? 2 : 1) + 1; }   // state-sized buffers beyond the state
 };
 
 // Host half of propagate_taylor: the steps of one call [t_start, t_stop], one at a time (next()), with the statistics
@@ -2290,7 +2346,7 @@ struct TaylorScheduler {
     int order, N, nt, ns;
     bool log_steps;
     pb200_run_stats st{};
-    struct Fit { TaylorPoly om, th, m[PB200_TAYLOR_SMAX]; bool ok; };
+    struct Fit { TaylorPoly om, omi, th, m[PB200_TAYLOR_SMAX]; double om_allow = 0.0; bool ok; };
 
     TaylorScheduler(Plan& P_, double t_start, double t_stop_, const pb200_run_opts* o) : P(P_), t_stop(t_stop_), t(t_start) {
         const double tlo = P.times.front(), thi = P.times.back();
@@ -2348,7 +2404,11 @@ struct TaylorScheduler {
             if (single_piece) out = taylor_fit(pc, P.times, order, a, h, PB200_TAYLOR_PMAX);
             return true;
         };
-        F.ok = one(C.om, F.om, third / A_sum) && one(P.tabs[0][0].det[0], F.th, third / N);
+        // a moving phase: each part of omega gets half the drive's third (|d omega| <= r_re + r_im)
+        F.om_allow = third / A_sum;
+        if (C.phase_moves) F.ok = one(C.om, F.om, 0.5 * F.om_allow) && one(C.om_im, F.omi, 0.5 * F.om_allow);
+        else F.ok = one(C.om, F.om, F.om_allow);
+        F.ok = F.ok && one(P.tabs[0][0].det[0], F.th, third / N);
         for (int s = 0; s < ns && F.ok; ++s) F.ok = one(C.shape[s], F.m[s], third / ns / C_sum[s]);
         for (int s = ns; s < PB200_TAYLOR_SMAX; ++s) { F.m[s].c.assign(1, 0.0); F.m[s].resid = 0.0; }
         return F;
@@ -2402,6 +2462,45 @@ struct TaylorScheduler {
                 }
             }
             double h = b - t;
+            // drive of the step where the plan's phase moves: one phase over the step (the imaginary part after the
+            // rotation onto the phase of the largest of omega(0), omega(1/2), omega(1) fits in the drive's allowance,
+            // booked as fit residual) runs the real kernels with the step's own unit; otherwise the complex kernels
+            int drive = 0;
+            c2 sunit = C.unit;
+            double om_resid = F.om.resid;
+            if (C.phase_moves) {
+                auto coef = [](const std::vector<double>& c, size_t j) { return j < c.size() ? c[j] : 0.0; };
+                auto poly = [](const std::vector<double>& c, double u) {
+                    double v = 0.0;
+                    for (int i = (int)c.size() - 1; i >= 0; --i) v = v * u + c[i];
+                    return v;
+                };
+                double best = 0.0, cph = 1.0, sph = 0.0;
+                for (double u : {0.0, 0.5, 1.0}) {
+                    const double x = poly(F.om.c, u), y = poly(F.omi.c, u), r = std::hypot(x, y);
+                    if (r > best) { best = r; cph = x / r; sph = y / r; }
+                }
+                const size_t nc = std::max(F.om.c.size(), F.omi.c.size());
+                std::vector<double> xr(nc), yr(nc);   // omega e^{-i phase}
+                double ybound = 0.0;
+                for (size_t j = 0; j < nc; ++j) {
+                    xr[j] = cph * coef(F.om.c, j) + sph * coef(F.omi.c, j);
+                    yr[j] = cph * coef(F.omi.c, j) - sph * coef(F.om.c, j);
+                    ybound += std::fabs(yr[j]);
+                }
+                const double r2 = F.om.resid + F.omi.resid;   // |omega - fit| <= |r_re + i r_im|
+                if (r2 + ybound <= F.om_allow) {
+                    F.om.c = xr;
+                    om_resid = r2 + ybound;
+                    if (cph != 1.0 || sph != 0.0) {
+                        drive = 1;
+                        sunit = {C.unit.x * cph - C.unit.y * sph, C.unit.x * sph + C.unit.y * cph};
+                    }
+                } else {
+                    drive = 2;
+                    om_resid = r2;
+                }
+            }
             // strip trailing zero coefficients
             auto trim = [](std::vector<double>& c, double scale) {
                 while (c.size() > 1 && std::fabs(c.back()) <= 1e-15 * scale) c.pop_back();
@@ -2410,8 +2509,10 @@ struct TaylorScheduler {
             {
                 double so = 0.0, sh = 0.0;
                 for (double v : F.om.c) so = std::max(so, std::fabs(v));
+                if (drive == 2) for (double v : F.omi.c) so = std::max(so, std::fabs(v));
                 for (double v : F.th.c) sh = std::max(sh, std::fabs(v));
                 trim(F.om.c, std::max(so, 1e-300)); trim(F.th.c, std::max(sh, 1e-300));
+                if (drive == 2) trim(F.omi.c, std::max(so, 1e-300));
                 for (int q = 0; q < PB200_TAYLOR_SMAX; ++q) {
                     double sm = 0.0;
                     for (double v : F.m[q].c) sm = std::max(sm, std::fabs(v));
@@ -2419,20 +2520,26 @@ struct TaylorScheduler {
                     p_m = std::max(p_m, (int)F.m[q].c.size() - 1);
                 }
             }
-            const int p_om = (int)F.om.c.size() - 1;
+            const int p_om = std::max((int)F.om.c.size(), drive == 2 ? (int)F.omi.c.size() : 0) - 1;
             const int p_th = std::max((int)F.th.c.size() - 1, p_m);   // degree of the diagonal (own-element) history
             const int p = std::max(p_om, p_th);
             auto th_c = [&](int j) { return j < (int)F.th.c.size() ? F.th.c[j] : 0.0; };
             auto m_c = [&](int q, int j) { return j < (int)F.m[q].c.size() ? F.m[q].c[j] : 0.0; };
+            // |omega_j|: the spectrum of omega_j X does not depend on the phase of omega_j
+            auto om_abs = [&](int j) {
+                const double x = j < (int)F.om.c.size() ? F.om.c[j] : 0.0;
+                if (drive != 2) return std::fabs(x);
+                return std::hypot(x, j < (int)F.omi.c.size() ? F.omi.c[j] : 0.0);
+            };
             // centres and norm bounds of H_j
             std::vector<double> gam(p + 1, 0.0), mj(p + 1, 0.0);
             {
                 double c0, hw0, mv[PB200_TAYLOR_SMAX];
                 for (int q = 0; q < PB200_TAYLOR_SMAX; ++q) mv[q] = m_c(q, 0);
-                taylor_bounds(P, F.om.c[0], F.th.c[0], mv, c0, hw0);
+                taylor_bounds(P, drive == 2 ? om_abs(0) : F.om.c[0], F.th.c[0], mv, c0, hw0);
                 gam[0] = c0; mj[0] = hw0;
                 for (int j = 1; j <= p; ++j) {
-                    const double thj = th_c(j), omj = j <= p_om ? F.om.c[j] : 0.0;
+                    const double thj = th_c(j), omj = j <= p_om ? om_abs(j) : 0.0;
                     gam[j] = -thj * 0.5 * N;
                     double mm = 0.0;
                     for (int q = 0; q < ns; ++q) mm += std::fabs(m_c(q, j)) * C_sum[q];
@@ -2458,20 +2565,23 @@ struct TaylorScheduler {
             s.gam = gam; s.K = K;
             s.n_chi = p_th + 2;
             s.n_g = p_om >= 1 ? p_om + 1 : 0;
+            s.drive = drive; s.unit = sunit;
+            s.omi = drive == 2 ? F.omi.c : std::vector<double>();
             // phase of the scalar centre: exp(-i h int_0^1 sum_j gam_j u^j du)
             double phi = 0.0;
             for (int j = 0; j <= p; ++j) phi += gam[j] / (j + 1);
             s.phi = phi * h;
             st.n_applies += K; st.n_exponentials += 1; ++st.n_steps;
             if (log_steps)
-                fprintf(stderr, "taylor step t=%.6f h_ns=%.3f p_om=%d p_th=%d p_m=%d K=%d ring=%d rho=%.3f resid=%.2e/%.2e/%.2e\n", t,
-                        h * 1e3, p_om, p_th, p_m, K, s.ring() + 1, mj[0] * h, F.om.resid, F.th.resid, F.m[0].resid);
+                fprintf(stderr, "taylor step t=%.6f h_ns=%.3f p_om=%d p_th=%d p_m=%d K=%d ring=%d rho=%.3f resid=%.2e/%.2e/%.2e drive=%s\n",
+                        t, h * 1e3, p_om, p_th, p_m, K, s.ring() + 1, mj[0] * h, om_resid, F.th.resid, F.m[0].resid,
+                        drive == 2 ? "cplx" : drive == 1 ? "rot" : "real");
             double rho_eff = 0.0;
             for (int j = 0; j <= p; ++j) rho_eff += mj[j] / (j + 1);
             st.max_rho = std::max(st.max_rho, rho_eff * h);
             double fit_m = 0.0;
             for (int q = 0; q < ns; ++q) fit_m += C_sum[q] * F.m[q].resid;
-            const double fit_err = h * (A_sum * F.om.resid + N * F.th.resid + fit_m);
+            const double fit_err = h * (A_sum * om_resid + N * F.th.resid + fit_m);
             st.err_estimate += trunc_bound + fit_err;
             fit_spent += fit_err;
             { const double r = kRoundUnit * std::exp(std::min(rho_eff * h, 40.0)); round2 += r * r; }
@@ -2498,7 +2608,7 @@ struct TaylorScheduler {
 // Ring of one step: chi[0] = the current state, the other slots from the buffers that are not the state (the Magnus
 // aux buffers too when the plan has them), then the plan's own Taylor work buffers, allocated on first need.
 struct TaylorRing {
-    std::vector<c2*> chi, gr;
+    std::vector<c2*> chi, gr, gr2;   // gr2: G' of a complex step
     DevBuf<c2>* acc_slot = nullptr;
 };
 
@@ -2517,11 +2627,12 @@ static TaylorRing taylor_ring(Plan& P, const TaylorStep& s) {
     taylor_grow_ring(P, s.ring());
     for (size_t i = 0; i < P.tay_ws.size(); ++i) free_slots.push_back(&P.tay_ws[i]);
     TaylorRing R;
-    R.chi.resize(s.n_chi); R.gr.resize(s.n_g);
+    R.chi.resize(s.n_chi); R.gr.resize(s.n_g); R.gr2.resize(s.drive == 2 ? s.n_g : 0);
     int fs = 0;
     R.chi[0] = P.buf[P.cur].get();
     for (int i = 1; i < s.n_chi; ++i) R.chi[i] = free_slots[fs++]->get();
     for (int i = 0; i < s.n_g; ++i) R.gr[i] = free_slots[fs++]->get();
+    for (size_t i = 0; i < R.gr2.size(); ++i) R.gr2[i] = free_slots[fs++]->get();
     R.acc_slot = free_slots[fs++];
     return R;
 }
@@ -2539,7 +2650,7 @@ static TaylorArgs taylor_args(const Plan& P, const PassGeom& geo, const TaylorSt
     a.dint_stride = P.dint_shared ? 0 : P.D;
     a.D = P.D;
     a.geo = geo;
-    a.unit = C.unit;
+    a.unit = s.unit;
     a.table = C.uniform ? nullptr : C.d_tab.get();
     a.tab_shapes = C.tab_shapes;
     a.to_bit = P.desc.drives[0].state_to; a.from_is_one = P.desc.drives[0].state_from;
@@ -2548,12 +2659,21 @@ static TaylorArgs taylor_args(const Plan& P, const PassGeom& geo, const TaylorSt
     a.scale = {0.0, -s.h / (k + 1)};
     a.nh = std::min(s.p, k);
     for (int j = 1; j <= a.nh; ++j) {
-        const double thj = th_c(j), omj = j <= s.p_om ? s.om[j] : 0.0;
+        const double thj = th_c(j), omj = j < (int)s.om.size() ? s.om[j] : 0.0;
         bool any_m = false;
         for (int q = 0; q < PB200_TAYLOR_SMAX; ++q) { a.hm[q][j - 1] = m_c(q, j); any_m = any_m || a.hm[q][j - 1] != 0.0; }
         a.hth[j - 1] = thj; a.hgam[j - 1] = s.gam[j]; a.hom[j - 1] = omj;
         a.hchi[j - 1] = (thj != 0.0 || any_m || s.gam[j] != 0.0) ? R.chi[(k - j) % s.n_chi] : nullptr;
         a.hg[j - 1] = (omj != 0.0) ? R.gr[(k - j) % s.n_g] : nullptr;
+        if (s.drive == 2) {
+            const double omij = j < (int)s.omi.size() ? s.omi[j] : 0.0;
+            a.homi[j - 1] = omij;
+            a.hg2[j - 1] = (omij != 0.0) ? R.gr2[(k - j) % s.n_g] : nullptr;
+        }
+    }
+    if (s.drive == 2) {
+        a.om0i = s.omi[0];
+        a.g2_out = (s.n_g && k + 1 < s.K) ? R.gr2[k % s.n_g] : nullptr;
     }
     const bool last = (k + 1 == s.K);
     if ((k & 1) == 0) { a.acc_on = 1; a.acc_add_v = 1; a.acc_read = k > 0; }
@@ -2572,9 +2692,12 @@ static void propagate_taylor(Plan& P, double t_start, double t_stop, const pb200
     TaylorScheduler S(P, t_start, t_stop, o);
     TaylorStep s;
     long long launches = 0;
+    std::deque<std::vector<double>> tables;   // tables of rotated steps, until the call's last synchronisation
     while (S.next(s)) {
         const TaylorRing R = taylor_ring(P, s);
-        for (int k = 0; k < s.K; ++k) launch_taylor_stage(P, use_rb ? &passes[0] : nullptr, taylor_args(P, passes[0], s, R, k), launches);
+        taylor_table_unit(P, s.drive == 1 ? s.unit : P.tay.unit, tables);
+        for (int k = 0; k < s.K; ++k)
+            launch_taylor_stage(P, use_rb ? &passes[0] : nullptr, taylor_args(P, passes[0], s, R, k), s.drive == 2, launches);
         CUDA_CHECK(cudaGetLastError());
         // the accumulator becomes the current state buffer
         std::swap(P.buf[P.cur], *R.acc_slot);
@@ -2683,19 +2806,22 @@ static PassGeom shard_geometry(const Plan& P) {
     return g;
 }
 
-// one order on one shard; no programmatic dependent launch: an order waits for its peers through events
-static void launch_taylor_shard(Plan& P, const TaylorArgs& a) {
-    constexpr int TB = kTaylorTileBits, RB = kTaylorRegBits, SM = PB200_TAYLOR_SMAX;
-    const bool real_g = a.unit.y == 0.0;
-    dim3 grid((unsigned)(P.D >> TB)), block(1 << (TB - RB));
+// one order on one shard; no programmatic dependent launch: an order waits for its peers through events.  cplx: a step
+// whose drive phase moves inside it
+static void launch_taylor_shard(Plan& P, const TaylorArgs& a, bool cplx) {
+    constexpr int TB = kTaylorTileBits, RB = kTaylorRegBits, RBC = kTaylorCplxRegBits, SM = PB200_TAYLOR_SMAX;
+    const bool real_g = a.unit.y == 0.0 && !cplx;
+    dim3 grid((unsigned)(P.D >> TB)), block(1 << (TB - (cplx ? RBC : RB)));
     if (a.table) {   // detuning shapes (the drive of a shard is uniform: pb200_shards_link)
         const size_t smem = taylor_shapes_smem(P.n);
-        if (real_g) launch_k(stage_d2_taylor_kernel<true, true, TB, RB, true, SM>, grid, block, smem, P.stream, false, a);
+        if (cplx) launch_k(stage_d2_taylor_kernel<true, false, TB, RBC, true, SM, true>, grid, block, smem, P.stream, false, a);
+        else if (real_g) launch_k(stage_d2_taylor_kernel<true, true, TB, RB, true, SM>, grid, block, smem, P.stream, false, a);
         else launch_k(stage_d2_taylor_kernel<true, false, TB, RB, true, SM>, grid, block, smem, P.stream, false, a);
         return;
     }
     const size_t smem = ((size_t)16 << TB) + (real_g ? 0 : (size_t)d2_table_stride(P.n) * 8);
-    if (real_g) launch_k(stage_d2_taylor_kernel<true, true, TB, RB, true>, grid, block, smem, P.stream, false, a);
+    if (cplx) launch_k(stage_d2_taylor_kernel<true, false, TB, RBC, true, 0, true>, grid, block, smem, P.stream, false, a);
+    else if (real_g) launch_k(stage_d2_taylor_kernel<true, true, TB, RB, true>, grid, block, smem, P.stream, false, a);
     else launch_k(stage_d2_taylor_kernel<true, false, TB, RB, true>, grid, block, smem, P.stream, false, a);
 }
 
@@ -2741,11 +2867,16 @@ static void shards_apply_h(const std::vector<Plan*>& G, double t, const std::vec
     const PassGeom geo = shard_geometry(P0);
     const int order = P0.desc.interp_order;
     const double om = eval_at(P0.tay.om, P0.times, t, order), th = eval_at(P0.tabs[0][0].det[0], P0.times, t, order);
+    const bool cplx = P0.tay.phase_moves;
     shards_sync(G);
     const int count = (int)G.size();
+    std::deque<std::vector<double>> tables;
     for (int r = 0; r < count; ++r) {
         Plan& P = *G[r];
+        CUDA_CHECK(cudaSetDevice(P.desc.device));
+        taylor_table_unit(P, P.tay.unit, tables);
         TaylorArgs a{};
+        if (cplx) a.om0i = eval_at(P0.tay.om_im, P0.times, t, order);
         a.v = in[r]; a.out = out[r];
         a.dint = P.has_interaction ? P.dint.get() : nullptr;
         a.D = P.D; a.geo = geo; a.unit = P.tay.unit;
@@ -2758,8 +2889,7 @@ static void shards_apply_h(const std::vector<Plan*>& G, double t, const std::vec
         a.acc_mul = {1.0, 0.0};
         a.shard_bits = P.shard_bits; a.shard = r;
         for (int q = 0; q < P.shard_bits; ++q) a.peer[q] = in[r ^ (1 << q)];
-        CUDA_CHECK(cudaSetDevice(P.desc.device));
-        launch_taylor_shard(P, a);
+        launch_taylor_shard(P, a, cplx);
     }
     CUDA_CHECK(cudaGetLastError());
     shards_sync(G);
@@ -3693,8 +3823,13 @@ int pb200_shards_propagate(pb200_plan** plans, int32_t count, double t_start, do
     long long launches = 0;
     bool first = true;
     std::vector<TaylorRing> R(count);
+    std::deque<std::vector<double>> tables;   // tables of rotated steps, until the call's last synchronisation
     for (const TaylorStep& s : steps) {
-        for (int r = 0; r < count; ++r) R[r] = taylor_ring(*G[r], s);
+        for (int r = 0; r < count; ++r) {
+            R[r] = taylor_ring(*G[r], s);
+            CUDA_CHECK(cudaSetDevice(G[r]->desc.device));
+            taylor_table_unit(*G[r], s.drive == 1 ? s.unit : G[r]->tay.unit, tables);
+        }
         for (int k = 0; k < s.K; ++k) {
             for (int r = 0; r < count; ++r) {
                 Plan& P = *G[r];
@@ -3706,7 +3841,7 @@ int pb200_shards_propagate(pb200_plan** plans, int32_t count, double t_start, do
                     a.peer[q] = R[peer].chi[k % s.n_chi];
                     if (!first) CUDA_CHECK(cudaStreamWaitEvent(P.stream, order_ev.ev[peer], 0));
                 }
-                launch_taylor_shard(P, a);
+                launch_taylor_shard(P, a, s.drive == 2);
                 ++launches;
             }
             for (int r = 0; r < count; ++r) {

@@ -7,8 +7,9 @@ an ordinary plan on ``devices[i]`` (several shards may share a device), and one 
 them all: ``pb200_shards_propagate`` runs every order of the time-dependent Taylor series on every
 shard, whose partners across the shard bits are read from the peers' slices.
 
-Scope: what the Taylor propagator takes with one state -- d = 2, one global drive amplitude of
-constant phase, per-qubit detuning of up to 4 time shapes (detuning maps), Ising interaction.  The methods mirror the single-state methods of ``DevicePlan`` that
+Scope: what the Taylor propagator takes with one state -- d = 2, one global drive (its phase may
+change in time: phase shifts, phase jumps between pulses, EOM drift correction), per-qubit detuning
+of up to 4 time shapes (detuning maps), Ising interaction.  The methods mirror the single-state methods of ``DevicePlan`` that
 ``B200Backend._stream``, ``DeviceStateView`` and ``DeviceHamiltonian`` call, with the same shapes
 (a leading trajectory axis of 1).
 """
@@ -102,7 +103,8 @@ class ShardedPlan:
                 f"{self.G} shards of a {self.n}-qubit state hold 2^{self.L} amplitudes each; a shard holds "
                 f"2^{MIN_LOCAL_BITS} to 2^{MAX_LOCAL_BITS}"
             )
-        # per-qubit detuning (detuning maps) is the library's to accept or refuse; drive amplitudes must be global
+        # per-qubit detuning (detuning maps) is the library's to accept or refuse; the drive rows must be identical
+        # (one global drive, whatever its phase does in time)
         coef = np.asarray(spec.drives[0].coef) if len(spec.drives) == 1 else None
         if spec.interaction_type == "XY" or coef is None or not (coef == coef[:1]).all():
             raise NotImplementedError(
