@@ -213,6 +213,50 @@ constexpr int kMaxExtraBits = 16;
 // a state-vector shard holds 2^L amplitudes, 13 <= L <= 29: at least one tile, and the local bits above the tile
 // (at most 16) stay partner loads of the single-pass geometry
 constexpr int kShardMaxLocalBits = 29;
+static_assert(kShardMaxLocalBits - kTaylorTileBits <= kMaxExtraBits, "a shard's local bits fit the single-pass geometry");
+
+// Every instantiation of the tiled Taylor stage (stage_d2_taylor_kernel), keyed by its template flags: device_setup raises
+// the shared-memory limit of each, launch_taylor_order launches the one a stage selects.  Shard variants launch without
+// programmatic dependent launch, because their orders wait for their peers through events.
+enum class TaylorSmem { Tile, TileTable, Shapes };   // the tile; + d2_table_stride(N) doubles; taylor_shapes_smem(N)
+struct TaylorVariant {
+    bool uniform, real_g, shard;
+    int ns;
+    bool cplx;
+    void (*kernel)(TaylorArgs);
+    int rb;
+    TaylorSmem smem;
+    bool pdl;
+};
+
+static const std::vector<TaylorVariant>& taylor_variants() {
+    constexpr int TB = kTaylorTileBits, RB = kTaylorRegBits, RBC = kTaylorCplxRegBits, SM = PB200_TAYLOR_SMAX;
+    using S = TaylorSmem;
+    static const std::vector<TaylorVariant> v = {
+        // one state, one drive coefficient (C2, C5)
+        {true,  true,  false, 0,  false, stage_d2_taylor_kernel<true, true, TB, RB, false, 0, false>,     RB,  S::Tile,      true},
+        {true,  false, false, 0,  false, stage_d2_taylor_kernel<true, false, TB, RB, false, 0, false>,    RB,  S::TileTable, true},
+        // trajectory batch, per-qubit factors of one detuning shape (C4)
+        {false, false, false, 1,  false, stage_d2_taylor_kernel<false, false, TB, RB, false, 1, false>,   RB,  S::TileTable, true},
+        // several detuning shapes: one state (detuning maps), batches
+        {true,  true,  false, SM, false, stage_d2_taylor_kernel<true, true, TB, RB, false, SM, false>,    RB,  S::Shapes,    true},
+        {true,  false, false, SM, false, stage_d2_taylor_kernel<true, false, TB, RB, false, SM, false>,   RB,  S::Shapes,    true},
+        {false, false, false, SM, false, stage_d2_taylor_kernel<false, false, TB, RB, false, SM, false>,  RB,  S::Shapes,    true},
+        // state-vector shards
+        {true,  true,  true,  0,  false, stage_d2_taylor_kernel<true, true, TB, RB, true, 0, false>,      RB,  S::Tile,      false},
+        {true,  false, true,  0,  false, stage_d2_taylor_kernel<true, false, TB, RB, true, 0, false>,     RB,  S::TileTable, false},
+        {true,  true,  true,  SM, false, stage_d2_taylor_kernel<true, true, TB, RB, true, SM, false>,     RB,  S::Shapes,    false},
+        {true,  false, true,  SM, false, stage_d2_taylor_kernel<true, false, TB, RB, true, SM, false>,    RB,  S::Shapes,    false},
+        // complex drive: the phase moves inside the step
+        {true,  false, false, 0,  true,  stage_d2_taylor_kernel<true, false, TB, RBC, false, 0, true>,    RBC, S::TileTable, true},
+        {false, false, false, 1,  true,  stage_d2_taylor_kernel<false, false, TB, RBC, false, 1, true>,   RBC, S::TileTable, true},
+        {true,  false, false, SM, true,  stage_d2_taylor_kernel<true, false, TB, RBC, false, SM, true>,   RBC, S::Shapes,    true},
+        {false, false, false, SM, true,  stage_d2_taylor_kernel<false, false, TB, RBC, false, SM, true>,  RBC, S::Shapes,    true},
+        {true,  false, true,  0,  true,  stage_d2_taylor_kernel<true, false, TB, RBC, true, 0, true>,     RBC, S::TileTable, false},
+        {true,  false, true,  SM, true,  stage_d2_taylor_kernel<true, false, TB, RBC, true, SM, true>,    RBC, S::Shapes,    false},
+    };
+    return v;
+}
 
 // once per device and process: SM count, > 48 KB of dynamic shared memory for the tile kernels
 static int device_setup(int dev) {
@@ -231,25 +275,10 @@ static int device_setup(int dev) {
     CUDA_CHECK(cudaFuncSetAttribute(stage_d2_rb_kernel<true, false, TB, RB>, cudaFuncAttributeMaxDynamicSharedMemorySize, max_smem));
     CUDA_CHECK(cudaFuncSetAttribute(stage_d2_rb_kernel<false, false, TB, RB>, cudaFuncAttributeMaxDynamicSharedMemorySize, max_smem));
     const int taylor_smem = (1 << kTaylorTileBits) * 16 + 2048;   // tile + per-bit table
-    CUDA_CHECK(cudaFuncSetAttribute(stage_d2_taylor_kernel<true, true, kTaylorTileBits, kTaylorRegBits>, cudaFuncAttributeMaxDynamicSharedMemorySize, taylor_smem));
-    CUDA_CHECK(cudaFuncSetAttribute(stage_d2_taylor_kernel<true, false, kTaylorTileBits, kTaylorRegBits>, cudaFuncAttributeMaxDynamicSharedMemorySize, taylor_smem));
-    CUDA_CHECK(cudaFuncSetAttribute(stage_d2_taylor_kernel<false, false, kTaylorTileBits, kTaylorRegBits>, cudaFuncAttributeMaxDynamicSharedMemorySize, taylor_smem));
-    CUDA_CHECK(cudaFuncSetAttribute(stage_d2_taylor_kernel<true, true, kTaylorTileBits, kTaylorRegBits, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, taylor_smem));
-    CUDA_CHECK(cudaFuncSetAttribute(stage_d2_taylor_kernel<true, false, kTaylorTileBits, kTaylorRegBits, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, taylor_smem));
-    const int shapes_smem = (int)taylor_shapes_smem(64);   // several detuning shapes, N <= 64
-    constexpr int SM = PB200_TAYLOR_SMAX;
-    CUDA_CHECK(cudaFuncSetAttribute(stage_d2_taylor_kernel<true, true, kTaylorTileBits, kTaylorRegBits, false, SM>, cudaFuncAttributeMaxDynamicSharedMemorySize, shapes_smem));
-    CUDA_CHECK(cudaFuncSetAttribute(stage_d2_taylor_kernel<true, false, kTaylorTileBits, kTaylorRegBits, false, SM>, cudaFuncAttributeMaxDynamicSharedMemorySize, shapes_smem));
-    CUDA_CHECK(cudaFuncSetAttribute(stage_d2_taylor_kernel<false, false, kTaylorTileBits, kTaylorRegBits, false, SM>, cudaFuncAttributeMaxDynamicSharedMemorySize, shapes_smem));
-    CUDA_CHECK(cudaFuncSetAttribute(stage_d2_taylor_kernel<true, true, kTaylorTileBits, kTaylorRegBits, true, SM>, cudaFuncAttributeMaxDynamicSharedMemorySize, shapes_smem));
-    CUDA_CHECK(cudaFuncSetAttribute(stage_d2_taylor_kernel<true, false, kTaylorTileBits, kTaylorRegBits, true, SM>, cudaFuncAttributeMaxDynamicSharedMemorySize, shapes_smem));
-    // complex-drive steps (the drive's phase moves inside the step)
-    CUDA_CHECK(cudaFuncSetAttribute(stage_d2_taylor_kernel<true, false, kTaylorTileBits, kTaylorCplxRegBits, false, 0, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, taylor_smem));
-    CUDA_CHECK(cudaFuncSetAttribute(stage_d2_taylor_kernel<true, false, kTaylorTileBits, kTaylorCplxRegBits, true, 0, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, taylor_smem));
-    CUDA_CHECK(cudaFuncSetAttribute(stage_d2_taylor_kernel<false, false, kTaylorTileBits, kTaylorCplxRegBits, false, 1, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, taylor_smem));
-    CUDA_CHECK(cudaFuncSetAttribute(stage_d2_taylor_kernel<true, false, kTaylorTileBits, kTaylorCplxRegBits, false, SM, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, shapes_smem));
-    CUDA_CHECK(cudaFuncSetAttribute(stage_d2_taylor_kernel<false, false, kTaylorTileBits, kTaylorCplxRegBits, false, SM, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, shapes_smem));
-    CUDA_CHECK(cudaFuncSetAttribute(stage_d2_taylor_kernel<true, false, kTaylorTileBits, kTaylorCplxRegBits, true, SM, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, shapes_smem));
+    const int shapes_smem = (int)taylor_shapes_smem(64);           // several detuning shapes, N <= 64
+    for (const TaylorVariant& v : taylor_variants())
+        CUDA_CHECK(cudaFuncSetAttribute(v.kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                        v.smem == TaylorSmem::Shapes ? shapes_smem : taylor_smem));
     CUDA_CHECK(cudaFuncSetAttribute(stage_d2_fwd_kernel<true, TB, RB>, cudaFuncAttributeMaxDynamicSharedMemorySize, 2 * 2048 * 16 + 256));
     CUDA_CHECK(cudaFuncSetAttribute(stage_d2_fwd_kernel<false, TB, RB>, cudaFuncAttributeMaxDynamicSharedMemorySize, 2 * 2048 * 16 + 256));
     if (dev >= 0 && dev < PB200_MAX_DEVICES) sm_count[dev] = sms;
@@ -1519,7 +1548,7 @@ static void propagate_mcwf(Plan& P, double t_start, double t_stop, const pb200_r
 static thread_local const char* g_taylor_why = "";   // why the Taylor propagator was not taken (PB200_TAYLOR_LOG)
 static bool taylor_prepare(Plan& P);
 static bool taylor_worthwhile(Plan& P, double gtol);
-static bool taylor_geometry(const Plan& P, std::vector<PassGeom>& passes, bool& use_rb);
+static bool taylor_geometry(const Plan& P, PassGeom& geo, bool& tiled);
 static void propagate_taylor(Plan& P, double t_start, double t_stop, const pb200_run_opts* o, pb200_run_stats* stats);
 
 static void propagate(Plan& P, double t_start, double t_stop, const pb200_run_opts* o, pb200_run_stats* stats) {
@@ -1544,9 +1573,9 @@ static void propagate(Plan& P, double t_start, double t_stop, const pb200_run_op
                                                    // H-applies for a Richardson-CF4 step of the same length)
         }
         if (want) {
-            bool use_rb = false;
-            std::vector<PassGeom> passes;
-            const bool ok = taylor_prepare(P) && taylor_geometry(P, passes, use_rb) &&
+            PassGeom geo;
+            bool tiled = false;
+            const bool ok = taylor_prepare(P) && taylor_geometry(P, geo, tiled) &&
                             (req == 3 || taylor_worthwhile(P, (o && o->tol > 0.0) ? o->tol : 1e-8));
             if (ok) { propagate_taylor(P, t_start, t_stop, o, stats); return; }
             if (env_int("PB200_TAYLOR_LOG", 0)) fprintf(stderr, "taylor not taken: %s\n", g_taylor_why);
@@ -2279,42 +2308,46 @@ static int taylor_order(double h, const std::vector<double>& mj, double tol, dou
     return std::max(kk, 1);
 }
 
-// cplx: a step whose drive phase moves inside it (the CPLX instantiations)
-static void launch_taylor_stage(Plan& P, const PassGeom* geo, const TaylorArgs& a, bool cplx, long long& launches) {
-    const bool uniform = a.table == nullptr;
-    if (geo) {
-        constexpr int TB = kTaylorTileBits, RB = kTaylorRegBits, RBC = kTaylorCplxRegBits, SM = PB200_TAYLOR_SMAX;
-        const bool real_g = a.unit.y == 0.0 && !cplx;
-        const bool local = a.tab_shapes && P.tay.drive_uniform;   // uniform drive, detuning shapes: one state
-        dim3 grid((unsigned)(P.D >> TB), (unsigned)(uniform || local ? 1 : P.B)), block(1 << (TB - (cplx ? RBC : RB)));
-        // the kernel keeps a per-bit table behind the tile unless the drive is uniform and real
-        const size_t smem = a.tab_shapes ? taylor_shapes_smem(P.n)
-                                         : ((size_t)16 << TB) + (uniform && real_g ? 0 : (size_t)d2_table_stride(P.n) * 8);
-        if (cplx) {
-            if (local) launch_k(stage_d2_taylor_kernel<true, false, TB, RBC, false, SM, true>, grid, block, smem, P.stream, true, a);
-            else if (a.tab_shapes) launch_k(stage_d2_taylor_kernel<false, false, TB, RBC, false, SM, true>, grid, block, smem, P.stream, true, a);
-            else if (!uniform) launch_k(stage_d2_taylor_kernel<false, false, TB, RBC, false, 1, true>, grid, block, smem, P.stream, true, a);
-            else launch_k(stage_d2_taylor_kernel<true, false, TB, RBC, false, 0, true>, grid, block, smem, P.stream, true, a);
-        } else if (local && real_g) launch_k(stage_d2_taylor_kernel<true, true, TB, RB, false, SM>, grid, block, smem, P.stream, true, a);
-        else if (local) launch_k(stage_d2_taylor_kernel<true, false, TB, RB, false, SM>, grid, block, smem, P.stream, true, a);
-        else if (a.tab_shapes) launch_k(stage_d2_taylor_kernel<false, false, TB, RB, false, SM>, grid, block, smem, P.stream, true, a);
-        else if (!uniform) launch_k(stage_d2_taylor_kernel<false, false, TB, RB>, grid, block, smem, P.stream, true, a);
-        else if (real_g) launch_k(stage_d2_taylor_kernel<true, true, TB, RB>, grid, block, smem, P.stream, true, a);
-        else launch_k(stage_d2_taylor_kernel<true, false, TB, RB>, grid, block, smem, P.stream, true, a);
-    } else {
-        dim3 grid((unsigned)((P.D + 255) / 256), (unsigned)P.B);
+// One order of a Taylor step: the tiled variant that the plan and the arguments select, or the plain kernel of small
+// registers (!tiled).  cplx: a step whose drive phase moves inside it
+static void launch_taylor_order(const Plan& P, bool tiled, const TaylorArgs& a, bool cplx) {
+    if (!tiled) {
+        const dim3 grid((unsigned)((P.D + 255) / 256), (unsigned)P.B);
         if (cplx) stage_d2_taylor_small_kernel<true><<<grid, 256, 0, P.stream>>>(a);
         else stage_d2_taylor_small_kernel<false><<<grid, 256, 0, P.stream>>>(a);
+        return;
     }
-    ++launches;
+    // one state unless the table holds per-trajectory factors (batches); a uniform drive with detuning shapes is one state
+    const bool uniform = !a.table || (a.tab_shapes && P.tay.drive_uniform);
+    const bool real_g = uniform && !cplx && a.unit.y == 0.0;
+    const bool shard = a.shard_bits > 0;
+    const int ns = a.tab_shapes ? PB200_TAYLOR_SMAX : uniform ? 0 : 1;
+    for (const TaylorVariant& v : taylor_variants()) {
+        if (v.uniform != uniform || v.real_g != real_g || v.shard != shard || v.ns != ns || v.cplx != cplx) continue;
+        const size_t tile = (size_t)16 << kTaylorTileBits;
+        const size_t smem = v.smem == TaylorSmem::Shapes      ? taylor_shapes_smem(P.n)
+                            : v.smem == TaylorSmem::TileTable ? tile + (size_t)d2_table_stride(P.n) * 8
+                                                              : tile;
+        launch_k(v.kernel, dim3((unsigned)(P.D >> kTaylorTileBits), uniform ? 1u : (unsigned)P.B),
+                 dim3(1u << (kTaylorTileBits - v.rb)), smem, P.stream, v.pdl, a);
+        return;
+    }
+    fail(PB200_ERR_UNSUPPORTED, "no Taylor stage kernel for UNIFORM=%d REAL_G=%d SHARD=%d NS=%d CPLX=%d", uniform, real_g,
+         shard, ns, cplx);
 }
 
-// geometry of the Taylor stage: the register-blocked single-pass kernel on its own 2^kTaylorTileBits tile (whatever
-// tile the Magnus stages use), or the plain kernel for small registers
-static bool taylor_geometry(const Plan& P, std::vector<PassGeom>& passes, bool& use_rb) {
-    passes = plan_passes(P.n, kTaylorTileBits, kMaxExtraBits);
-    use_rb = passes.size() == 1 && passes[0].first_pass && passes[0].hi_bits == 0 && passes[0].lo_bits == kTaylorTileBits;
-    return use_rb || P.n <= 16;
+// Geometry of the Taylor stage on the 2^L amplitudes a plan holds (L = N, or N - shard_bits on a shard): the
+// register-blocked single-pass kernel on its own 2^kTaylorTileBits tile (whatever tile the Magnus stages use), the local
+// bits above the tile as partner loads (tiled), or the plain kernel for small registers.  n_bits is the global N.
+// False where neither applies; a shard without the single-pass geometry is refused.
+static bool taylor_geometry(const Plan& P, PassGeom& geo, bool& tiled) {
+    const int L = P.n - P.shard_bits;
+    const std::vector<PassGeom> passes = plan_passes(L, kTaylorTileBits, kMaxExtraBits);
+    if (P.shard_bits && passes.size() != 1) fail(PB200_ERR_UNSUPPORTED, "shard of 2^%d amplitudes: no single-pass geometry", L);
+    geo = passes[0];
+    geo.n_bits = P.n;
+    tiled = passes.size() == 1 && geo.first_pass && geo.hi_bits == 0 && geo.lo_bits == kTaylorTileBits;
+    return tiled || P.n <= 16;
 }
 
 // One step of the Taylor propagator as the host schedules it: the polynomial fits, the centres gamma_j, the order K and
@@ -2336,9 +2369,10 @@ struct TaylorStep {
     int ring() const { return (n_chi - 1) + n_g * (drive == 2 ? 2 : 1) + 1; }   // state-sized buffers beyond the state
 };
 
-// Host half of propagate_taylor: the steps of one call [t_start, t_stop], one at a time (next()), with the statistics
-// the launches do not change.  The single-plan path launches every step as soon as it is scheduled (the host fit of
-// the next step overlaps the device work); the sharded path schedules the whole call before its first launch.
+// Host half of the Taylor propagator (taylor_launch_steps is the launching half): the steps of one call
+// [t_start, t_stop], one at a time (next()), with the statistics the launches do not change.  A whole state launches
+// every step as soon as it is scheduled (the host fit of the next step overlaps the device work); shards schedule the
+// whole call before their first launch.
 struct TaylorScheduler {
     Plan& P;
     double t_stop, eps = 1e-12, gtol, rate, rho_target, fit_total, fit_spent = 0.0, round2 = 0.0;
@@ -2414,178 +2448,189 @@ struct TaylorScheduler {
         return F;
     }
 
+    // end of the longest candidate step from t (in interval i0): rho accumulated over the sampling intervals up to
+    // rho_target, or the length a step cut by the rho check left behind
+    double candidate_end(int i0) {
+        const Plan::TaylorCache& C = P.tay;
+        double b = t, acc = 0.0, cur = t;
+        int i = i0;
+        while (i < nt - 1) {
+            const double e1 = std::min(P.times[i + 1], t_stop);
+            const double w = std::max(C.w_knot[i], C.w_knot[i + 1]);
+            const double need = w * (e1 - cur);
+            if (acc + need > rho_target) {
+                if (i == i0 || acc == 0.0) b = cur + (rho_target - acc) / std::max(w, 1e-300);  // inside the first interval
+                else b = cur;
+                break;
+            }
+            acc += need; cur = e1; b = e1; ++i;
+            if (e1 >= t_stop - eps) break;
+        }
+        b = std::min(b, t_stop);
+        if (t_retry_len > 0.0) { b = std::min(b, t + t_retry_len); t_retry_len = 0.0; }
+        if (b <= t + eps) b = std::min(P.times[i0 + 1], t_stop);
+        return b;
+    }
+
+    // longest step [t, b] on which every spline is a polynomial of degree <= PB200_TAYLOR_PMAX to within the budget:
+    // bisection over the number of whole sampling intervals beyond the first one (a step inside one interval is a cubic:
+    // exact).  b comes in as the candidate end.
+    Fit longest_fit(int i0, double& b) {
+        const bool single = b <= P.times[i0 + 1] + eps;
+        Fit F = fit_step(t, b - t, single);
+        if (F.ok || single) return F;
+        int lo_keep = 0, hi_keep = find_piece(P.times, b - eps) - i0;   // lo passes (one interval), hi fails
+        Fit Flo; bool have_lo = false;
+        while (hi_keep - lo_keep > 1) {
+            const int mid = (lo_keep + hi_keep) / 2;
+            const double bm = P.times[i0 + 1 + mid];
+            Fit Fm = fit_step(t, bm - t, false);
+            if (Fm.ok) { lo_keep = mid; Flo = Fm; have_lo = true; } else hi_keep = mid;
+        }
+        b = P.times[i0 + 1 + lo_keep];
+        return have_lo ? Flo : fit_step(t, b - t, lo_keep == 0);
+    }
+
+    // Drive of a step where the plan's phase moves: one phase over the step (the imaginary part after the rotation onto
+    // the phase of the largest of omega(0), omega(1/2), omega(1) fits in the drive's allowance, booked as fit residual)
+    // runs the real kernels with the step's own unit; otherwise the complex kernels.  Returns the drive's fit residual.
+    double classify_drive(Fit& F, int& drive, c2& unit) const {
+        auto coef = [](const std::vector<double>& c, size_t j) { return j < c.size() ? c[j] : 0.0; };
+        auto poly = [](const std::vector<double>& c, double u) {
+            double v = 0.0;
+            for (int i = (int)c.size() - 1; i >= 0; --i) v = v * u + c[i];
+            return v;
+        };
+        double best = 0.0, cph = 1.0, sph = 0.0;
+        for (double u : {0.0, 0.5, 1.0}) {
+            const double x = poly(F.om.c, u), y = poly(F.omi.c, u), r = std::hypot(x, y);
+            if (r > best) { best = r; cph = x / r; sph = y / r; }
+        }
+        const size_t nc = std::max(F.om.c.size(), F.omi.c.size());
+        std::vector<double> xr(nc), yr(nc);   // omega e^{-i phase}
+        double ybound = 0.0;
+        for (size_t j = 0; j < nc; ++j) {
+            xr[j] = cph * coef(F.om.c, j) + sph * coef(F.omi.c, j);
+            yr[j] = cph * coef(F.omi.c, j) - sph * coef(F.om.c, j);
+            ybound += std::fabs(yr[j]);
+        }
+        const double r2 = F.om.resid + F.omi.resid;   // |omega - fit| <= |r_re + i r_im|
+        if (r2 + ybound <= F.om_allow) {
+            F.om.c = xr;
+            if (cph != 1.0 || sph != 0.0) {
+                const c2 u = P.tay.unit;
+                drive = 1;
+                unit = {u.x * cph - u.y * sph, u.x * sph + u.y * cph};
+            }
+            return r2 + ybound;
+        }
+        drive = 2;
+        return r2;
+    }
+
+    // strip trailing zero coefficients (of omega's imaginary part too on a complex step); returns the shapes' degree
+    static int trim(Fit& F, bool cplx) {
+        auto trim1 = [](std::vector<double>& c, double scale) {
+            while (c.size() > 1 && std::fabs(c.back()) <= 1e-15 * scale) c.pop_back();
+        };
+        double so = 0.0, sh = 0.0;
+        for (double v : F.om.c) so = std::max(so, std::fabs(v));
+        if (cplx) for (double v : F.omi.c) so = std::max(so, std::fabs(v));
+        for (double v : F.th.c) sh = std::max(sh, std::fabs(v));
+        trim1(F.om.c, std::max(so, 1e-300)); trim1(F.th.c, std::max(sh, 1e-300));
+        if (cplx) trim1(F.omi.c, std::max(so, 1e-300));
+        int p_m = 0;
+        for (int q = 0; q < PB200_TAYLOR_SMAX; ++q) {
+            double sm = 0.0;
+            for (double v : F.m[q].c) sm = std::max(sm, std::fabs(v));
+            trim1(F.m[q].c, std::max(sm, 1e-300));
+            p_m = std::max(p_m, (int)F.m[q].c.size() - 1);
+        }
+        return p_m;
+    }
+
+    // centres gamma_j and norm bounds m_j of H_j, j <= p
+    void centres_and_bounds(const Fit& F, bool cplx, int p_om, int p, std::vector<double>& gam, std::vector<double>& mj) const {
+        auto th_c = [&](int j) { return j < (int)F.th.c.size() ? F.th.c[j] : 0.0; };
+        auto m_c = [&](int q, int j) { return j < (int)F.m[q].c.size() ? F.m[q].c[j] : 0.0; };
+        // |omega_j|: the spectrum of omega_j X does not depend on the phase of omega_j
+        auto om_abs = [&](int j) {
+            const double x = j < (int)F.om.c.size() ? F.om.c[j] : 0.0;
+            if (!cplx) return std::fabs(x);
+            return std::hypot(x, j < (int)F.omi.c.size() ? F.omi.c[j] : 0.0);
+        };
+        gam.assign(p + 1, 0.0); mj.assign(p + 1, 0.0);
+        double c0, hw0, mv[PB200_TAYLOR_SMAX];
+        for (int q = 0; q < PB200_TAYLOR_SMAX; ++q) mv[q] = m_c(q, 0);
+        taylor_bounds(P, cplx ? om_abs(0) : F.om.c[0], F.th.c[0], mv, c0, hw0);
+        gam[0] = c0; mj[0] = hw0;
+        for (int j = 1; j <= p; ++j) {
+            const double thj = th_c(j), omj = j <= p_om ? om_abs(j) : 0.0;
+            gam[j] = -thj * 0.5 * N;
+            double mm = 0.0;
+            for (int q = 0; q < ns; ++q) mm += std::fabs(m_c(q, j)) * C_sum[q];
+            mj[j] = std::fabs(thj) * 0.5 * N + mm + std::fabs(omj) * A_sum;
+        }
+    }
+
+    // the order of step s, its log line and its share of the error estimate; rho = h sum_j m_j / (j + 1)
+    void record(TaylorStep& s, const Fit& F, const std::vector<double>& mj, int p_m, double om_resid, double rho) {
+        double trunc_bound = 0.0;
+        s.K = taylor_order(s.h, mj, std::max(1e-15, 0.1 * rate * s.h), trunc_bound);
+        st.n_applies += s.K; st.n_exponentials += 1; ++st.n_steps;
+        if (log_steps)
+            fprintf(stderr, "taylor step t=%.6f h_ns=%.3f p_om=%d p_th=%d p_m=%d K=%d ring=%d rho=%.3f resid=%.2e/%.2e/%.2e drive=%s\n",
+                    s.t, s.h * 1e3, s.p_om, s.p_th, p_m, s.K, s.ring() + 1, mj[0] * s.h, om_resid, F.th.resid, F.m[0].resid,
+                    s.drive == 2 ? "cplx" : s.drive == 1 ? "rot" : "real");
+        st.max_rho = std::max(st.max_rho, rho);
+        double fit_m = 0.0;
+        for (int q = 0; q < ns; ++q) fit_m += C_sum[q] * F.m[q].resid;
+        const double fit_err = s.h * (A_sum * om_resid + N * F.th.resid + fit_m);
+        st.err_estimate += trunc_bound + fit_err;
+        fit_spent += fit_err;
+        { const double r = kRoundUnit * std::exp(std::min(rho, 40.0)); round2 += r * r; }
+        steps_len += s.h;
+    }
+
     // the next step of the call; false once t_stop is reached
     bool next(TaylorStep& s) {
-        const Plan::TaylorCache& C = P.tay;
         while (t < t_stop - eps) {
             const int i0 = find_piece(P.times, t + eps);
-            // longest candidate: accumulate rho over the sampling intervals
-            double b = t;
-            {
-                double acc = 0.0;
-                int i = i0;
-                double cur = t;
-                while (i < nt - 1) {
-                    const double e1 = std::min(P.times[i + 1], t_stop);
-                    const double w = std::max(C.w_knot[i], C.w_knot[i + 1]);
-                    const double need = w * (e1 - cur);
-                    if (acc + need > rho_target) {
-                        if (i == i0 || acc == 0.0) b = cur + (rho_target - acc) / std::max(w, 1e-300);  // inside the first interval
-                        else b = cur;
-                        break;
-                    }
-                    acc += need; cur = e1; b = e1; ++i;
-                    if (e1 >= t_stop - eps) break;
-                }
-                b = std::min(b, t_stop);
-                if (t_retry_len > 0.0) { b = std::min(b, t + t_retry_len); t_retry_len = 0.0; }
-                if (b <= t + eps) b = std::min(P.times[i0 + 1], t_stop);
-            }
-            // longest step on which both splines are polynomials of degree <= PB200_TAYLOR_PMAX to within the budget: bisection over
-            // the number of whole sampling intervals beyond the first one (a step inside one interval is a cubic: exact)
-            Fit F;
-            {
-                bool single = b <= P.times[i0 + 1] + eps;
-                F = fit_step(t, b - t, single);
-                if (!F.ok && !single) {
-                    int lo_keep = 0, hi_keep = find_piece(P.times, b - eps) - i0;   // lo passes (one interval), hi fails
-                    Fit Flo; bool have_lo = false;
-                    while (hi_keep - lo_keep > 1) {
-                        const int mid = (lo_keep + hi_keep) / 2;
-                        const double bm = P.times[i0 + 1 + mid];
-                        Fit Fm = fit_step(t, bm - t, false);
-                        if (Fm.ok) { lo_keep = mid; Flo = Fm; have_lo = true; } else hi_keep = mid;
-                    }
-                    b = P.times[i0 + 1 + lo_keep];
-                    single = lo_keep == 0;
-                    F = have_lo ? Flo : fit_step(t, b - t, single);
-                }
-            }
-            double h = b - t;
-            // drive of the step where the plan's phase moves: one phase over the step (the imaginary part after the
-            // rotation onto the phase of the largest of omega(0), omega(1/2), omega(1) fits in the drive's allowance,
-            // booked as fit residual) runs the real kernels with the step's own unit; otherwise the complex kernels
+            double b = candidate_end(i0);
+            Fit F = longest_fit(i0, b);
+            const double h = b - t;
             int drive = 0;
-            c2 sunit = C.unit;
-            double om_resid = F.om.resid;
-            if (C.phase_moves) {
-                auto coef = [](const std::vector<double>& c, size_t j) { return j < c.size() ? c[j] : 0.0; };
-                auto poly = [](const std::vector<double>& c, double u) {
-                    double v = 0.0;
-                    for (int i = (int)c.size() - 1; i >= 0; --i) v = v * u + c[i];
-                    return v;
-                };
-                double best = 0.0, cph = 1.0, sph = 0.0;
-                for (double u : {0.0, 0.5, 1.0}) {
-                    const double x = poly(F.om.c, u), y = poly(F.omi.c, u), r = std::hypot(x, y);
-                    if (r > best) { best = r; cph = x / r; sph = y / r; }
-                }
-                const size_t nc = std::max(F.om.c.size(), F.omi.c.size());
-                std::vector<double> xr(nc), yr(nc);   // omega e^{-i phase}
-                double ybound = 0.0;
-                for (size_t j = 0; j < nc; ++j) {
-                    xr[j] = cph * coef(F.om.c, j) + sph * coef(F.omi.c, j);
-                    yr[j] = cph * coef(F.omi.c, j) - sph * coef(F.om.c, j);
-                    ybound += std::fabs(yr[j]);
-                }
-                const double r2 = F.om.resid + F.omi.resid;   // |omega - fit| <= |r_re + i r_im|
-                if (r2 + ybound <= F.om_allow) {
-                    F.om.c = xr;
-                    om_resid = r2 + ybound;
-                    if (cph != 1.0 || sph != 0.0) {
-                        drive = 1;
-                        sunit = {C.unit.x * cph - C.unit.y * sph, C.unit.x * sph + C.unit.y * cph};
-                    }
-                } else {
-                    drive = 2;
-                    om_resid = r2;
-                }
-            }
-            // strip trailing zero coefficients
-            auto trim = [](std::vector<double>& c, double scale) {
-                while (c.size() > 1 && std::fabs(c.back()) <= 1e-15 * scale) c.pop_back();
-            };
-            int p_m = 0;
-            {
-                double so = 0.0, sh = 0.0;
-                for (double v : F.om.c) so = std::max(so, std::fabs(v));
-                if (drive == 2) for (double v : F.omi.c) so = std::max(so, std::fabs(v));
-                for (double v : F.th.c) sh = std::max(sh, std::fabs(v));
-                trim(F.om.c, std::max(so, 1e-300)); trim(F.th.c, std::max(sh, 1e-300));
-                if (drive == 2) trim(F.omi.c, std::max(so, 1e-300));
-                for (int q = 0; q < PB200_TAYLOR_SMAX; ++q) {
-                    double sm = 0.0;
-                    for (double v : F.m[q].c) sm = std::max(sm, std::fabs(v));
-                    trim(F.m[q].c, std::max(sm, 1e-300));
-                    p_m = std::max(p_m, (int)F.m[q].c.size() - 1);
-                }
-            }
+            c2 unit = P.tay.unit;
+            const double om_resid = P.tay.phase_moves ? classify_drive(F, drive, unit) : F.om.resid;
+            const int p_m = trim(F, drive == 2);
             const int p_om = std::max((int)F.om.c.size(), drive == 2 ? (int)F.omi.c.size() : 0) - 1;
             const int p_th = std::max((int)F.th.c.size() - 1, p_m);   // degree of the diagonal (own-element) history
             const int p = std::max(p_om, p_th);
-            auto th_c = [&](int j) { return j < (int)F.th.c.size() ? F.th.c[j] : 0.0; };
-            auto m_c = [&](int q, int j) { return j < (int)F.m[q].c.size() ? F.m[q].c[j] : 0.0; };
-            // |omega_j|: the spectrum of omega_j X does not depend on the phase of omega_j
-            auto om_abs = [&](int j) {
-                const double x = j < (int)F.om.c.size() ? F.om.c[j] : 0.0;
-                if (drive != 2) return std::fabs(x);
-                return std::hypot(x, j < (int)F.omi.c.size() ? F.omi.c[j] : 0.0);
-            };
-            // centres and norm bounds of H_j
-            std::vector<double> gam(p + 1, 0.0), mj(p + 1, 0.0);
-            {
-                double c0, hw0, mv[PB200_TAYLOR_SMAX];
-                for (int q = 0; q < PB200_TAYLOR_SMAX; ++q) mv[q] = m_c(q, 0);
-                taylor_bounds(P, drive == 2 ? om_abs(0) : F.om.c[0], F.th.c[0], mv, c0, hw0);
-                gam[0] = c0; mj[0] = hw0;
-                for (int j = 1; j <= p; ++j) {
-                    const double thj = th_c(j), omj = j <= p_om ? om_abs(j) : 0.0;
-                    gam[j] = -thj * 0.5 * N;
-                    double mm = 0.0;
-                    for (int q = 0; q < ns; ++q) mm += std::fabs(m_c(q, j)) * C_sum[q];
-                    mj[j] = std::fabs(thj) * 0.5 * N + mm + std::fabs(omj) * A_sum;
-                }
+            std::vector<double> gam, mj;
+            centres_and_bounds(F, drive == 2, p_om, p, gam, mj);
+            // the fp64 cancellation of the series grows like e^rho: a step whose majorant exponent overshoots the target
+            // (the half-width grew inside the step) is cut and fitted again
+            double rho = 0.0;
+            for (int j = 0; j <= p; ++j) rho += mj[j] / (j + 1);
+            rho *= h;
+            if (rho > 1.12 * rho_target && h > 1e-9) {
+                t_retry_len = h * rho_target / rho;
+                continue;
             }
-            {   // the fp64 cancellation of the series grows like e^rho: a step whose majorant exponent overshoots the
-                // target (the half-width grew inside the step) is cut and fitted again
-                double rho_eff = 0.0;
-                for (int j = 0; j <= p; ++j) rho_eff += mj[j] / (j + 1);
-                rho_eff *= h;
-                if (rho_eff > 1.12 * rho_target && h > 1e-9) {
-                    t_retry_len = h * rho_target / rho_eff;
-                    continue;
-                }
-            }
-            double trunc_bound = 0.0;
-            const int K = taylor_order(h, mj, std::max(1e-15, 0.1 * rate * h), trunc_bound);
             s.t = t; s.h = h;
             s.om = F.om.c; s.th = F.th.c;
             for (int q = 0; q < PB200_TAYLOR_SMAX; ++q) s.m[q] = F.m[q].c;
             s.p_om = p_om; s.p_th = p_th; s.p = p;
-            s.gam = gam; s.K = K;
+            s.gam = gam;
             s.n_chi = p_th + 2;
             s.n_g = p_om >= 1 ? p_om + 1 : 0;
-            s.drive = drive; s.unit = sunit;
+            s.drive = drive; s.unit = unit;
             s.omi = drive == 2 ? F.omi.c : std::vector<double>();
             // phase of the scalar centre: exp(-i h int_0^1 sum_j gam_j u^j du)
             double phi = 0.0;
             for (int j = 0; j <= p; ++j) phi += gam[j] / (j + 1);
             s.phi = phi * h;
-            st.n_applies += K; st.n_exponentials += 1; ++st.n_steps;
-            if (log_steps)
-                fprintf(stderr, "taylor step t=%.6f h_ns=%.3f p_om=%d p_th=%d p_m=%d K=%d ring=%d rho=%.3f resid=%.2e/%.2e/%.2e drive=%s\n",
-                        t, h * 1e3, p_om, p_th, p_m, K, s.ring() + 1, mj[0] * h, om_resid, F.th.resid, F.m[0].resid,
-                        drive == 2 ? "cplx" : drive == 1 ? "rot" : "real");
-            double rho_eff = 0.0;
-            for (int j = 0; j <= p; ++j) rho_eff += mj[j] / (j + 1);
-            st.max_rho = std::max(st.max_rho, rho_eff * h);
-            double fit_m = 0.0;
-            for (int q = 0; q < ns; ++q) fit_m += C_sum[q] * F.m[q].resid;
-            const double fit_err = h * (A_sum * om_resid + N * F.th.resid + fit_m);
-            st.err_estimate += trunc_bound + fit_err;
-            fit_spent += fit_err;
-            { const double r = kRoundUnit * std::exp(std::min(rho_eff * h, 40.0)); round2 += r * r; }
-            steps_len += h;
+            record(s, F, mj, p_m, om_resid, rho);
             t = b;
             return true;
         }
@@ -2637,23 +2682,30 @@ static TaylorRing taylor_ring(Plan& P, const TaylorStep& s) {
     return R;
 }
 
-// arguments of order k of a step
-static TaylorArgs taylor_args(const Plan& P, const PassGeom& geo, const TaylorStep& s, const TaylorRing& R, int k) {
-    const Plan::TaylorCache& C = P.tay;
-    auto th_c = [&](int j) { return j < (int)s.th.size() ? s.th[j] : 0.0; };
-    auto m_c = [&](int q, int j) { return j < (int)s.m[q].size() ? s.m[q][j] : 0.0; };
+// the arguments of a Taylor stage that depend on the plan alone: chi_k = v and chi_{k+1} = out, the interaction, the
+// per-trajectory table, the drive's states and unit, the shard.  Everything else is zero: scale, history, accumulator
+static TaylorArgs taylor_plan_args(const Plan& P, const PassGeom& geo, const c2* v, c2* out, c2 unit) {
     TaylorArgs a{};
-    a.v = R.chi[k % s.n_chi]; a.out = R.chi[(k + 1) % s.n_chi];
-    a.g_out = (s.n_g && k + 1 < s.K) ? R.gr[k % s.n_g] : nullptr;
-    a.acc = R.acc_slot->get();
+    a.v = v; a.out = out;
     a.dint = P.has_interaction ? P.dint.get() : nullptr;
     a.dint_stride = P.dint_shared ? 0 : P.D;
     a.D = P.D;
     a.geo = geo;
-    a.unit = s.unit;
-    a.table = C.uniform ? nullptr : C.d_tab.get();
-    a.tab_shapes = C.tab_shapes;
+    a.unit = unit;
+    a.table = P.tay.uniform ? nullptr : P.tay.d_tab.get();
+    a.tab_shapes = P.tay.tab_shapes;
     a.to_bit = P.desc.drives[0].state_to; a.from_is_one = P.desc.drives[0].state_from;
+    a.shard_bits = P.shard_bits; a.shard = P.shard;
+    return a;
+}
+
+// arguments of order k of a step
+static TaylorArgs taylor_args(const Plan& P, const PassGeom& geo, const TaylorStep& s, const TaylorRing& R, int k) {
+    auto th_c = [&](int j) { return j < (int)s.th.size() ? s.th[j] : 0.0; };
+    auto m_c = [&](int q, int j) { return j < (int)s.m[q].size() ? s.m[q][j] : 0.0; };
+    TaylorArgs a = taylor_plan_args(P, geo, R.chi[k % s.n_chi], R.chi[(k + 1) % s.n_chi], s.unit);
+    a.g_out = (s.n_g && k + 1 < s.K) ? R.gr[k % s.n_g] : nullptr;
+    a.acc = R.acc_slot->get();
     a.th0 = s.th[0]; a.gam0 = s.gam[0]; a.om0 = s.om[0];
     for (int q = 0; q < PB200_TAYLOR_SMAX; ++q) a.m0[q] = m_c(q, 0);
     a.scale = {0.0, -s.h / (k + 1)};
@@ -2682,30 +2734,87 @@ static TaylorArgs taylor_args(const Plan& P, const PassGeom& geo, const TaylorSt
     return a;
 }
 
-static void propagate_taylor(Plan& P, double t_start, double t_stop, const pb200_run_opts* o, pb200_run_stats* stats) {
-    std::vector<PassGeom> passes;
-    bool use_rb = false;
-    if (!taylor_geometry(P, passes, use_rb)) fail(PB200_ERR_UNSUPPORTED, "Taylor propagator: unsupported register size");
-    EventPair evs;
-    CUDA_CHECK(cudaEventRecord(evs.a, P.stream));
-    ensure_aux_buffers(P);
-    TaylorScheduler S(P, t_start, t_stop, o);
-    TaylorStep s;
-    long long launches = 0;
+// CUDA events of a group of plans, one per plan, released on every exit path
+struct ShardEvents {
+    std::vector<cudaEvent_t> ev;
+    ShardEvents(const std::vector<Plan*>& G, unsigned flags) : ev(G.size(), nullptr) {
+        for (size_t r = 0; r < G.size(); ++r) {
+            CUDA_CHECK(cudaSetDevice(G[r]->desc.device));
+            CUDA_CHECK(cudaEventCreateWithFlags(&ev[r], flags));
+        }
+    }
+    ~ShardEvents() { for (cudaEvent_t e : ev) if (e) cudaEventDestroy(e); }
+    ShardEvents(const ShardEvents&) = delete;
+    ShardEvents& operator=(const ShardEvents&) = delete;
+};
+
+// Launching half of the Taylor propagator for the plans that hold one state: {&P}, or the linked shards in shard order.
+// next(s) yields the steps of the call.  Returns the largest device time of any plan, in ms.  On shards, order k on
+// shard r reads chi_k of its peers: it waits for the previous launch (order k - 1, or the last order of the previous
+// step) of every peer, and every shard's waits for an order are enqueued before any shard records that order's event.
+// A slot a peer may still be gathering from is never overwritten: n_chi >= 2, and every order waits for the one before
+// it.  The previous call ended with every stream synchronised.  A whole state records no event per order, so
+// programmatic dependent launch chains its orders.
+template <class Next>
+static float taylor_launch_steps(const std::vector<Plan*>& G, const PassGeom& geo, bool tiled, Next&& next,
+                                 long long& launches) {
+    const int count = (int)G.size(), sb = G[0]->shard_bits;
+    // plan r, its device current (a whole state's already is)
+    auto use = [&](int r) -> Plan& {
+        if (count > 1) CUDA_CHECK(cudaSetDevice(G[r]->desc.device));
+        return *G[r];
+    };
+    ShardEvents order_ev(sb ? G : std::vector<Plan*>(), cudaEventDisableTiming), t0(G, cudaEventDefault),
+        t1(G, cudaEventDefault);
+    for (int r = 0; r < count; ++r) CUDA_CHECK(cudaEventRecord(t0.ev[r], use(r).stream));
+    bool first = true;
+    std::vector<TaylorRing> R(count);
     std::deque<std::vector<double>> tables;   // tables of rotated steps, until the call's last synchronisation
-    while (S.next(s)) {
-        const TaylorRing R = taylor_ring(P, s);
-        taylor_table_unit(P, s.drive == 1 ? s.unit : P.tay.unit, tables);
-        for (int k = 0; k < s.K; ++k)
-            launch_taylor_stage(P, use_rb ? &passes[0] : nullptr, taylor_args(P, passes[0], s, R, k), s.drive == 2, launches);
+    for (TaylorStep s; next(s);) {
+        for (int r = 0; r < count; ++r) {
+            Plan& P = use(r);
+            R[r] = taylor_ring(P, s);
+            taylor_table_unit(P, s.drive == 1 ? s.unit : P.tay.unit, tables);
+        }
+        for (int k = 0; k < s.K; ++k) {
+            for (int r = 0; r < count; ++r) {
+                Plan& P = use(r);
+                TaylorArgs a = taylor_args(P, geo, s, R[r], k);
+                for (int q = 0; q < sb; ++q) {
+                    const int peer = r ^ (1 << q);
+                    a.peer[q] = R[peer].chi[k % s.n_chi];
+                    if (!first) CUDA_CHECK(cudaStreamWaitEvent(P.stream, order_ev.ev[peer], 0));
+                }
+                launch_taylor_order(P, tiled, a, s.drive == 2);
+                ++launches;
+            }
+            for (int r = 0; r < count && sb; ++r) CUDA_CHECK(cudaEventRecord(order_ev.ev[r], use(r).stream));
+            first = false;
+        }
         CUDA_CHECK(cudaGetLastError());
         // the accumulator becomes the current state buffer
-        std::swap(P.buf[P.cur], *R.acc_slot);
+        for (int r = 0; r < count; ++r) std::swap(G[r]->buf[G[r]->cur], *R[r].acc_slot);
     }
-    CUDA_CHECK(cudaEventRecord(evs.b, P.stream));
-    CUDA_CHECK(cudaEventSynchronize(evs.b));
-    float ms = 0.f;
-    CUDA_CHECK(cudaEventElapsedTime(&ms, evs.a, evs.b));
+    float ms_max = 0.f;
+    for (int r = 0; r < count; ++r) CUDA_CHECK(cudaEventRecord(t1.ev[r], use(r).stream));
+    for (int r = 0; r < count; ++r) {
+        CUDA_CHECK(cudaEventSynchronize(t1.ev[r]));
+        float ms = 0.f;
+        CUDA_CHECK(cudaEventElapsedTime(&ms, t0.ev[r], t1.ev[r]));
+        ms_max = std::max(ms_max, ms);
+    }
+    return ms_max;
+}
+
+// a whole state: each step is launched as soon as it is scheduled, so the host fit of the next step overlaps the device
+static void propagate_taylor(Plan& P, double t_start, double t_stop, const pb200_run_opts* o, pb200_run_stats* stats) {
+    PassGeom geo;
+    bool tiled = false;
+    if (!taylor_geometry(P, geo, tiled)) fail(PB200_ERR_UNSUPPORTED, "Taylor propagator: unsupported register size");
+    ensure_aux_buffers(P);
+    TaylorScheduler S(P, t_start, t_stop, o);
+    long long launches = 0;
+    const float ms = taylor_launch_steps({&P}, geo, tiled, [&S](TaylorStep& s) { return S.next(s); }, launches);
     if (stats) *stats = S.finish(ms, launches);
 }
 
@@ -2794,36 +2903,8 @@ static void refuse_shard(const Plan& P, const char* who, const char* instead) {
 // ---- state-vector shards -------------------------------------------------------------------------------------------
 // A shard is an ordinary plan holding 2^L amplitudes (L = N - shard_bits) of one state: the global indices
 // [shard 2^L, (shard + 1) 2^L).  One process drives every shard of a group: the host schedule of a call is computed
-// once, then every order of the Taylor series is launched on every shard (stage_d2_taylor_kernel<..., true>), whose
-// partners across a shard bit are loads from the peer's chi_k (peer access between distinct devices).
-
-// the one-pass geometry of a slice: the 2^13 tile, the local bits above it as partner loads; n_bits = global N
-static PassGeom shard_geometry(const Plan& P) {
-    const std::vector<PassGeom> passes = plan_passes(P.n - P.shard_bits, kTaylorTileBits, kShardMaxLocalBits - kTaylorTileBits);
-    if (passes.size() != 1) fail(PB200_ERR_UNSUPPORTED, "shard of 2^%d amplitudes: no single-pass geometry", P.n - P.shard_bits);
-    PassGeom g = passes[0];
-    g.n_bits = P.n;
-    return g;
-}
-
-// one order on one shard; no programmatic dependent launch: an order waits for its peers through events.  cplx: a step
-// whose drive phase moves inside it
-static void launch_taylor_shard(Plan& P, const TaylorArgs& a, bool cplx) {
-    constexpr int TB = kTaylorTileBits, RB = kTaylorRegBits, RBC = kTaylorCplxRegBits, SM = PB200_TAYLOR_SMAX;
-    const bool real_g = a.unit.y == 0.0 && !cplx;
-    dim3 grid((unsigned)(P.D >> TB)), block(1 << (TB - (cplx ? RBC : RB)));
-    if (a.table) {   // detuning shapes (the drive of a shard is uniform: pb200_shards_link)
-        const size_t smem = taylor_shapes_smem(P.n);
-        if (cplx) launch_k(stage_d2_taylor_kernel<true, false, TB, RBC, true, SM, true>, grid, block, smem, P.stream, false, a);
-        else if (real_g) launch_k(stage_d2_taylor_kernel<true, true, TB, RB, true, SM>, grid, block, smem, P.stream, false, a);
-        else launch_k(stage_d2_taylor_kernel<true, false, TB, RB, true, SM>, grid, block, smem, P.stream, false, a);
-        return;
-    }
-    const size_t smem = ((size_t)16 << TB) + (real_g ? 0 : (size_t)d2_table_stride(P.n) * 8);
-    if (cplx) launch_k(stage_d2_taylor_kernel<true, false, TB, RBC, true, 0, true>, grid, block, smem, P.stream, false, a);
-    else if (real_g) launch_k(stage_d2_taylor_kernel<true, true, TB, RB, true>, grid, block, smem, P.stream, false, a);
-    else launch_k(stage_d2_taylor_kernel<true, false, TB, RB, true>, grid, block, smem, P.stream, false, a);
-}
+// once, then every order of the Taylor series is launched on every shard (taylor_launch_steps), whose partners
+// across a shard bit are loads from the peer's chi_k (peer access between distinct devices).
 
 // plans[i] = shard i of a group linked by pb200_shards_link
 static std::vector<Plan*> shard_group(pb200_plan** plans, int count, const char* who) {
@@ -2839,20 +2920,6 @@ static std::vector<Plan*> shard_group(pb200_plan** plans, int count, const char*
     return G;
 }
 
-// CUDA events of a group, one per shard, released on every exit path
-struct ShardEvents {
-    std::vector<cudaEvent_t> ev;
-    ShardEvents(const std::vector<Plan*>& G, unsigned flags) : ev(G.size(), nullptr) {
-        for (size_t r = 0; r < G.size(); ++r) {
-            CUDA_CHECK(cudaSetDevice(G[r]->desc.device));
-            CUDA_CHECK(cudaEventCreateWithFlags(&ev[r], flags));
-        }
-    }
-    ~ShardEvents() { for (cudaEvent_t e : ev) if (e) cudaEventDestroy(e); }
-    ShardEvents(const ShardEvents&) = delete;
-    ShardEvents& operator=(const ShardEvents&) = delete;
-};
-
 static void shards_sync(const std::vector<Plan*>& G) {
     for (Plan* P : G) {
         CUDA_CHECK(cudaSetDevice(P->desc.device));
@@ -2864,7 +2931,9 @@ static void shards_sync(const std::vector<Plan*>& G) {
 // (Dint - theta n_from + omega X) v.  The inputs are complete (every stream synchronised) before any shard reads a peer's.
 static void shards_apply_h(const std::vector<Plan*>& G, double t, const std::vector<c2*>& in, const std::vector<c2*>& out) {
     const Plan& P0 = *G[0];
-    const PassGeom geo = shard_geometry(P0);
+    PassGeom geo;
+    bool tiled = false;
+    taylor_geometry(P0, geo, tiled);
     const int order = P0.desc.interp_order;
     const double om = eval_at(P0.tay.om, P0.times, t, order), th = eval_at(P0.tabs[0][0].det[0], P0.times, t, order);
     const bool cplx = P0.tay.phase_moves;
@@ -2875,21 +2944,14 @@ static void shards_apply_h(const std::vector<Plan*>& G, double t, const std::vec
         Plan& P = *G[r];
         CUDA_CHECK(cudaSetDevice(P.desc.device));
         taylor_table_unit(P, P.tay.unit, tables);
-        TaylorArgs a{};
+        TaylorArgs a = taylor_plan_args(P, geo, in[r], out[r], P.tay.unit);
         if (cplx) a.om0i = eval_at(P0.tay.om_im, P0.times, t, order);
-        a.v = in[r]; a.out = out[r];
-        a.dint = P.has_interaction ? P.dint.get() : nullptr;
-        a.D = P.D; a.geo = geo; a.unit = P.tay.unit;
-        a.table = P.tay.uniform ? nullptr : P.tay.d_tab.get();
-        a.tab_shapes = P.tay.tab_shapes;
         for (int s = 0; s < P.tay.ns; ++s) a.m0[s] = eval_at(P.tay.shape[s], P.times, t, order);
-        a.to_bit = P.desc.drives[0].state_to; a.from_is_one = P.desc.drives[0].state_from;
         a.th0 = th; a.om0 = om;
         a.scale = {1.0, 0.0};
         a.acc_mul = {1.0, 0.0};
-        a.shard_bits = P.shard_bits; a.shard = r;
         for (int q = 0; q < P.shard_bits; ++q) a.peer[q] = in[r ^ (1 << q)];
-        launch_taylor_shard(P, a, cplx);
+        launch_taylor_order(P, tiled, a, cplx);
     }
     CUDA_CHECK(cudaGetLastError());
     shards_sync(G);
@@ -3792,7 +3854,9 @@ int pb200_shards_propagate(pb200_plan** plans, int32_t count, double t_start, do
     if (t_start < tlo - eps || t_stop > thi + eps || t_stop < t_start)
         fail(PB200_ERR_INVALID, "pb200_shards_propagate: [%g, %g] outside sampling times [%g, %g]", t_start, t_stop, tlo, thi);
     t_start = std::max(t_start, tlo); t_stop = std::min(t_stop, thi);
-    const PassGeom geo = shard_geometry(P0);
+    PassGeom geo;
+    bool tiled = false;
+    taylor_geometry(P0, geo, tiled);
     // host half: the whole call, before any launch
     TaylorScheduler S(P0, t_start, t_stop, o);
     std::vector<TaylorStep> steps;
@@ -3810,62 +3874,15 @@ int pb200_shards_propagate(pb200_plan** plans, int32_t count, double t_start, do
                  need, (long long)(16 * P->D), (int)P->D, e.what());
         }
     }
-    ShardEvents order_ev(G, cudaEventDisableTiming), t0(G, cudaEventDefault), t1(G, cudaEventDefault);
-    for (int r = 0; r < count; ++r) {
-        CUDA_CHECK(cudaSetDevice(G[r]->desc.device));
-        CUDA_CHECK(cudaEventRecord(t0.ev[r], G[r]->stream));
-    }
-    // launching half.  Order k on shard r reads chi_k of its peers: it waits for the previous launch (order k - 1, or the
-    // last order of the previous step) of every peer, and every shard's waits for an order are enqueued before any
-    // shard records that order's event.  A slot a peer may still be gathering from is never overwritten: n_chi >= 2,
-    // and every order waits for the one before it.  The previous call ended with every stream synchronised.
-    const int sb = P0.shard_bits;
     long long launches = 0;
-    bool first = true;
-    std::vector<TaylorRing> R(count);
-    std::deque<std::vector<double>> tables;   // tables of rotated steps, until the call's last synchronisation
-    for (const TaylorStep& s : steps) {
-        for (int r = 0; r < count; ++r) {
-            R[r] = taylor_ring(*G[r], s);
-            CUDA_CHECK(cudaSetDevice(G[r]->desc.device));
-            taylor_table_unit(*G[r], s.drive == 1 ? s.unit : G[r]->tay.unit, tables);
-        }
-        for (int k = 0; k < s.K; ++k) {
-            for (int r = 0; r < count; ++r) {
-                Plan& P = *G[r];
-                CUDA_CHECK(cudaSetDevice(P.desc.device));
-                TaylorArgs a = taylor_args(P, geo, s, R[r], k);
-                a.shard_bits = sb; a.shard = r;
-                for (int q = 0; q < sb; ++q) {
-                    const int peer = r ^ (1 << q);
-                    a.peer[q] = R[peer].chi[k % s.n_chi];
-                    if (!first) CUDA_CHECK(cudaStreamWaitEvent(P.stream, order_ev.ev[peer], 0));
-                }
-                launch_taylor_shard(P, a, s.drive == 2);
-                ++launches;
-            }
-            for (int r = 0; r < count; ++r) {
-                CUDA_CHECK(cudaSetDevice(G[r]->desc.device));
-                CUDA_CHECK(cudaEventRecord(order_ev.ev[r], G[r]->stream));
-            }
-            first = false;
-        }
-        CUDA_CHECK(cudaGetLastError());
-        // the accumulator becomes the current state buffer
-        for (int r = 0; r < count; ++r) std::swap(G[r]->buf[G[r]->cur], *R[r].acc_slot);
-    }
-    float ms_max = 0.f;
-    for (int r = 0; r < count; ++r) {
-        CUDA_CHECK(cudaSetDevice(G[r]->desc.device));
-        CUDA_CHECK(cudaEventRecord(t1.ev[r], G[r]->stream));
-    }
-    for (int r = 0; r < count; ++r) {
-        CUDA_CHECK(cudaEventSynchronize(t1.ev[r]));
-        float ms = 0.f;
-        CUDA_CHECK(cudaEventElapsedTime(&ms, t0.ev[r], t1.ev[r]));
-        ms_max = std::max(ms_max, ms);
-    }
-    if (stats) *stats = S.finish(ms_max, launches);
+    size_t i = 0;
+    auto next = [&](TaylorStep& s) {
+        if (i == steps.size()) return false;
+        s = steps[i++];
+        return true;
+    };
+    const float ms = taylor_launch_steps(G, geo, tiled, next, launches);
+    if (stats) *stats = S.finish(ms, launches);
     PB200_CATCH
 }
 
