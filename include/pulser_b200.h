@@ -97,9 +97,19 @@ typedef struct pb200_run_opts {
                                  Richardson-CF4 Magnus steps; 3 time-dependent Taylor
                                  series (one global drive, its phase constant or
                                  moving, d = 2, one state: no Magnus error, ~1
-                                 H-apply per ns on C2);
+                                 H-apply per ns on C2; also the master equation
+                                 of a dissipator plan whose atoms share one
+                                 generator without single-bit flips -- dephasing,
+                                 relaxation, depolarizing -- under a drive of
+                                 constant phase, with the dissipator inside the
+                                 series and a default tol of 1e-10 instead of
+                                 the splitting path's 1e-6; anything else with
+                                 integrator 3 is PB200_ERR_UNSUPPORTED, reason
+                                 given);
                                  0 auto: 3 where it applies, else 2 for strongly
-                                 blockaded / HBM-resident registers, else 1 */
+                                 blockaded / HBM-resident registers, else 1.
+                                 1 / 2 on a dissipator plan: Strang splitting of
+                                 the dissipator around the Magnus steps */
 } pb200_run_opts;
 
 typedef struct pb200_run_stats {

@@ -821,6 +821,15 @@ struct TaylorArgs {
     double om0i;
     const c2* hg2[PB200_TAYLOR_PMAX];    // G'_{k-j}   (nullptr when omi_j = 0)
     double homi[PB200_TAYLOR_PMAX];
+    // master equation (stage kernels with DISS = true): the state is vec(rho) of n_pair atoms, s = (r << n_pair) | c,
+    // and (k+1) chi_{k+1} = h (-i H chi_k + D chi_k - i sum_j H_j chi_{k-j}): the dissipator D is static, so it acts on
+    // chi_k alone and never enters G_k.  Every atom carries the same 4 x 4 generator Gen on its (row bit, column bit)
+    // pair, with no entry that flips exactly one of the two bits:
+    //   diagonal   dw[0] + dw[1] popc(r) + dw[2] popc(c) + dw[3] popc(r & c)
+    //   both-flip  df[i] chi[s ^ pair bits], i = 2 row bit + column bit of s, df[i] = Gen[i][3 - i]
+    c2 dw[4], df[4];
+    int n_pair;        // 0: no dissipator
+    int diss_flip;     // 0: every df is zero (dephasing): no partner loads
 };
 
 // epilogue of one amplitude block: everything after the partner sums.  idx is the index inside the trajectory, voff
@@ -829,12 +838,13 @@ struct TaylorArgs {
 // r is either `off[r]` = sum_k c_k [digit_k == from] of the one shape (0 for uniform drives), or, with several shapes,
 // a functor off(r, J) = sum_s m_{s,J} sum_k c_{k,s} [digit_k == from] with the shapes' order-0 coefficients (J = 0)
 // or those of history term J - 1.
-// CPLX: (qx, qy) is G' of the complex-drive step.
-template <int R, int H = (R >= 4) ? R / 2 : R, bool SHARD = false, bool CPLX = false, class Off>
+// CPLX: (qx, qy) is G' of the complex-drive step.  DISS: (ex, ey) = i D chi_k, added to the sum that -i h / (k+1) scales.
+template <int R, int H = (R >= 4) ? R / 2 : R, bool SHARD = false, bool CPLX = false, bool DISS = false, class Off>
 __device__ __forceinline__ void taylor_epilogue(const TaylorArgs& a, const long long (&idx)[R], const c2 (&v)[R],
                                                 const double (&gx)[R], const double (&gy)[R], const Off& off,
                                                 long long voff, const double* __restrict__ dsrc,
-                                                const double* qx = nullptr, const double* qy = nullptr) {
+                                                const double* qx = nullptr, const double* qy = nullptr,
+                                                const double* ex = nullptr, const double* ey = nullptr) {
     constexpr bool SHAPES = !std::is_array<Off>::value;
     const int nb = a.geo.n_bits;
     const int ones_hi = SHARD ? __popc(a.shard) : 0;
@@ -855,6 +865,7 @@ __device__ __forceinline__ void taylor_epilogue(const TaylorArgs& a, const long 
                 sx[r] = fma(diag, v[h0 + r].x, a.om0 * gx[h0 + r]);
                 sy[r] = fma(diag, v[h0 + r].y, a.om0 * gy[h0 + r]);
                 if constexpr (CPLX) { sx[r] = fma(a.om0i, qx[h0 + r], sx[r]); sy[r] = fma(a.om0i, qy[h0 + r], sy[r]); }
+                if constexpr (DISS) { sx[r] += ex[h0 + r]; sy[r] += ey[h0 + r]; }
             }
         }
         for (int j = 0; j < a.nh; ++j) {
@@ -911,6 +922,24 @@ __device__ __forceinline__ void taylor_epilogue(const TaylorArgs& a, const long 
     }
 }
 
+// master equation (TaylorArgs::dw): the diagonal of the dissipator at s times chi_k[s]
+__device__ __forceinline__ c2 taylor_diss_diag(const TaylorArgs& a, long long s, c2 v) {
+    const unsigned long long c = (unsigned long long)s & ((1ULL << a.n_pair) - 1), r = (unsigned long long)s >> a.n_pair;
+    const double nr = (double)__popcll(r), nc = (double)__popcll(c), nrc = (double)__popcll(r & c);
+    const double wx = fma(a.dw[3].x, nrc, fma(a.dw[2].x, nc, fma(a.dw[1].x, nr, a.dw[0].x)));
+    const double wy = fma(a.dw[3].y, nrc, fma(a.dw[2].y, nc, fma(a.dw[1].y, nr, a.dw[0].y)));
+    return {wx * v.x - wy * v.y, wx * v.y + wy * v.x};
+}
+
+// master equation (TaylorArgs::df): (dx, dy) += the both-flip entry of the pair (row bit pr, column bit pc) at s times
+// the partner chi_k[s ^ 2^pr ^ 2^pc] = pv
+__device__ __forceinline__ void taylor_diss_flip(const TaylorArgs& a, long long s, int pr, int pc, double2 pv, double& dx,
+                                                 double& dy) {
+    const c2 f = a.df[(int)((((s >> pr) & 1) << 1) | ((s >> pc) & 1))];
+    dx = fma(f.x, pv.x, dx); dx = fma(-f.y, pv.y, dx);
+    dy = fma(f.x, pv.y, dy); dy = fma(f.y, pv.x, dy);
+}
+
 // UNIFORM: one drive coefficient for every qubit and a single state (C2, C5); otherwise per-(trajectory, qubit) static
 // factors from `table`, blockIdx.y = trajectory (C4: doppler + amplitude noise batches).
 // The tile is the TBITS low bits of the index (taylor_geometry), the bits above it are coalesced partner loads.  A thread
@@ -929,13 +958,20 @@ __device__ __forceinline__ void taylor_epilogue(const TaylorArgs& a, const long 
 // the signed sum P - Q of the same partner loads, i.e. G' as well as G.  The two sums of a chunk do not fit in 128
 // registers; these launches use fewer threads with more chunks each (kTaylorCplxRegBits) and one CTA's worth of
 // registers per SM.
-template <bool UNIFORM, bool REAL_G, int TBITS, int RB, bool SHARD = false, int NS = (UNIFORM ? 0 : 1), bool CPLX = false>
-__global__ void __launch_bounds__(1 << (TBITS - RB), CPLX ? 1 : (65536 / ((1 << (TBITS - RB)) * (RB >= 3 ? 128 : 64))))
+// DISS: the master equation on vec(rho) (TaylorArgs::dw, df; the batch gather, whose per-bit table carries the column
+// drive -conj(omega)).  The dissipator sum of a chunk is a second accumulator, which does not fit in 128 registers
+// either: the same launch shape as CPLX.  A pair whose row bit lies in the tile reads its both-flip partner from shared
+// memory, one above the tile costs one more coalesced load per atom.
+template <bool UNIFORM, bool REAL_G, int TBITS, int RB, bool SHARD = false, int NS = (UNIFORM ? 0 : 1), bool CPLX = false,
+          bool DISS = false>
+__global__ void __launch_bounds__(1 << (TBITS - RB),
+                                  (CPLX || DISS) ? 1 : (65536 / ((1 << (TBITS - RB)) * (RB >= 3 ? 128 : 64))))
 stage_d2_taylor_kernel(const __grid_constant__ TaylorArgs a) {
     static_assert(RB >= 3, "chunks of 8 amplitudes per thread");
     static_assert(UNIFORM || !SHARD, "shards carry one state with a uniform drive");
     static_assert(NS == (UNIFORM ? 0 : 1) || NS == PB200_TAYLOR_SMAX, "one-shape table, or PB200_TAYLOR_SMAX shapes");
     static_assert(!CPLX || !REAL_G, "a complex drive gathers through the per-bit table");
+    static_assert(!DISS || (!UNIFORM && !SHARD && !CPLX), "a density matrix runs the batch gather, one device, one phase");
     constexpr bool SHAPES = NS == PB200_TAYLOR_SMAX;
     constexpr int NT = 1 << (TBITS - RB);
     constexpr int TSIZE = 1 << TBITS;
@@ -1129,6 +1165,37 @@ stage_d2_taylor_kernel(const __grid_constant__ TaylorArgs a) {
             }
             off[r] = acc;
         }
+        double ex[RC], ey[RC];   // DISS: i D chi_k
+        if constexpr (DISS) {
+            double dx[RC], dy[RC];
+#pragma unroll
+            for (int r = 0; r < RC; ++r) {
+                const c2 w = taylor_diss_diag(a, idx[r], v[r]);
+                dx[r] = w.x; dy[r] = w.y;
+            }
+            if (a.diss_flip) {
+                const int tpos = tid + (c << STB);   // tile position of the chunk's first amplitude
+                for (int pc = 0; pc < a.n_pair; ++pc) {
+                    const int pr = pc + a.n_pair;
+                    const long long mask = (1LL << pr) | (1LL << pc);
+                    double2 pv[RC];
+                    if (pr < TBITS) {
+#pragma unroll
+                        for (int r = 0; r < RC; ++r) {
+                            const c2 t = tile[(tpos + r * NT) ^ (int)mask];
+                            pv[r] = make_double2(t.x, t.y);
+                        }
+                    } else {
+#pragma unroll
+                        for (int r = 0; r < RC; ++r) pv[r] = __ldg(reinterpret_cast<const double2*>(vsrc + (idx[r] ^ mask)));
+                    }
+#pragma unroll
+                    for (int r = 0; r < RC; ++r) taylor_diss_flip(a, idx[r], pr, pc, pv[r], dx[r], dy[r]);
+                }
+            }
+#pragma unroll
+            for (int r = 0; r < RC; ++r) { ex[r] = -dy[r]; ey[r] = dx[r]; }
+        }
         // per-qubit factors (off != 0) leave the registers for 2 amplitudes' operands at a time, not 4
         if constexpr (CPLX) {
             double qx[RC], qy[RC];   // G' = i (P - Q)
@@ -1145,17 +1212,20 @@ stage_d2_taylor_kernel(const __grid_constant__ TaylorArgs a) {
         } else if constexpr (SHAPES) {
             const double* lc = bl + c * RC;
             const double* lt = at + tid;
-            taylor_epilogue<RC, RC / 4, SHARD>(
-                a, idx, v, pr, pi, [&](int r, int J) { return lt[J * NT] + lc[(J << RB) + r]; }, voff, dsrc);
+            taylor_epilogue<RC, RC / 4, SHARD, false, DISS>(
+                a, idx, v, pr, pi, [&](int r, int J) { return lt[J * NT] + lc[(J << RB) + r]; }, voff, dsrc, nullptr,
+                nullptr, ex, ey);
         } else {
-            taylor_epilogue<RC, UNIFORM ? RC / 2 : RC / 4, SHARD>(a, idx, v, pr, pi, off, voff, dsrc);
+            taylor_epilogue<RC, UNIFORM ? RC / 2 : RC / 4, SHARD, false, DISS>(a, idx, v, pr, pi, off, voff, dsrc, nullptr,
+                                                                             nullptr, ex, ey);
         }
     }
 }
 
 // any register size (N < 13 in particular): one thread per amplitude, partners through global loads.  CPLX: the
-// complex-drive step, G' = i (P - Q) as well (stage_d2_taylor_kernel)
-template <bool CPLX = false>
+// complex-drive step, G' = i (P - Q) as well (stage_d2_taylor_kernel).  DISS: the master equation on vec(rho), the
+// both-flip partners through global loads too.
+template <bool CPLX = false, bool DISS = false>
 __global__ void __launch_bounds__(256) stage_d2_taylor_small_kernel(const __grid_constant__ TaylorArgs a) {
     const long long s = (long long)blockIdx.x * blockDim.x + threadIdx.x;
     if (s >= a.D) return;
@@ -1205,6 +1275,19 @@ __global__ void __launch_bounds__(256) stage_d2_taylor_small_kernel(const __grid
     const c2 v[1] = {{own.x, own.y}};
     const double gx[1] = {gxs}, gy[1] = {gys}, offv1[1] = {offv[0]};
     const double qx[1] = {q2x}, qy[1] = {q2y};
+    double ex[1] = {0.0}, ey[1] = {0.0};   // DISS: i D chi_k
+    if constexpr (DISS) {
+        const c2 w = taylor_diss_diag(a, s, v[0]);
+        double dx = w.x, dy = w.y;
+        if (a.diss_flip) {
+            for (int pc = 0; pc < a.n_pair; ++pc) {
+                const int pr = pc + a.n_pair;
+                const double2 pv = __ldg(reinterpret_cast<const double2*>(a.v + voff + (s ^ (1LL << pr) ^ (1LL << pc))));
+                taylor_diss_flip(a, s, pr, pc, pv, dx, dy);
+            }
+        }
+        ex[0] = -dy; ey[0] = dx;
+    }
     auto local = [&](int, int J) {
         double acc = 0.0;
 #pragma unroll
@@ -1212,8 +1295,8 @@ __global__ void __launch_bounds__(256) stage_d2_taylor_small_kernel(const __grid
         return acc;
     };
     const double* dsrc = a.dint ? a.dint + traj * a.dint_stride : nullptr;
-    if (a.tab_shapes) taylor_epilogue<1, 1, false, CPLX>(a, idx, v, gx, gy, local, voff, dsrc, qx, qy);
-    else taylor_epilogue<1, 1, false, CPLX>(a, idx, v, gx, gy, offv1, voff, dsrc, qx, qy);
+    if (a.tab_shapes) taylor_epilogue<1, 1, false, CPLX, DISS>(a, idx, v, gx, gy, local, voff, dsrc, qx, qy, ex, ey);
+    else taylor_epilogue<1, 1, false, CPLX, DISS>(a, idx, v, gx, gy, offv1, voff, dsrc, qx, qy, ex, ey);
 }
 
 // ---- generic-d stage kernel (any dim, several drives; global gathers) -------

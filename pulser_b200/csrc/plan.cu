@@ -227,6 +227,7 @@ struct TaylorVariant {
     int rb;
     TaylorSmem smem;
     bool pdl;
+    bool diss = false;   // master equation (TaylorArgs::n_pair > 0)
 };
 
 static const std::vector<TaylorVariant>& taylor_variants() {
@@ -254,6 +255,9 @@ static const std::vector<TaylorVariant>& taylor_variants() {
         {false, false, false, SM, true,  stage_d2_taylor_kernel<false, false, TB, RBC, false, SM, true>,  RBC, S::Shapes,    true},
         {true,  false, true,  0,  true,  stage_d2_taylor_kernel<true, false, TB, RBC, true, 0, true>,     RBC, S::TileTable, false},
         {true,  false, true,  SM, true,  stage_d2_taylor_kernel<true, false, TB, RBC, true, SM, true>,    RBC, S::Shapes,    false},
+        // master equation on vec(rho): the batch gather (the column drive is -conj(omega)), one or several shapes
+        {false, false, false, 1,  false, stage_d2_taylor_kernel<false, false, TB, RBC, false, 1, false, true>,  RBC, S::TileTable, true, true},
+        {false, false, false, SM, false, stage_d2_taylor_kernel<false, false, TB, RBC, false, SM, false, true>, RBC, S::Shapes,    true, true},
     };
     return v;
 }
@@ -336,6 +340,14 @@ struct Plan {
     bool use_krylov = false;
     long long kry_iters = 0;
     bool has_diss = false;
+    // the dissipator as the Taylor stage applies it (TaylorArgs::dw, df), when it qualifies (diss_taylor_analyse)
+    struct DissTaylor {
+        bool ok = false;
+        const char* why = "";
+        c2 dw[4] = {}, df[4] = {};
+        bool flip = false;        // some both-flip entry is non-zero
+        double norm = 0.0;        // bound on the 2-norm of the dissipator (max row / column sum)
+    } diss_tay;
     // Monte-Carlo wave function: single-qudit collapse operators (L^+L diagonal), thresholds, RNG
     std::vector<std::vector<cplx>> jump_ops;      // [n_ops][d*d]
     std::vector<std::vector<double>> jump_ldl;    // [n_ops][d]: diagonal of L^+L
@@ -1551,6 +1563,12 @@ static bool taylor_worthwhile(Plan& P, double gtol);
 static bool taylor_geometry(const Plan& P, PassGeom& geo, bool& tiled);
 static void propagate_taylor(Plan& P, double t_start, double t_stop, const pb200_run_opts* o, pb200_run_stats* stats);
 
+// error budget of a Taylor run: the caller's tol, else 1e-8 for states and 1e-10 for density matrices (no splitting
+// error to pay for: the master equation gets the same a-priori control as a pure state, at a tighter default)
+static double taylor_default_tol(const Plan& P, const pb200_run_opts* o) {
+    return (o && o->tol > 0.0) ? o->tol : (P.has_diss ? 1e-10 : 1e-8);
+}
+
 static void propagate(Plan& P, double t_start, double t_stop, const pb200_run_opts* o, pb200_run_stats* stats) {
     if (!P.state_set) fail(PB200_ERR_STATE, "pb200_propagate: no state set (call pb200_state_set first)");
     check_drives_set(P, "pb200_propagate");
@@ -1576,12 +1594,13 @@ static void propagate(Plan& P, double t_start, double t_stop, const pb200_run_op
             PassGeom geo;
             bool tiled = false;
             const bool ok = taylor_prepare(P) && taylor_geometry(P, geo, tiled) &&
-                            (req == 3 || taylor_worthwhile(P, (o && o->tol > 0.0) ? o->tol : 1e-8));
+                            (req == 3 || taylor_worthwhile(P, taylor_default_tol(P, o)));
             if (ok) { propagate_taylor(P, t_start, t_stop, o, stats); return; }
             if (env_int("PB200_TAYLOR_LOG", 0)) fprintf(stderr, "taylor not taken: %s\n", g_taylor_why);
             if (req == 3)
                 fail(PB200_ERR_UNSUPPORTED, "integrator 3 (Taylor) needs a d = 2 register whose drive rows are multiples of one row "
-                                            "(per-qubit static factors / detuning offsets allowed), no collapse operators / SLM mask: %s",
+                                            "(per-qubit static factors / detuning offsets allowed), no collapse operators / SLM mask, "
+                                            "and a dissipator of one generator without single-bit flips: %s",
                      g_taylor_why);
         }
     }
@@ -1897,6 +1916,7 @@ static void propagate(Plan& P, double t_start, double t_stop, const pb200_run_op
 // samples.  Least-squares factors with extended-precision sums (4001 same-sign terms: a plain double sum is only good
 // to ~1e-13, which is the size of the residual being tested).  Host only; also reachable through
 // pb200_host_taylor_separable (one shape) and pb200_host_taylor_shapes.
+static const char* const kWhyDriveRows = "a drive row is not a constant multiple of the reference row";
 struct SeparableFit {
     bool ok = false;
     const char* why = "";
@@ -1972,7 +1992,7 @@ static SeparableFit taylor_separable(int B, int N, int nt, CS cs, DS ds, int max
             }
             for (int i = 0; i < nt; ++i)
                 if (std::abs(cs(b, k, i) - aa * cs(F.ref_b, F.ref_k, i)) > 2e-13 * std::max(scale, 1e-300)) {
-                    F.why = "a drive row is not a constant multiple of the reference row";
+                    F.why = kWhyDriveRows;
                     return F;
                 }
             F.a[(size_t)b * N + k] = (ref2 > 0.0L) ? aa : cplx(0.0, 0.0);
@@ -2034,13 +2054,55 @@ static std::vector<double> taylor_table(const Plan& P, cplx unit) {
     return tab;
 }
 
+// Can the Taylor stage apply this dissipator (TaylorArgs::dw, df)?  d = 2, the same generator on every atom, and no entry
+// that flips exactly one bit of an atom's (row, column) pair: Gen = diagonal + "both bits flip" entries.  Pulser's
+// dephasing, relaxation and depolarizing channels qualify, as does any set of collapse operators each of which is
+// diagonal or off-diagonal; an operator that mixes the two does not.
+static Plan::DissTaylor diss_taylor_analyse(const std::vector<std::vector<cplx>>& gen, int dim) {
+    Plan::DissTaylor T;
+    if (dim != 2) { T.why = "a master equation of d = 3 levels: the Taylor propagator takes d = 2 only"; return T; }
+    const std::vector<cplx>& G = gen[0];
+    double scale = 0.0;
+    for (const std::vector<cplx>& g : gen)
+        for (const cplx& z : g) scale = std::max(scale, std::abs(z));
+    const double tiny = 1e-15 * scale;
+    for (const std::vector<cplx>& g : gen)
+        for (int i = 0; i < 16; ++i)
+            if (std::abs(g[i] - G[i]) > tiny) { T.why = "the atoms carry different dissipator generators"; return T; }
+    for (int i = 0; i < 4; ++i)
+        for (int j = 0; j < 4; ++j)
+            if (((i ^ j) == 1 || (i ^ j) == 2) && std::abs(G[i * 4 + j]) > tiny) {
+                T.why = "the dissipator has single-bit-flip entries (a collapse operator mixes diagonal and off-diagonal "
+                        "elements; each one diagonal or each one off-diagonal qualifies)";
+                return T;
+            }
+    auto c = [](cplx z) { return c2{z.real(), z.imag()}; };
+    const cplx g0 = G[0], g1 = G[5], g2 = G[10], g3 = G[15];   // pair value i = 2 row bit + column bit
+    T.dw[0] = c(g0 * (double)gen.size()); T.dw[1] = c(g2 - g0); T.dw[2] = c(g1 - g0); T.dw[3] = c(g0 - g1 - g2 + g3);
+    double row = 0.0, col = 0.0;
+    for (int i = 0; i < 4; ++i) {
+        T.df[i] = c(G[i * 4 + (3 - i)]);
+        T.flip = T.flip || G[i * 4 + (3 - i)] != 0.0;
+        row = std::max(row, std::abs(G[i * 5]) + std::abs(G[i * 4 + (3 - i)]));
+        col = std::max(col, std::abs(G[i * 5]) + std::abs(G[(3 - i) * 4 + i]));
+    }
+    // ||Gen||_2 <= sqrt(||Gen||_1 ||Gen||_inf), one per atom
+    T.norm = (double)gen.size() * std::max(row, col);
+    T.ok = true;
+    return T;
+}
+
+static const char* const kWhyMovingPhaseRho =
+    "the drive phase moves: on a density matrix the column drive -conj(omega(t)) is not a multiple of omega(t)";
+
 // the drive relative to the phase of its largest sample (real and imaginary parts), per-(trajectory, qubit) static
 // factors, device table
 static bool taylor_prepare(Plan& P) {
     Plan::TaylorCache& C = P.tay;
-    g_taylor_why = "structure (d, drives, collapse / dissipator / mask, interpolation order)";
+    g_taylor_why = "structure (d, drives, collapse / mask, interpolation order)";
+    if (P.has_diss && !P.diss_tay.ok) { g_taylor_why = P.diss_tay.why; return false; }
     if (!is_d2path(P)) return false;
-    if (P.has_diss || P.has_collapse || P.has_slm) return false;
+    if (P.has_collapse || P.has_slm) return false;
     if (P.desc.interp_order != 3 && P.desc.interp_order != 1) return false;
     if (C.valid) { g_taylor_why = C.ok ? "" : C.why; return C.ok; }
     C.valid = true; C.ok = false;
@@ -2059,7 +2121,10 @@ static bool taylor_prepare(Plan& P) {
         [&](int b, int k, int i) { const PiecewiseCubic<cplx>* pc = crow[(size_t)b * N + k]; return i < npc ? pc->c0[i] : pc->y_last; },
         [&](int b, int k, int i) { const PiecewiseCubic<double>* pc = drow[(size_t)b * N + k]; return i < npc ? pc->c0[i] : pc->y_last; },
         PB200_TAYLOR_SMAX);
-    if (!F.ok) { g_taylor_why = C.why = F.why; return false; }
+    if (!F.ok) {
+        g_taylor_why = C.why = (P.has_diss && F.why == kWhyDriveRows) ? kWhyMovingPhaseRho : F.why;
+        return false;
+    }
     const double scale = F.scale;
     const cplx unit = scale > 0.0 ? F.big / scale : cplx(1.0, 0.0);
     const cplx cu = std::conj(unit);
@@ -2081,10 +2146,11 @@ static bool taylor_prepare(Plan& P) {
     C.om.y_last = (ref.y_last * cu).real();
     C.om_im.y_last = (ref.y_last * cu).imag();
     if (!C.phase_moves) C.om_im = PiecewiseCubic<double>();   // constant phase: the real drive of before, exactly
+    else if (P.has_diss) { g_taylor_why = C.why = kWhyMovingPhaseRho; return false; }
     C.unit = {unit.real(), unit.imag()};
     C.a = F.a; C.c = F.c; C.ns = F.ns;
     for (int s = 0; s < C.ns; ++s) C.shape[s] = make_interpolant<double>(P.times.data(), F.m[s].data(), nt, P.desc.interp_order);
-    C.drive_uniform = B == 1;
+    C.drive_uniform = B == 1 && !P.has_diss;   // vec(rho) always runs the batch gather (stage kernels with DISS)
     C.a_sum_max = 0.0;
     for (int s = 0; s < PB200_TAYLOR_SMAX; ++s) C.c_sum_max[s] = 0.0;
     for (int b = 0; b < B; ++b) {
@@ -2189,7 +2255,7 @@ static void taylor_knot_widths(Plan& P) {
         double om = eval_at(C.om, P.times, P.times[i], order);
         if (C.phase_moves) om = std::hypot(om, eval_at(C.om_im, P.times, P.times[i], order));
         taylor_bounds(P, om, eval_at(th_pc, P.times, P.times[i], order), mv, c, hw);
-        C.w_knot[i] = hw;
+        C.w_knot[i] = hw + P.diss_tay.norm;   // a master equation: + the bound of its dissipator (0 otherwise)
     }
 }
 
@@ -2219,6 +2285,9 @@ static bool taylor_worthwhile(Plan& P, double gtol) {
     int cnt = 0;
     for (char c : rough) cnt += c;
     if (4 * cnt > nt) { g_taylor_why = "splines too rough for multi-interval polynomial steps"; return false; }
+    // (iii) a master equation: the alternative is the splitting path, not Krylov; measured faster at every size it runs
+    // (experiments/lindblad_cost.py, DESIGN.md section 3a)
+    if (P.has_diss) return true;
     taylor_knot_widths(P);
     double wsum = 0.0;
     for (int i = 0; i + 1 < nt; ++i) wsum += 0.5 * (P.tay.w_knot[i] + P.tay.w_knot[i + 1]) * (P.times[i + 1] - P.times[i]);
@@ -2311,9 +2380,12 @@ static int taylor_order(double h, const std::vector<double>& mj, double tol, dou
 // One order of a Taylor step: the tiled variant that the plan and the arguments select, or the plain kernel of small
 // registers (!tiled).  cplx: a step whose drive phase moves inside it
 static void launch_taylor_order(const Plan& P, bool tiled, const TaylorArgs& a, bool cplx) {
+    const bool diss = a.n_pair > 0;
     if (!tiled) {
         const dim3 grid((unsigned)((P.D + 255) / 256), (unsigned)P.B);
-        if (cplx) stage_d2_taylor_small_kernel<true><<<grid, 256, 0, P.stream>>>(a);
+        if (diss && !cplx) stage_d2_taylor_small_kernel<false, true><<<grid, 256, 0, P.stream>>>(a);
+        else if (diss) fail(PB200_ERR_UNSUPPORTED, "no Taylor stage kernel for a dissipator with a complex drive");
+        else if (cplx) stage_d2_taylor_small_kernel<true><<<grid, 256, 0, P.stream>>>(a);
         else stage_d2_taylor_small_kernel<false><<<grid, 256, 0, P.stream>>>(a);
         return;
     }
@@ -2323,7 +2395,9 @@ static void launch_taylor_order(const Plan& P, bool tiled, const TaylorArgs& a, 
     const bool shard = a.shard_bits > 0;
     const int ns = a.tab_shapes ? PB200_TAYLOR_SMAX : uniform ? 0 : 1;
     for (const TaylorVariant& v : taylor_variants()) {
-        if (v.uniform != uniform || v.real_g != real_g || v.shard != shard || v.ns != ns || v.cplx != cplx) continue;
+        if (v.uniform != uniform || v.real_g != real_g || v.shard != shard || v.ns != ns || v.cplx != cplx ||
+            v.diss != diss)
+            continue;
         const size_t tile = (size_t)16 << kTaylorTileBits;
         const size_t smem = v.smem == TaylorSmem::Shapes      ? taylor_shapes_smem(P.n)
                             : v.smem == TaylorSmem::TileTable ? tile + (size_t)d2_table_stride(P.n) * 8
@@ -2332,8 +2406,8 @@ static void launch_taylor_order(const Plan& P, bool tiled, const TaylorArgs& a, 
                  dim3(1u << (kTaylorTileBits - v.rb)), smem, P.stream, v.pdl, a);
         return;
     }
-    fail(PB200_ERR_UNSUPPORTED, "no Taylor stage kernel for UNIFORM=%d REAL_G=%d SHARD=%d NS=%d CPLX=%d", uniform, real_g,
-         shard, ns, cplx);
+    fail(PB200_ERR_UNSUPPORTED, "no Taylor stage kernel for UNIFORM=%d REAL_G=%d SHARD=%d NS=%d CPLX=%d DISS=%d", uniform,
+         real_g, shard, ns, cplx, diss);
 }
 
 // Geometry of the Taylor stage on the 2^L amplitudes a plan holds (L = N, or N - shard_bits on a shard): the
@@ -2384,7 +2458,7 @@ struct TaylorScheduler {
 
     TaylorScheduler(Plan& P_, double t_start, double t_stop_, const pb200_run_opts* o) : P(P_), t_stop(t_stop_), t(t_start) {
         const double tlo = P.times.front(), thi = P.times.back();
-        gtol = (o && o->tol > 0.0) ? o->tol : 1e-8;
+        gtol = taylor_default_tol(P, o);
         rate = gtol / std::max(thi - tlo, 1e-30);       // error budget per unit of time
         constexpr double kTaylorRhoMax = 14.0;
         order = P.desc.interp_order;
@@ -2563,7 +2637,8 @@ struct TaylorScheduler {
         double c0, hw0, mv[PB200_TAYLOR_SMAX];
         for (int q = 0; q < PB200_TAYLOR_SMAX; ++q) mv[q] = m_c(q, 0);
         taylor_bounds(P, cplx ? om_abs(0) : F.om.c[0], F.th.c[0], mv, c0, hw0);
-        gam[0] = c0; mj[0] = hw0;
+        // the dissipator is static and not centred: its bound joins m_0 (0 without one)
+        gam[0] = c0; mj[0] = hw0 + P.diss_tay.norm;
         for (int j = 1; j <= p; ++j) {
             const double thj = th_c(j), omj = j <= p_om ? om_abs(j) : 0.0;
             gam[j] = -thj * 0.5 * N;
@@ -2696,6 +2771,11 @@ static TaylorArgs taylor_plan_args(const Plan& P, const PassGeom& geo, const c2*
     a.tab_shapes = P.tay.tab_shapes;
     a.to_bit = P.desc.drives[0].state_to; a.from_is_one = P.desc.drives[0].state_from;
     a.shard_bits = P.shard_bits; a.shard = P.shard;
+    if (P.has_diss) {
+        for (int i = 0; i < 4; ++i) { a.dw[i] = P.diss_tay.dw[i]; a.df[i] = P.diss_tay.df[i]; }
+        a.n_pair = P.n / 2;
+        a.diss_flip = P.diss_tay.flip ? 1 : 0;
+    }
     return a;
 }
 
@@ -3415,6 +3495,7 @@ int pb200_plan_set_dissipator(pb200_plan* h, int32_t n_pairs, const double* gene
     if (!h || !generators) fail(PB200_ERR_INVALID, "null argument");
     Plan& P = h->p;
     if (P.dim > 3) fail(PB200_ERR_UNSUPPORTED, "dissipator: d <= 3 only");
+    if (P.shard_bits) fail(PB200_ERR_UNSUPPORTED, "dissipator: not on state-vector shards");
     if (n_pairs < 1 || 2 * n_pairs != P.n) fail(PB200_ERR_INVALID, "dissipator: the plan must hold 2*n_pairs qudits");
     const int dd = P.dim * P.dim;
     P.diss_gen.assign(n_pairs, std::vector<cplx>((size_t)dd * dd));
@@ -3426,6 +3507,8 @@ int pb200_plan_set_dissipator(pb200_plan* h, int32_t n_pairs, const double* gene
             P.diss_gen[k][i] = z;
         }
     P.has_diss = true;
+    P.diss_tay = diss_taylor_analyse(P.diss_gen, P.dim);
+    P.tay.valid = false;
     PB200_CATCH
 }
 

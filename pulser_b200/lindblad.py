@@ -13,8 +13,13 @@ column qudits; in XY mode the real symmetric exchange couplings become ``-U^xy``
 there as well), so the unitary part reuses the Schroedinger kernels unchanged;
 the dissipator of single-qudit collapse operators factorises into one
 ``d^2 x d^2`` matrix per (row digit, column digit) pair (``pair_op_kernel``).
-The two are combined by symmetric splitting + Richardson extrapolation inside
-``pb200_propagate`` (see include/pulser_b200.h).
+Where every atom's generator is the same and has no entry that flips exactly
+one bit of the (row, column) pair -- dephasing, relaxation, depolarizing, any
+set of collapse operators each diagonal or off-diagonal -- and the drive keeps
+one phase, ``pb200_propagate`` runs the time-dependent Taylor propagator with
+the dissipator inside the series (no splitting error; default tolerance 1e-10).
+Otherwise, or with ``integrator=1 / 2``, the two are combined by symmetric
+splitting + Richardson extrapolation (see include/pulser_b200.h).
 """
 from __future__ import annotations
 

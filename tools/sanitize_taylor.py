@@ -21,3 +21,13 @@ with engine.DevicePlan(specs) as plan:
     plan.set_state("all-ground")
     st = plan.propagate(0.0, base.sampling_times[-1])
     print("batch n", n, "integrator", st["integrator"], "launches", st["n_launches"], "norm2", plan.norm2())
+# master equation (DISS kernels): N = 3 (small kernel, 2N = 6) and N = 7 (tiled, both-flip partners in and above the tile)
+from pulser_b200.lindblad import LindbladPlan
+ops = np.array([np.diag([np.sqrt(0.1), 0.0]), [[0.0, 0.0], [0.3, 0.0]]], dtype=complex)
+for n in (3, 7):
+    spec = W.ising_global_spec(W.disc_register(n, 16.0, 5.0, 3), W.C6_LEVEL_60, amp, det)
+    spec.collapse_ops = ops
+    with LindbladPlan(spec) as lp:
+        lp.set_state(np.eye(1, 2**n, 2**n - 1)[0])
+        st = lp.propagate(0.0, spec.sampling_times[-1], integrator=3)
+        print("lindblad n", n, "launches", st["n_launches"], "trace", np.trace(lp.get_rho()[0]).real)
