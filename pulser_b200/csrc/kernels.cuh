@@ -785,8 +785,14 @@ struct TaylorArgs {
     c2* out;           // chi_{k+1}
     c2* g_out;         // G_k = X chi_k (nullptr: nobody reads it later)
     c2* acc;           // accumulator of sum_k chi_k
-    const double* dint;  // nullptr: no interaction
+    const double* dint;  // Dint of the small kernel (nullptr: no interaction)
     long long dint_stride;  // 0: Dint shared by the trajectories
+    // couplings of the tiled stage, which forms Dint itself (taylor_dint_setup): the symmetric N x N matrix U of
+    // dint_kernel (atom i at bit position N - 1 - i, zero diagonal, bad atoms zeroed); nullptr: no interaction.  A pair
+    // counts where both bits equal ryd_bit (the Rydberg digit)
+    const double* cpl;
+    long long cpl_stride;   // 0: shared by the trajectories, else N * N
+    int ryd_bit;
     long long D;
     PassGeom geo;
     c2 unit;           // uniform drive: e^{-i phi}, the drive's phase on the step (TaylorStep::unit)
@@ -806,7 +812,8 @@ struct TaylorArgs {
     double hth[PB200_TAYLOR_PMAX], hgam[PB200_TAYLOR_PMAX], hom[PB200_TAYLOR_PMAX];
     double hm[PB200_TAYLOR_SMAX][PB200_TAYLOR_PMAX];   // hm[s][j]: shape s, history j
     int acc_read;      // 1: acc is read before it is updated (0: first write of the step)
-    int acc_add_v;     // 1: chi_k joins the update (even orders), 0: chi_{k+1} alone
+    int acc_add_v;     // 1: chi_k joins the update, 0: chi_{k+1} alone
+    int acc_add_h;     // 1: chi_{k-1} (history term hchi[0]) joins the update as well
     int acc_on;        // 0: this order leaves the accumulator alone
     c2 acc_mul;        // factor of the whole accumulator (phase of the scalar centre on the last order, else 1)
     // state-vector shards (stage_d2_taylor_kernel<..., SHARD = true>): the top shard_bits qubits of the global index
@@ -838,11 +845,14 @@ struct TaylorArgs {
 // r is either `off[r]` = sum_k c_k [digit_k == from] of the one shape (0 for uniform drives), or, with several shapes,
 // a functor off(r, J) = sum_s m_{s,J} sum_k c_{k,s} [digit_k == from] with the shapes' order-0 coefficients (J = 0)
 // or those of history term J - 1.
+// dint(r) is the interaction diagonal of amplitude r.  v is consumed: with acc_add_h, chi_{k-1} is added into it once the
+// diagonal term no longer needs it, so the accumulator update reads no extra operand.
 // CPLX: (qx, qy) is G' of the complex-drive step.  DISS: (ex, ey) = i D chi_k, added to the sum that -i h / (k+1) scales.
-template <int R, int H = (R >= 4) ? R / 2 : R, bool SHARD = false, bool CPLX = false, bool DISS = false, class Off>
-__device__ __forceinline__ void taylor_epilogue(const TaylorArgs& a, const long long (&idx)[R], const c2 (&v)[R],
+template <int R, int H = (R >= 4) ? R / 2 : R, bool SHARD = false, bool CPLX = false, bool DISS = false, class Off,
+          class Dint>
+__device__ __forceinline__ void taylor_epilogue(const TaylorArgs& a, const long long (&idx)[R], c2 (&v)[R],
                                                 const double (&gx)[R], const double (&gy)[R], const Off& off,
-                                                long long voff, const double* __restrict__ dsrc,
+                                                long long voff, const Dint& dint,
                                                 const double* qx = nullptr, const double* qy = nullptr,
                                                 const double* ex = nullptr, const double* ey = nullptr) {
     constexpr bool SHAPES = !std::is_array<Off>::value;
@@ -854,7 +864,7 @@ __device__ __forceinline__ void taylor_epilogue(const TaylorArgs& a, const long 
         {
             double dv[H];
 #pragma unroll
-            for (int r = 0; r < H; ++r) dv[r] = dsrc ? __ldcs(dsrc + idx[h0 + r]) : 0.0;
+            for (int r = 0; r < H; ++r) dv[r] = dint(h0 + r);
 #pragma unroll
             for (int r = 0; r < H; ++r) {
                 const int ones = __popcll((unsigned long long)idx[h0 + r]) + ones_hi;
@@ -879,6 +889,7 @@ __device__ __forceinline__ void taylor_epilogue(const TaylorArgs& a, const long 
                     if constexpr (SHAPES) d = -fma(a.hth[j], cn[r], a.hgam[j] + off(h0 + r, j + 1));
                     else d = -fma(a.hth[j], cn[r], fma(a.hm[0][j], off[h0 + r], a.hgam[j]));
                     sx[r] = fma(d, c[r].x, sx[r]); sy[r] = fma(d, c[r].y, sy[r]);
+                    if (j == 0 && a.acc_add_h) v[h0 + r] = cadd(v[h0 + r], c[r]);
                 }
             }
             if (a.hg[j]) {
@@ -940,6 +951,89 @@ __device__ __forceinline__ void taylor_diss_flip(const TaylorArgs& a, long long 
     dy = fma(f.x, pv.y, dy); dy = fma(f.y, pv.x, dy);
 }
 
+// ---- interaction diagonal inside the tiled Taylor stage ------------------------------------------------------------
+// Dint[s] = sum_{p<q} W_pq [bit p = ryd_bit][bit q = ryd_bit], W_pq = U of the atoms at bit positions p and q
+// (TaylorArgs::cpl), factorised along the stage's index
+// layout idx = base + tid + m NT (m = c RC + r, RB register bits above the TBITS - RB bits of tid): the bits above the
+// tile are fixed per CTA, those of tid per thread, so that
+//     Dint = xt[0][tid] + ts[m] + sum_{q : bit q of m = 1} xt[1 + q][tid]
+//   ts[m]     = sum over the register bits set in m of (their pairs + their couplings to the set bits above the tile)
+//   xt[0]     = the pair sum of the set bits above the tile and in tid   (+ sum_q y_q when ryd_bit = 0)
+//   xt[1 + q] = y_q = the couplings of register bit q to the set bits of tid   (negated when ryd_bit = 0: "set" is
+//               then bit q = 0, and sum_{q : bit = 0} y_q = sum_q y_q - sum_{q : bit = 1} y_q)
+// Shared memory, in doubles: wt[TBITS^2] couplings among the tile bits, wj[TBITS] couplings of each tile bit to the set
+// bits above the tile, hh their pair sum, ts[2^RB], xt[RB + 1][NT], then a copy of the N x N matrix.
+__host__ __device__ constexpr int taylor_dint_doubles(int tbits, int rb) {
+    return tbits * tbits + tbits + 1 + (1 << rb) + (rb + 1) * (1 << (tbits - rb));
+}
+
+// fills the shared-memory factors above; ends with this thread's xt written (read back by this thread only).  hi: the
+// global index bits above the tile of this CTA (a shard's index included).  Contains __syncthreads.
+template <int TBITS, int RB>
+__device__ __forceinline__ void taylor_dint_setup(const TaylorArgs& a, long long traj, unsigned long long hi, int tid,
+                                                  double* dsm) {
+    constexpr int NT = 1 << (TBITS - RB), L0 = TBITS - RB;
+    const int nb = a.geo.n_bits;
+    double* Ws = dsm + taylor_dint_doubles(TBITS, RB);   // the whole matrix, one coalesced pass
+    const double* Wq = a.cpl + traj * a.cpl_stride;
+    for (int i = tid; i < nb * nb; i += NT) Ws[i] = __ldg(Wq + i);
+    __syncthreads();
+    auto W = [&](int p, int q) { return Ws[(nb - 1 - p) * nb + (nb - 1 - q)]; };   // atom nb - 1 - p at bit p
+    const unsigned long long flip = a.ryd_bit ? 0ULL : ~0ULL;
+    const unsigned long long nmask = nb >= 64 ? ~0ULL : (1ULL << nb) - 1;
+    const unsigned long long hs = (hi ^ flip) & nmask & ~((1ULL << TBITS) - 1);   // set bits above the tile
+    double* wt = dsm;
+    double* wj = wt + TBITS * TBITS;
+    double* hh = wj + TBITS;
+    double* ts = hh + 1;
+    double* xt = ts + (1 << RB);
+    for (int i = tid; i < TBITS * TBITS; i += NT) wt[i] = W(i / TBITS, i % TBITS);
+    if (tid < TBITS) {
+        double s = 0.0;
+        for (unsigned long long m = hs; m; m &= m - 1) s += W(__ffsll((long long)m) - 1, tid);
+        wj[tid] = s;
+    } else if (tid >= 32 && tid < 32 + (1 << RB)) {
+        const int m = tid - 32;
+        const unsigned ms = ((unsigned)m ^ (unsigned)flip) & ((1u << RB) - 1);
+        double s = 0.0;
+        for (int q = 0; q < RB; ++q) {
+            if (!((ms >> q) & 1)) continue;
+            for (unsigned long long h = hs; h; h &= h - 1) s += W(L0 + q, __ffsll((long long)h) - 1);
+            for (int q2 = q + 1; q2 < RB; ++q2) if ((ms >> q2) & 1) s += W(L0 + q, L0 + q2);
+        }
+        ts[m] = s;
+    } else if (tid >= 64 && tid < 96) {
+        double s = 0.0;
+        for (int p = TBITS + (tid - 64); p < nb; p += 32) {
+            if (!((hs >> p) & 1)) continue;
+            for (unsigned long long h = hs & ~((2ULL << p) - 1); h; h &= h - 1) s += W(p, __ffsll((long long)h) - 1);
+        }
+#pragma unroll
+        for (int o = 16; o; o >>= 1) s += __shfl_xor_sync(0xffffffffu, s, o);
+        if (tid == 64) hh[0] = s;
+    }
+    __syncthreads();
+    const unsigned tb = ((unsigned)tid ^ (unsigned)flip) & (NT - 1);   // set bits of tid
+    double ct = hh[0];
+    double y[RB];
+#pragma unroll
+    for (int q = 0; q < RB; ++q) y[q] = 0.0;
+#pragma unroll 1
+    for (int i = 0; i < L0; ++i) {
+        const bool bi = (tb >> i) & 1;
+        ct += bi ? wj[i] : 0.0;
+        for (int j = i + 1; j < L0; ++j) ct += (bi && ((tb >> j) & 1)) ? wt[i * TBITS + j] : 0.0;
+#pragma unroll
+        for (int q = 0; q < RB; ++q) y[q] += bi ? wt[i * TBITS + L0 + q] : 0.0;
+    }
+#pragma unroll
+    for (int q = 0; q < RB; ++q) {
+        if (!a.ryd_bit) { ct += y[q]; y[q] = -y[q]; }
+        xt[(q + 1) * NT + tid] = y[q];
+    }
+    xt[tid] = ct;
+}
+
 // UNIFORM: one drive coefficient for every qubit and a single state (C2, C5); otherwise per-(trajectory, qubit) static
 // factors from `table`, blockIdx.y = trajectory (C4: doppler + amplitude noise batches).
 // The tile is the TBITS low bits of the index (taylor_geometry), the bits above it are coalesced partner loads.  A thread
@@ -994,13 +1088,22 @@ stage_d2_taylor_kernel(const __grid_constant__ TaylorArgs a) {
 
     if (tid == 0) mbar_init(&mbar, 1);
     __syncthreads();
+    double* dsm = reinterpret_cast<double*>(tile + TSIZE);   // taylor_dint_setup
+    const double* ts = dsm + TBITS * TBITS + TBITS + 1;
+    const double* xt = ts + (1 << RB);
+    double* tab = dsm + taylor_dint_doubles(TBITS, RB) + g.n_bits * g.n_bits;
+    // the interaction's factors depend on the plan alone: formed before the wait on the previous order, so that they
+    // overlap its tail (behind the first chunk's partner loads, the setup's registers would spill)
+    if (a.cpl)
+        taylor_dint_setup<TBITS, RB>(
+            a, traj, (unsigned long long)base | (SHARD ? (unsigned long long)a.shard << (g.n_bits - a.shard_bits) : 0ULL),
+            tid, dsm);
     pdl_wait();
     pdl_launch_dependents();
     if (tid == 0) {
         mbar_arrive_expect_tx(&mbar, (uint32_t)TSIZE * 16u);
         tma_load_1d(tile, vsrc + base, (uint32_t)TSIZE * 16u, &mbar);
     }
-    double* tab = reinterpret_cast<double*>(tile + TSIZE);
     // SHAPES, for J = 0 (order-0 coefficients m0) and J = 1 + history j (hm[s][j]) up to nh, behind the per-bit table:
     //   bl[J][i]   = sum_s m_{s,J} x (shape s's weights of the register bits i, relative to i = 0), the same for all
     //   at[J][tid] = sum_s m_{s,J} x (shape s's weights of the bits of base + tid, shard bits included)
@@ -1063,7 +1166,6 @@ stage_d2_taylor_kernel(const __grid_constant__ TaylorArgs a) {
             at[J * NT + tid] = acc;   // read by this thread only
         }
     }
-    const double* dsrc = a.dint ? a.dint + traj * a.dint_stride : nullptr;
 #pragma unroll 1
     for (int c = 0; c < (1 << CB); ++c) {
         const long long i0 = base + tid + c * RC * NT;   // index of the chunk's first amplitude; the r-th is i0 + r*NT
@@ -1121,6 +1223,15 @@ stage_d2_taylor_kernel(const __grid_constant__ TaylorArgs a) {
             }
         }
         if (c == 0) mbar_wait(&mbar, 0);
+        auto dint = [&](int r) {
+            if (!a.cpl) return 0.0;
+            const int m = c * RC + r;
+            double d = ts[m] + xt[tid];
+#pragma unroll
+            for (int q = 0; q < RB; ++q)
+                if ((m >> q) & 1) d += xt[(q + 1) * NT + tid];
+            return d;
+        };
         const c2* sub = tile + (c << STB);
         c2 v[RC];
         double qd[RC];   // the Q sums of rb_tile_gather: not used by the two instantiations below
@@ -1205,18 +1316,18 @@ stage_d2_taylor_kernel(const __grid_constant__ TaylorArgs a) {
                 const double* lc = bl + c * RC;
                 const double* lt = at + tid;
                 taylor_epilogue<RC, RC / 4, SHARD, true>(
-                    a, idx, v, pr, pi, [&](int r, int J) { return lt[J * NT] + lc[(J << RB) + r]; }, voff, dsrc, qx, qy);
+                    a, idx, v, pr, pi, [&](int r, int J) { return lt[J * NT] + lc[(J << RB) + r]; }, voff, dint, qx, qy);
             } else {
-                taylor_epilogue<RC, RC / 4, SHARD, true>(a, idx, v, pr, pi, off, voff, dsrc, qx, qy);
+                taylor_epilogue<RC, RC / 4, SHARD, true>(a, idx, v, pr, pi, off, voff, dint, qx, qy);
             }
         } else if constexpr (SHAPES) {
             const double* lc = bl + c * RC;
             const double* lt = at + tid;
             taylor_epilogue<RC, RC / 4, SHARD, false, DISS>(
-                a, idx, v, pr, pi, [&](int r, int J) { return lt[J * NT] + lc[(J << RB) + r]; }, voff, dsrc, nullptr,
+                a, idx, v, pr, pi, [&](int r, int J) { return lt[J * NT] + lc[(J << RB) + r]; }, voff, dint, nullptr,
                 nullptr, ex, ey);
         } else {
-            taylor_epilogue<RC, UNIFORM ? RC / 2 : RC / 4, SHARD, false, DISS>(a, idx, v, pr, pi, off, voff, dsrc, nullptr,
+            taylor_epilogue<RC, UNIFORM ? RC / 2 : RC / 4, SHARD, false, DISS>(a, idx, v, pr, pi, off, voff, dint, nullptr,
                                                                              nullptr, ex, ey);
         }
     }
@@ -1272,7 +1383,7 @@ __global__ void __launch_bounds__(256) stage_d2_taylor_small_kernel(const __grid
     }
     const long long idx[1] = {s};
     const double2 own = __ldg(reinterpret_cast<const double2*>(a.v + voff + s));
-    const c2 v[1] = {{own.x, own.y}};
+    c2 v[1] = {{own.x, own.y}};
     const double gx[1] = {gxs}, gy[1] = {gys}, offv1[1] = {offv[0]};
     const double qx[1] = {q2x}, qy[1] = {q2y};
     double ex[1] = {0.0}, ey[1] = {0.0};   // DISS: i D chi_k
@@ -1295,8 +1406,9 @@ __global__ void __launch_bounds__(256) stage_d2_taylor_small_kernel(const __grid
         return acc;
     };
     const double* dsrc = a.dint ? a.dint + traj * a.dint_stride : nullptr;
-    if (a.tab_shapes) taylor_epilogue<1, 1, false, CPLX, DISS>(a, idx, v, gx, gy, local, voff, dsrc, qx, qy, ex, ey);
-    else taylor_epilogue<1, 1, false, CPLX, DISS>(a, idx, v, gx, gy, offv1, voff, dsrc, qx, qy, ex, ey);
+    auto dint = [&](int) { return dsrc ? __ldcs(dsrc + s) : 0.0; };
+    if (a.tab_shapes) taylor_epilogue<1, 1, false, CPLX, DISS>(a, idx, v, gx, gy, local, voff, dint, qx, qy, ex, ey);
+    else taylor_epilogue<1, 1, false, CPLX, DISS>(a, idx, v, gx, gy, offv1, voff, dint, qx, qy, ex, ey);
 }
 
 // ---- generic-d stage kernel (any dim, several drives; global gathers) -------

@@ -262,6 +262,16 @@ static const std::vector<TaylorVariant>& taylor_variants() {
     return v;
 }
 
+// dynamic shared memory of a variant on N qubits: the tile, the interaction's factors and couplings (taylor_dint_setup), then the
+// per-bit table or the shapes' sums
+static size_t taylor_variant_smem(const TaylorVariant& v, int n) {
+    const size_t tile = (size_t)16 << kTaylorTileBits;
+    const size_t rest = v.smem == TaylorSmem::Shapes      ? taylor_shapes_smem(n) - tile
+                        : v.smem == TaylorSmem::TileTable ? (size_t)d2_table_stride(n) * 8
+                                                          : 0;
+    return tile + (size_t)(taylor_dint_doubles(kTaylorTileBits, v.rb) + n * n) * 8 + rest;
+}
+
 // once per device and process: SM count, > 48 KB of dynamic shared memory for the tile kernels
 static int device_setup(int dev) {
     static std::mutex mu;
@@ -278,11 +288,9 @@ static int device_setup(int dev) {
     CUDA_CHECK(cudaFuncSetAttribute(stage_d2_rb_kernel<true, true, TB, RB>, cudaFuncAttributeMaxDynamicSharedMemorySize, max_smem));
     CUDA_CHECK(cudaFuncSetAttribute(stage_d2_rb_kernel<true, false, TB, RB>, cudaFuncAttributeMaxDynamicSharedMemorySize, max_smem));
     CUDA_CHECK(cudaFuncSetAttribute(stage_d2_rb_kernel<false, false, TB, RB>, cudaFuncAttributeMaxDynamicSharedMemorySize, max_smem));
-    const int taylor_smem = (1 << kTaylorTileBits) * 16 + 2048;   // tile + per-bit table
-    const int shapes_smem = (int)taylor_shapes_smem(64);           // several detuning shapes, N <= 64
-    for (const TaylorVariant& v : taylor_variants())
+    for (const TaylorVariant& v : taylor_variants())   // N <= 64
         CUDA_CHECK(cudaFuncSetAttribute(v.kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                        v.smem == TaylorSmem::Shapes ? shapes_smem : taylor_smem));
+                                        (int)taylor_variant_smem(v, 64)));
     CUDA_CHECK(cudaFuncSetAttribute(stage_d2_fwd_kernel<true, TB, RB>, cudaFuncAttributeMaxDynamicSharedMemorySize, 2 * 2048 * 16 + 256));
     CUDA_CHECK(cudaFuncSetAttribute(stage_d2_fwd_kernel<false, TB, RB>, cudaFuncAttributeMaxDynamicSharedMemorySize, 2 * 2048 * 16 + 256));
     if (dev >= 0 && dev < PB200_MAX_DEVICES) sm_count[dev] = sms;
@@ -319,6 +327,7 @@ struct Plan {
     DevBuf<c2> aux[6];  // [0..3] chain pools, [4..5] check copies
     int cur = 0;  // index of the current state buffer
     DevBuf<double> dint;
+    DevBuf<double> cpl;      // the couplings behind dint, N x N per trajectory slot (TaylorArgs::cpl)
     bool dint_shared = true;
     bool has_interaction = false;
     DevBuf<double> d_table;  // per-exponential coefficient tables
@@ -2398,12 +2407,8 @@ static void launch_taylor_order(const Plan& P, bool tiled, const TaylorArgs& a, 
         if (v.uniform != uniform || v.real_g != real_g || v.shard != shard || v.ns != ns || v.cplx != cplx ||
             v.diss != diss)
             continue;
-        const size_t tile = (size_t)16 << kTaylorTileBits;
-        const size_t smem = v.smem == TaylorSmem::Shapes      ? taylor_shapes_smem(P.n)
-                            : v.smem == TaylorSmem::TileTable ? tile + (size_t)d2_table_stride(P.n) * 8
-                                                              : tile;
         launch_k(v.kernel, dim3((unsigned)(P.D >> kTaylorTileBits), uniform ? 1u : (unsigned)P.B),
-                 dim3(1u << (kTaylorTileBits - v.rb)), smem, P.stream, v.pdl, a);
+                 dim3(1u << (kTaylorTileBits - v.rb)), taylor_variant_smem(v, P.n), P.stream, v.pdl, a);
         return;
     }
     fail(PB200_ERR_UNSUPPORTED, "no Taylor stage kernel for UNIFORM=%d REAL_G=%d SHARD=%d NS=%d CPLX=%d DISS=%d", uniform,
@@ -2764,6 +2769,9 @@ static TaylorArgs taylor_plan_args(const Plan& P, const PassGeom& geo, const c2*
     a.v = v; a.out = out;
     a.dint = P.has_interaction ? P.dint.get() : nullptr;
     a.dint_stride = P.dint_shared ? 0 : P.D;
+    a.cpl = P.has_interaction ? P.cpl.get() : nullptr;
+    a.cpl_stride = P.dint_shared ? 0 : (long long)P.n * P.n;
+    a.ryd_bit = P.desc.rydberg_state;
     a.D = P.D;
     a.geo = geo;
     a.unit = unit;
@@ -2808,8 +2816,19 @@ static TaylorArgs taylor_args(const Plan& P, const PassGeom& geo, const TaylorSt
         a.g2_out = (s.n_g && k + 1 < s.K) ? R.gr2[k % s.n_g] : nullptr;
     }
     const bool last = (k + 1 == s.K);
-    if ((k & 1) == 0) { a.acc_on = 1; a.acc_add_v = 1; a.acc_read = k > 0; }
-    else { a.acc_on = last ? 1 : 0; a.acc_add_v = 0; a.acc_read = 1; }
+    // sum_k chi_k: the update of order k adds chi_{k+1} and, with acc_add_v, chi_k.  Where every order k >= 1 reads
+    // chi_{k-1} as a history term, the update takes it too, and the accumulator is read and written on every third
+    // order only: order 0 writes chi_0 + chi_1, order k = 0 mod 3 adds chi_{k-1} + chi_k + chi_{k+1}, and the last
+    // order adds what is left.  Otherwise every even order adds chi_k + chi_{k+1}.
+    bool chi_hist = false;   // hchi[0] is set on every order k >= 1
+    if (s.p >= 1) {
+        chi_hist = th_c(1) != 0.0 || s.gam[1] != 0.0;
+        for (int q = 0; q < PB200_TAYLOR_SMAX; ++q) chi_hist = chi_hist || m_c(q, 1) != 0.0;
+    }
+    const int period = chi_hist ? 3 : 2;
+    a.acc_read = k > 0;
+    if (k % period == 0) { a.acc_on = 1; a.acc_add_v = 1; a.acc_add_h = k > 0 && chi_hist; }
+    else { a.acc_on = last ? 1 : 0; a.acc_add_v = k % period == 2; a.acc_add_h = 0; }
     a.acc_mul = last ? c2{std::cos(s.phi), -std::sin(s.phi)} : c2{1.0, 0.0};
     return a;
 }
@@ -3334,7 +3353,11 @@ int pb200_plan_set_interaction(pb200_plan* h, int32_t traj0, int32_t count, cons
     const bool want_shared = shared != 0;
     if (!P.dint || P.dint_shared != want_shared) {
         P.dint.reset(P, (size_t)P.D * (want_shared ? 1 : P.B));
-        if (!want_shared) CUDA_CHECK(cudaMemsetAsync(P.dint.get(), 0, sizeof(double) * (size_t)P.D * P.B, P.stream));
+        P.cpl.reset(P, (size_t)N * N * (want_shared ? 1 : P.B));
+        if (!want_shared) {
+            CUDA_CHECK(cudaMemsetAsync(P.dint.get(), 0, sizeof(double) * (size_t)P.D * P.B, P.stream));
+            CUDA_CHECK(cudaMemsetAsync(P.cpl.get(), 0, sizeof(double) * (size_t)N * N * P.B, P.stream));
+        }
     }
     P.dint_shared = want_shared;
     P.dmin_traj.resize(want_shared ? 1 : P.B, 0.0);
@@ -3345,7 +3368,7 @@ int pb200_plan_set_interaction(pb200_plan* h, int32_t traj0, int32_t count, cons
         P.dmin2_traj.assign(want_shared ? 1 : P.B, 0.0);
         P.dmax2_traj.assign(want_shared ? 1 : P.B, 0.0);
     }
-    DevBuf<double> dU(P, (size_t)N * N);
+    DevBuf<double> dU2(P, (size_t)N * N);   // part 1; part 0 stays on the device in P.cpl
     std::vector<double> Uc((size_t)N * N);
     // part 0: pairs weighted by w (all pairs, or the pairs not touching the SLM mask); part 1: the pairs touching it
     for (int c = 0; c < count; ++c)
@@ -3362,12 +3385,13 @@ int pb200_plan_set_interaction(pb200_plan* h, int32_t traj0, int32_t count, cons
                 }
                 Uc[(size_t)i * N + j] = u;
             }
-        CUDA_CHECK(cudaMemcpyAsync(dU.get(), Uc.data(), sizeof(double) * N * N, cudaMemcpyHostToDevice, P.stream));
+        double* dU = part == 0 ? P.cpl.get() + (want_shared ? 0 : (size_t)(traj0 + c) * N * N) : dU2.get();
+        CUDA_CHECK(cudaMemcpyAsync(dU, Uc.data(), sizeof(double) * N * N, cudaMemcpyHostToDevice, P.stream));
         double* dst = (part == 0 ? P.dint : P.dint2).get() + (want_shared ? 0 : (size_t)(traj0 + c) * P.D);
         const int threads = 256;
         const long long blocks = std::min<long long>((P.D + threads - 1) / threads, (long long)P.sm_count * 16);
         dint_kernel<<<(unsigned)std::max<long long>(blocks, 1), threads, sizeof(double) * N * N, P.stream>>>(
-            dst, dU.get(), N, P.dim, P.desc.rydberg_state, P.D, P.shard_offset());
+            dst, dU, N, P.dim, P.desc.rydberg_state, P.D, P.shard_offset());
         CUDA_CHECK(cudaGetLastError());
         // bounds per |r>-count
         std::vector<double> mins(N + 1, 1e300), maxs(N + 1, -1e300);
