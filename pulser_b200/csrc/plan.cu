@@ -67,6 +67,14 @@ struct EventPair {
         if (cudaEventCreate(&b) != cudaSuccess) { cudaEventDestroy(a); a = nullptr; fail(PB200_ERR_CUDA, "cudaEventCreate failed"); }
     }
     ~EventPair() { if (a) cudaEventDestroy(a); if (b) cudaEventDestroy(b); }
+    void start(cudaStream_t s) { CUDA_CHECK(cudaEventRecord(a, s)); }
+    float stop_ms(cudaStream_t s) {   // device time since start(); waits for the stream's work so far
+        CUDA_CHECK(cudaEventRecord(b, s));
+        CUDA_CHECK(cudaEventSynchronize(b));
+        float ms = 0.f;
+        CUDA_CHECK(cudaEventElapsedTime(&ms, a, b));
+        return ms;
+    }
     EventPair(const EventPair&) = delete;
     EventPair& operator=(const EventPair&) = delete;
 };
@@ -346,8 +354,6 @@ struct Plan {
     DevBuf<c2> kry; int kry_cap = 0;        // (kry_cap + 3) vectors of B*D
     DevBuf<double> d_kry;                   // alpha[m][B], beta[m][B], acc[3][B][2], norm[B], y[B][m][2]
     int m_last = 8;
-    bool use_krylov = false;
-    long long kry_iters = 0;
     bool has_diss = false;
     // the dissipator as the Taylor stage applies it (TaylorArgs::dw, df), when it qualifies (diss_taylor_analyse)
     struct DissTaylor {
@@ -375,13 +381,17 @@ struct Plan {
     std::vector<double> thresholds;               // per trajectory
     std::vector<long long> jump_count;
     // step-controller state kept between pb200_propagate calls (evaluation times cut a run into many calls):
-    // interval classification of the sampling grid (cache key = window, rough_tol) and the current smooth-step length
+    // interval classification of the sampling grid (cache key = window, rough_tol) and the current smooth-step length,
+    // with the options it was reached under
     struct FineCache { bool valid = false; int window = -1; double rtol = -1.0; std::vector<char> fine, jump; std::vector<int> dist; } fine_cache;
-    double ctrl_Kc = -1.0; double ctrl_key = 0.0; double ctrl_t_end = -1e300;
-    // partner-sum forwarding between Clenshaw stages (stage_d2_fwd_kernel): geometry of a chain's first stage [0],
-    // of the high-bit tile [1] and of the later low-bit stages [2]; one buffer of forwarded sums per chain
-    bool fwd_now = false;           // decided per propagate call
-    PassGeom fwd_geo[3];
+    struct CtrlOptions {
+        double gtol = 0.0; bool extrap = false; int order = 0, Kmax = 0;
+        bool operator==(const CtrlOptions& o) const {
+            return gtol == o.gtol && extrap == o.extrap && order == o.order && Kmax == o.Kmax;
+        }
+    };
+    double ctrl_Kc = -1.0; CtrlOptions ctrl_opts; double ctrl_t_end = -1e300;
+    // partner-sum forwarding between Clenshaw stages (stage_d2_fwd_kernel): one buffer of forwarded sums per chain
     DevBuf<c2> wbuf[2];
     // time-dependent Taylor propagator: the drive relative to the phase of its largest sample, half-width of H at the
     // sampling times, extra ring buffers (beyond buf / aux) for polynomial degrees > 2
@@ -536,6 +546,18 @@ struct ExpParams {  // one exponential exp(-i G), G from Magnus moments
 
 static inline bool is_d2path(const Plan& P) { return P.dim == 2 && P.n_drives == 1 && !P.has_xy; }
 
+// one state with one drive row: the stages read the drive from their arguments (UniformDrive), not from a table
+static inline bool one_uniform_state(const Plan& P) { return is_d2path(P) && P.all_uniform() && P.B == 1; }
+
+// what one propagate call decided for its exponentials
+struct ExpChoice {
+    bool krylov = false;            // Lanczos, else Chebyshev-Clenshaw
+    bool fwd = false;               // partner-sum forwarding between Clenshaw stages (stage_d2_fwd_kernel)
+    PassGeom fwd_passes[3];         // forwarding: a chain's first stage [0], the high-bit tile [1], later low-bit stages [2]
+    std::vector<PassGeom> passes;   // stage geometry without forwarding
+    bool dual_ok = false;           // two chains may share every launch
+};
+
 static inline size_t pidx(const Plan& P, int traj, int q, int row) {
     return ((size_t)traj * P.n_drives + q) * P.n + row;
 }
@@ -667,12 +689,12 @@ static void launch_stage_multi(Plan& P, const std::vector<PassGeom>& passes, con
 constexpr int kFwdMinN = 17, kFwdMaxN = 19;
 
 static bool fwd_eligible(const Plan& P, const std::vector<PassGeom>& passes) {
-    if (!is_d2path(P) || !P.all_uniform() || P.B != 1) return false;
+    if (!one_uniform_state(P)) return false;
     if (passes.size() != 1 || passes[0].hi_bits != 0 || passes[0].lo_bits != kStageTileBits) return false;
     return P.n >= kFwdMinN && P.n <= kFwdMaxN;
 }
 
-static void plan_fwd_geometry(Plan& P) {
+static void plan_fwd_passes(const Plan& P, PassGeom geo[3]) {
     const int N = P.n, TB = kStageTileBits;
     const int hb = std::min(N - TB, TB - 2);
     const unsigned long long all = (N >= 64) ? ~0ULL : ((1ULL << N) - 1ULL);
@@ -681,24 +703,24 @@ static void plan_fwd_geometry(Plan& P) {
     a.n_bits = N; a.lo_bits = TB; a.hi_shift = TB; a.hi_bits = 0; a.first_pass = 1;
     a.tile_flip_mask = (1u << TB) - 1u;
     a.extra_mask = all & ~((1ULL << TB) - 1ULL);
-    P.fwd_geo[0] = a;
+    geo[0] = a;
     a.extra_mask = rest;
-    P.fwd_geo[2] = a;
+    geo[2] = a;
     PassGeom b{};
     b.n_bits = N; b.lo_bits = TB - hb; b.hi_shift = TB; b.hi_bits = hb; b.first_pass = 1;
     b.tile_flip_mask = ((1u << hb) - 1u) << b.lo_bits;
     b.extra_mask = rest;
-    P.fwd_geo[1] = b;
+    geo[1] = b;
 }
 
-static void launch_stage_fwd(Plan& P, const StageIO* io, int n, long long& launches) {
+static void launch_stage_fwd(Plan& P, const ExpChoice& X, const StageIO* io, int n, long long& launches) {
     bool real_g = true;
     for (int c = 0; c < n; ++c) real_g = real_g && io[c].real_g;
     constexpr int TB = kStageTileBits, RB = kStageRegBits;
     StageArgs2 m{};
     for (int c = 0; c < n; ++c) {
         StageArgs& a = m.a[c];
-        a = make_stage_args(P, P.fwd_geo[io[c].fwd_role], io[c], true);
+        a = make_stage_args(P, X.fwd_passes[io[c].fwd_role], io[c], true);
         a.w_in = (io[c].fwd_role > 0) ? io[c].wbuf : nullptr;
         a.w_out = io[c].fwd_emit ? io[c].wbuf : nullptr;
         a.w_plane = P.D * (long long)P.B;
@@ -896,9 +918,8 @@ struct Chain {
 
 static void apply_dissipator(Plan& P, c2* buf, double h, long long& launches);
 
-static void run_chains(Plan& P, Chain* chains, int n, const std::vector<PassGeom>& passes, pb200_run_stats& st) {
-    const bool d2path = is_d2path(P);
-    const bool uniform = d2path && P.all_uniform() && P.B == 1;
+static void run_chains(Plan& P, Chain* chains, int n, const ExpChoice& X, pb200_run_stats& st) {
+    const bool uniform = one_uniform_state(P);
     if (!uniform) {
         size_t total = 0;
         for (int c = 0; c < n; ++c) { chains[c].table_base = total; total += chains[c].prog->tables.size(); }
@@ -911,7 +932,7 @@ static void run_chains(Plan& P, Chain* chains, int n, const std::vector<PassGeom
     }
     long long launches = 0;
     StageIO io[2];
-    if (P.fwd_now)
+    if (X.fwd)
         for (int c = 0; c < n; ++c)
             if (!P.wbuf[c]) P.wbuf[c].reset(P, (size_t)P.D * P.B * 2);
     if (P.has_diss && n != 1) fail(PB200_ERR_STATE, "internal: Lindblad splitting runs one chain at a time");
@@ -929,8 +950,8 @@ static void run_chains(Plan& P, Chain* chains, int n, const std::vector<PassGeom
                 chains[c].next(P, uniform, io[k++]);
             }
         if (k == 0) break;
-        if (P.fwd_now) launch_stage_fwd(P, io, k, launches);
-        else launch_stage_multi(P, passes, io, k, uniform, launches);
+        if (X.fwd) launch_stage_fwd(P, X, io, k, launches);
+        else launch_stage_multi(P, X.passes, io, k, uniform, launches);
         if (P.has_diss && chains[0].e != e_before && chains[0].prog->post_diss[e_before] > 0.0)
             apply_dissipator(P, chains[0].psi, chains[0].prog->post_diss[e_before], launches);
     }
@@ -1022,8 +1043,8 @@ static int krylov_capacity(const Plan& P) {
 // On the register-blocked kernels every iteration is ONE launch: the stage computes the raw vector
 // r_j = G v_j - beta_{j-1} v_{j-1} with its two inner products fused, and the normalisation / orthogonalisation
 // of v_{j+1} is folded into the own-element operands of the next stage (LanczosFuse, kernels.cuh).
-static void krylov_exponential(Plan& P, const ExpParams& E, double tol, const std::vector<PassGeom>& passes,
-                               pb200_run_stats& st) {
+static void krylov_exponential(Plan& P, const ExpParams& E, double tol, const ExpChoice& X, pb200_run_stats& st) {
+    const std::vector<PassGeom>& passes = X.passes;
     if (P.kry_cap == 0) ensure_krylov(P, krylov_capacity(P));
     const int M = P.kry_cap;
     const int B = P.B;
@@ -1035,7 +1056,7 @@ static void krylov_exponential(Plan& P, const ExpParams& E, double tol, const st
     double* d_norm = d_acc + (size_t)6 * B;
     double* d_y = d_norm + B;
     const bool d2path = is_d2path(P);
-    const bool uniform = d2path && P.all_uniform() && B == 1;
+    const bool uniform = one_uniform_state(P);
     double gm, rh; std::vector<double> host;
     build_tables(P, E, gm, rh, host, d2path, /*scaled=*/false);
     st.max_rho = std::max(st.max_rho, rh);
@@ -1150,39 +1171,44 @@ static void krylov_exponential(Plan& P, const ExpParams& E, double tol, const st
     st.n_launches += launches;
     st.n_applies += m_used;
     st.n_exponentials += 1;
-    P.kry_iters += m_used;
 }
 
-static void run_program_krylov(Plan& P, const Program& prog, const std::vector<PassGeom>& passes, pb200_run_stats& st) {
+static void run_program_krylov(Plan& P, const Program& prog, const ExpChoice& X, pb200_run_stats& st) {
     long long launches = 0;
     for (size_t e = 0; e < prog.raw.size(); ++e) {
         if (P.has_diss && prog.pre_diss[e] > 0.0) apply_dissipator(P, P.buf[P.cur].get(), prog.pre_diss[e], launches);
-        krylov_exponential(P, prog.raw[e], prog.ktol.empty() ? 1e-12 : prog.ktol[e], passes, st);
+        krylov_exponential(P, prog.raw[e], prog.ktol.empty() ? 1e-12 : prog.ktol[e], X, st);
         if (P.has_diss && prog.post_diss[e] > 0.0) apply_dissipator(P, P.buf[P.cur].get(), prog.post_diss[e], launches);
     }
     st.n_launches += launches;
 }
 
 // apply exp(-iG) for every exponential in the program, in order, to the current state
-static void run_program(Plan& P, const Program& prog, const std::vector<PassGeom>& passes, pb200_run_stats& st) {
+static void run_program(Plan& P, const Program& prog, const ExpChoice& X, pb200_run_stats& st) {
     if (prog.cheb.empty()) return;
-    if (P.use_krylov) { run_program_krylov(P, prog, passes, st); return; }
+    if (X.krylov) { run_program_krylov(P, prog, X, st); return; }
     Chain ch;
     ch.prog = &prog;
     ch.psi = P.buf[P.cur].get();
     ch.psi_is_private = true;
     for (int i = 0; i < 3; ++i) ch.pool[i] = P.buf[i].get();
-    run_chains(P, &ch, 1, passes, st);
+    run_chains(P, &ch, 1, X, st);
     for (int i = 0; i < 3; ++i)
         if (P.buf[i].get() == ch.result()) P.cur = i;
 }
 
 // ---------------------------------------------------------------------------
-static void moments_for_step(const Plan& P, double a, double b, std::vector<cplx>& g0, std::vector<cplx>& g1,
-                             std::vector<double>& t0, std::vector<double>& t1) {
+// the generator of the order-2 Magnus exponential over [a, b], m0 = int H dt (wc: the SLM weight), and on request the
+// first moment m1 = (1/(b-a)) int (t - mid) H dt (m1->w = 0: the interaction strength is constant)
+static ExpParams step_generator(const Plan& P, double a, double b, ExpParams* m1_out = nullptr) {
     const int N = P.n, B = P.B, nd = P.n_drives;
+    ExpParams m0, m1;
+    std::vector<cplx>& g0 = m0.g; std::vector<cplx>& g1 = m1.g;
+    std::vector<double>& t0 = m0.th; std::vector<double>& t1 = m1.th;
     g0.assign((size_t)B * nd * N, cplx(0)); g1 = g0;
     t0.assign((size_t)B * nd * N, 0.0); t1 = t0;
+    m0.w = b - a;
+    if (P.has_slm) magnus_moments(P.slm_coef, P.times, a, b, m0.wc, m1.wc);
     for (int tr = 0; tr < B; ++tr)
         for (int q = 0; q < nd; ++q) {
             const DriveTables& T = P.tabs[tr][q];
@@ -1202,15 +1228,18 @@ static void moments_for_step(const Plan& P, double a, double b, std::vector<cplx
                 }
             }
         }
+    if (m1_out) *m1_out = std::move(m1);
+    return m0;
 }
 
-// Magnus moments of the SLM coefficient over [a, b]: c0 = int c dt, c1 = (1/(b-a)) int (t - mid) c dt
-static void slm_moments(const Plan& P, double a, double b, double& c0, double& c1) {
-    c0 = 0.0; c1 = 0.0;
-    if (P.has_slm) magnus_moments(P.slm_coef, P.times, a, b, c0, c1);
+// spectral half-width of a generator
+static double generator_rho(const Plan& P, const ExpParams& E) {
+    double gamma0, rho; std::vector<double> scratch_tab;
+    build_tables(P, E, gamma0, rho, scratch_tab, is_d2path(P));
+    return rho;
 }
 
-static void add_exponential(const Plan& P, Program& prog, const ExpParams& E, double tol) {
+static void add_exponential(const Plan& P, Program& prog, const ExpParams& E, double tol, const ExpChoice& X) {
     const bool d2path = is_d2path(P);
     double gamma0, rho;
     std::vector<double> host;
@@ -1229,7 +1258,7 @@ static void add_exponential(const Plan& P, Program& prog, const ExpParams& E, do
     prog.real_g.push_back(g.imag() == 0.0 ? 1 : 0);
     prog.pre_diss.push_back(0.0);
     prog.post_diss.push_back(0.0);
-    if (P.use_krylov) { prog.raw.push_back(E); prog.ktol.push_back(tol); }
+    if (X.krylov) { prog.raw.push_back(E); prog.ktol.push_back(tol); }
 }
 
 // exp(h*A) of a small dense matrix (scaling and squaring, Taylor order 20)
@@ -1334,12 +1363,24 @@ static std::vector<char> fine_intervals(const Plan& P, int window, double rough_
     return fine;
 }
 
+// defaults of refine_window and rough_tol
+constexpr int kRefineWindow = 8;
+constexpr double kRoughTol = 1e-4;
+
+// the interval classification of the sampling grid, cached on the plan; jump intervals count as fine
+static const Plan::FineCache& interval_classes(Plan& P, int window, double rough_tol) {
+    Plan::FineCache& F = P.fine_cache;
+    if (!F.valid || F.window != window || F.rtol != rough_tol) {
+        F.fine = fine_intervals(P, window, rough_tol, 0.05, F.jump, F.dist);
+        for (size_t i = 0; i < F.fine.size(); ++i) if (F.jump[i]) F.fine[i] = 1;
+        F.window = window; F.rtol = rough_tol; F.valid = true;
+    }
+    return F;
+}
+
 // Magnus step [a, b] appended to the program (2 exponentials for order 4)
-static void add_step(const Plan& P, Program& prog, double a, double b, int order, double tol) {
-    std::vector<cplx> g0, g1; std::vector<double> th0, th1;
-    moments_for_step(P, a, b, g0, g1, th0, th1);
+static void add_step(const Plan& P, Program& prog, const ExpChoice& X, double a, double b, int order, double tol) {
     const double h = b - a;
-    const size_t cnt = g0.size();
     const size_t first = prog.cheb.size();
     struct DissMark {  // symmetric splitting exp(h/2 D) U(h) exp(h/2 D) around the unitary part of the step
         const Plan& P; Program& prog; size_t first; double h;
@@ -1351,36 +1392,33 @@ static void add_step(const Plan& P, Program& prog, double a, double b, int order
         }
     } mark{P, prog, first, h};
     if (order == 4) {
+        ExpParams m1;
+        const ExpParams m0 = step_generator(P, a, b, &m1);
+        const size_t cnt = m0.g.size();
         ExpParams E1, E2;
         E1.g.resize(cnt); E1.th.resize(cnt); E2.g.resize(cnt); E2.th.resize(cnt);
         for (size_t x = 0; x < cnt; ++x) {
-            E1.g[x] = 0.5 * g0[x] - 2.0 * g1[x]; E1.th[x] = 0.5 * th0[x] - 2.0 * th1[x];
-            E2.g[x] = 0.5 * g0[x] + 2.0 * g1[x]; E2.th[x] = 0.5 * th0[x] + 2.0 * th1[x];
+            E1.g[x] = 0.5 * m0.g[x] - 2.0 * m1.g[x]; E1.th[x] = 0.5 * m0.th[x] - 2.0 * m1.th[x];
+            E2.g[x] = 0.5 * m0.g[x] + 2.0 * m1.g[x]; E2.th[x] = 0.5 * m0.th[x] + 2.0 * m1.th[x];
         }
         E1.w = 0.5 * h; E2.w = 0.5 * h;
-        { double c0, c1; slm_moments(P, a, b, c0, c1); E1.wc = 0.5 * c0 - 2.0 * c1; E2.wc = 0.5 * c0 + 2.0 * c1; }
-        add_exponential(P, prog, E1, tol);
-        add_exponential(P, prog, E2, tol);
+        E1.wc = 0.5 * m0.wc - 2.0 * m1.wc; E2.wc = 0.5 * m0.wc + 2.0 * m1.wc;
+        add_exponential(P, prog, E1, tol, X);
+        add_exponential(P, prog, E2, tol, X);
     } else {
-        ExpParams E; E.g = g0; E.th = th0; E.w = h;
-        { double c0, c1; slm_moments(P, a, b, c0, c1); E.wc = c0; }
-        add_exponential(P, prog, E, tol);
+        add_exponential(P, prog, step_generator(P, a, b), tol, X);
     }
 }
 
 // number of sub-steps of a jump interval from the a-priori Magnus remainder bound
 static int jump_substeps(const Plan& P, double a, double b, double magnus_tol) {
-    std::vector<cplx> g0, g1; std::vector<double> th0, th1;
-    moments_for_step(P, a, b, g0, g1, th0, th1);
-    ExpParams E; E.g = g0; E.th = th0; E.w = b - a;
-    { double c0, c1; slm_moments(P, a, b, c0, c1); E.wc = c0; }
-    double gm, rh; std::vector<double> scratch_tab;
-    build_tables(P, E, gm, rh, scratch_tab, is_d2path(P));
+    ExpParams m1;
+    const double rh = generator_rho(P, step_generator(P, a, b, &m1));
     double b1 = 0.0;
     for (int tr = 0; tr < P.B; ++tr) {
         double acc = 0.0;
         for (int q = 0; q < P.n_drives; ++q)
-            for (int k = 0; k < P.n; ++k) acc += std::abs(g1[pidx(P, tr, q, k)]) + std::fabs(th1[pidx(P, tr, q, k)]);
+            for (int k = 0; k < P.n; ++k) acc += std::abs(m1.g[pidx(P, tr, q, k)]) + std::fabs(m1.th[pidx(P, tr, q, k)]);
         b1 = std::max(b1, acc);
     }
     const double est = 8.0 * rh * rh * rh * b1 / 60.0;  // (2 rho)^3 |B1| / 60
@@ -1400,11 +1438,9 @@ static void propagate_mcwf(Plan& P, double t_start, double t_stop, const pb200_r
     const double eps = 1e-12;
     const int nt = (int)P.times.size();
     pb200_run_stats st{};
-    P.use_krylov = false; P.fwd_now = false;
-    const std::vector<PassGeom> passes = plan_passes(P.n, kStageTileBits, kMaxExtraBits);
-    std::vector<char> jump; std::vector<int> dist;
-    const std::vector<char> fine = fine_intervals(P, 8, 1e-4, 0.05, jump, dist);
-    (void)fine;
+    ExpChoice X;   // Chebyshev, no forwarding
+    X.passes = plan_passes(P.n, kStageTileBits, kMaxExtraBits);
+    const std::vector<char>& jump = interval_classes(P, kRefineWindow, kRoughTol).jump;
     const int K = (o && o->max_step_samples > 0) ? o->max_step_samples : 1;
     DecayTable dt{};
     for (int dgt = 0; dgt < P.dim; ++dgt) {
@@ -1415,8 +1451,7 @@ static void propagate_mcwf(Plan& P, double t_start, double t_stop, const pb200_r
     const long long blocks = std::min<long long>((P.D + 255) / 256, (long long)P.sm_count * 8);
     dim3 bgrid((unsigned)std::max<long long>(blocks, 1), (unsigned)P.B);
     EventPair evs;
-    cudaEvent_t ev0 = evs.a, ev1 = evs.b;
-    CUDA_CHECK(cudaEventRecord(ev0, P.stream));
+    evs.start(P.stream);
     std::vector<double> norms(P.B), occ((size_t)P.dim * P.n);
     DevBuf<double> d_occ(P, (size_t)P.dim * P.n);   // populations [digit][qudit]
     std::uniform_real_distribution<double> uni(0.0, 1.0);
@@ -1479,8 +1514,8 @@ static void propagate_mcwf(Plan& P, double t_start, double t_stop, const pb200_r
         // exp(-i H_eff h) ~ decay(h/2) U(h) decay(h/2)
         decay(0.25 * h);
         Program prog;
-        add_step(P, prog, t, b, 4, ctol);
-        run_program(P, prog, passes, st);
+        add_step(P, prog, X, t, b, 4, ctol);
+        run_program(P, prog, X, st);
         CUDA_CHECK(cudaStreamSynchronize(P.stream));
         decay(0.25 * h);
         CUDA_CHECK(cudaGetLastError());
@@ -1558,11 +1593,7 @@ static void propagate_mcwf(Plan& P, double t_start, double t_stop, const pb200_r
         P.thresholds[tr] = std::min(P.thresholds[tr], 1.0);
     }
     CUDA_CHECK(cudaGetLastError());
-    CUDA_CHECK(cudaEventRecord(ev1, P.stream));
-    CUDA_CHECK(cudaEventSynchronize(ev1));
-    float ms = 0.f;
-    CUDA_CHECK(cudaEventElapsedTime(&ms, ev0, ev1));
-    st.gpu_ms = ms; st.integrator = 1; st.mean_step_samples = K;
+    st.gpu_ms = evs.stop_ms(P.stream); st.integrator = 1; st.mean_step_samples = K;
     if (stats) *stats = st;
 }
 
@@ -1576,6 +1607,288 @@ static void propagate_taylor(Plan& P, double t_start, double t_stop, const pb200
 // error to pay for: the master equation gets the same a-priori control as a pure state, at a tighter default)
 static double taylor_default_tol(const Plan& P, const pb200_run_opts* o) {
     return (o && o->tol > 0.0) ? o->tol : (P.has_diss ? 1e-10 : 1e-8);
+}
+
+// Host half of the Magnus propagator (integrators 1 and 2): the options of one call [t_start, t_stop] resolved once, the
+// call's exponential choice, and the step controller -- where a step ends, the step-doubling check, accept / reject.
+// Every step is error-controlled.  "Fine" intervals (next to a non-smooth sample) are never merged with their
+// neighbours; elsewhere up to Kc intervals form one step.  In both cases the step may be a fraction of an interval when
+// the controller or the convergence-radius cap ask for it.
+struct MagnusController {
+    Plan& P;
+    double t_stop, eps = 1e-12;
+    double gtol, tol_user, rtol, rate_allowed, rho_cap;
+    bool extrap, adaptive;
+    int Kmax, W, order, check_every, pw_base;
+    ExpChoice X;
+    const Plan::FineCache* F = nullptr;
+    double Kc;                   // current smooth-step length in sampling intervals (real: < 1 means sub-steps)
+    int since_check = 1 << 30;   // force a check at the first smooth step
+    int n_rejected = 0;          // consecutive rejections of the current step
+    bool last_fine = false;
+    double smooth_len = 0.0; long long smooth_steps = 0;
+    pb200_run_stats st{};
+    Program prog;                // steps queued for the next flush
+
+    MagnusController(Plan& P_, double t_start, double t_stop_, const pb200_run_opts* o) : P(P_), t_stop(t_stop_) {
+        gtol = (o && o->tol != 0.0) ? o->tol : (P.has_diss ? 1e-6 : 1e-8);
+        // Richardson extrapolation: on by default (extrapolate = 0 or 1), -1 switches it off
+        extrap = !(o && o->extrapolate < 0);
+        adaptive = gtol > 0.0;
+        // defaults of max_step_samples (adaptive + extrapolated / adaptive / fixed steps)
+        constexpr int kMaxStepExtrap = 32, kMaxStepAdaptive = 16, kMaxStepFixed = 4;
+        Kmax = (o && o->max_step_samples > 0) ? o->max_step_samples
+                                              : (adaptive ? (extrap ? kMaxStepExtrap : kMaxStepAdaptive) : kMaxStepFixed);
+        W = (o && o->refine_window >= 0) ? o->refine_window : kRefineWindow;
+        tol_user = (o && o->cheb_tol > 0) ? o->cheb_tol : 0.0;
+        rtol = (o && o->rough_tol > 0) ? o->rough_tol : kRoughTol;
+        order = (o && o->magnus_order) ? o->magnus_order : 4;
+        check_every = (o && o->check_every > 0) ? o->check_every : 12;
+        if (order != 2 && order != 4) fail(PB200_ERR_INVALID, "magnus_order must be 2 or 4");
+        // error budget per unit of time: gtol over the whole sampling-time range
+        rate_allowed = adaptive ? gtol / std::max(P.times.back() - P.times.front(), 1e-30) : 0.0;
+        // order of the one-step map whose error the controller / extrapolation sees: the Lindblad splitting is
+        // a symmetric 2nd-order scheme whatever the order of its unitary part
+        pw_base = P.has_diss ? 2 : ((order == 4) ? 4 : 2);
+        F = &interval_classes(P, W, rtol);
+        // exponential: Chebyshev-Clenshaw (cost ~ full spectral width) or Lanczos (cost ~ populated spectral width);
+        // auto picks Lanczos when one sampling interval already spans a Chebyshev half-width near 1, i.e. for
+        // strongly blockaded registers whose high-energy states are not populated
+        constexpr double kKrylovRhoPerInterval = 0.9;
+        constexpr double kKrylovStateBytes = 64.0 * 1048576.0;
+        const int req = o ? o->integrator : 0;
+        X.krylov = req == 2;
+        if (req == 0) {
+            const int nt = (int)P.times.size();
+            const double rh1 = generator_rho(P, step_generator(P, P.times[0], P.times[std::min(1, nt - 1)]));
+            // ... or when the state no longer fits L2 (fewer, fatter iterations win once HBM-bound)
+            X.krylov = rh1 > kKrylovRhoPerInterval || (double)P.D * P.B * 16.0 > kKrylovStateBytes;
+        }
+        // spectral half-width of one step's exponential: Chebyshev / Lanczos
+        constexpr double kRhoCapChebyshev = 3.6, kRhoCapKrylov = 12.0;
+        rho_cap = X.krylov ? kRhoCapKrylov : kRhoCapChebyshev;
+        X.passes = plan_passes(P.n, kStageTileBits, kMaxExtraBits);
+        X.dual_ok = dual_chain_ok(P, X.passes) && !P.has_diss && !X.krylov;
+        X.fwd = !X.krylov && !P.has_diss && fwd_eligible(P, X.passes);
+        if (X.fwd) plan_fwd_passes(P, X.fwd_passes);
+        Kc = adaptive ? std::min(extrap ? 8.0 : 4.0, (double)Kmax) : (double)Kmax;
+        // a call that continues where the previous one stopped (same options) inherits its step length: with "Full"
+        // evaluation times every sampling interval is its own call, and re-growing the step from scratch (and paying
+        // the 3x-cost check) on each of them would dominate the run
+        if (adaptive && P.ctrl_Kc > 0.0 && P.ctrl_opts == options() && std::fabs(P.ctrl_t_end - t_start) < 1e-9) {
+            Kc = std::min(P.ctrl_Kc, (double)Kmax);
+            since_check = check_every / 2;
+        }
+    }
+
+    Plan::CtrlOptions options() const { return {gtol, extrap, order, Kmax}; }
+
+    // Chebyshev truncation per exponential: a fifth of the step's share of the error budget
+    // (a hundredth inside a step-doubling check so that the estimate is not truncation noise)
+    double cheb_tol_for(double h, bool check) const {
+        if (tol_user > 0.0) return tol_user;
+        if (!adaptive) return 1e-12;
+        const double share = rate_allowed * h;
+        return std::min(1e-12, std::max(2e-15, (check ? 0.01 : 0.2) * share));
+    }
+
+    void flush() {
+        if (prog.cheb.empty()) return;
+        run_program(P, prog, X, st);
+        CUDA_CHECK(cudaStreamSynchronize(P.stream));  // tables are copied asynchronously from prog
+        prog = Program();
+    }
+
+    void copy_state(const DevBuf<c2>& dst, const DevBuf<c2>& src) {
+        CUDA_CHECK(cudaMemcpyAsync(dst.get(), src.get(), sizeof(c2) * P.D * P.B, cudaMemcpyDeviceToDevice, P.stream));
+    }
+
+    double max_diff2(const DevBuf<c2>& x, const DevBuf<c2>& y) {
+        const int nb = std::min(P.B, 4096);
+        const long long blocks = std::min<long long>((P.D + 255) / 256, (long long)P.sm_count * 4);
+        dim3 grid((unsigned)std::max<long long>(blocks, 1), (unsigned)nb);
+        std::vector<double> d2(nb);
+        device_sum(P, P.d_scratch.get(), nb, d2.data(),
+                   [&] { diffnorm2_kernel<<<grid, 256, 0, P.stream>>>(x.get(), y.get(), P.D, P.d_scratch.get()); });
+        st.n_launches += 1;
+        double e = 0.0;
+        for (double v : d2) e = std::max(e, v);
+        return e;
+    }
+
+    // end of the step from t, which lies in sampling interval i
+    double step_end(double t, int i) {
+        const int nt = (int)P.times.size();
+        const double hi_i = P.times[i + 1] - P.times[i];
+        const bool is_fine = F->fine[i] != 0;
+        if (is_fine != last_fine) { since_check = 1 << 30; last_fine = is_fine; }  // re-validate on region change
+        double Kuse = is_fine ? std::min(Kc, 1.0) : Kc;
+        {   // keep the step inside the convergence radius of the Magnus expansion: the spectral
+            // half-width of int H dt over the step stays below rho_cap (~pi)
+            const double b1 = std::min(P.times[i + 1], t_stop);
+            const double frac = (b1 - t) / hi_i;  // fraction of a sampling interval covered by this probe
+            const double rho_per_sample = generator_rho(P, step_generator(P, t, b1)) / std::max(frac, 1e-9);
+            Kuse = std::min(Kuse, rho_cap / std::max(rho_per_sample, 1e-12));
+        }
+        double b;
+        if (Kuse >= 1.0) {
+            int K = std::max(1, std::min((int)std::floor(Kuse + 1e-9), Kmax));
+            if (is_fine) {
+                b = P.times[i + 1];
+            } else {
+                // graded steps: no longer than half the distance to the nearest non-smooth sample on either side
+                K = std::max(1, std::min(K, F->dist[i] / 2));
+                int j = i, cnt = 0;
+                while (j < nt - 1 && !F->fine[j] && cnt < K && (cnt == 0 || 2 * (cnt + 1) <= std::max(F->dist[j], 2))) { ++j; ++cnt; }
+                b = P.times[j];
+            }
+        } else {
+            const int nsub = std::min(64, (int)std::ceil(1.0 / std::max(Kuse, 1.0 / 64.0) - 1e-9));
+            b = std::min(P.times[i + 1], t + hi_i / nsub);
+        }
+        if (F->jump[i] && order == 4) {  // a-priori sub-stepping of sample-to-sample jumps
+            constexpr double kMagnusTol = 1e-11;
+            const int nsub = jump_substeps(P, t, std::min(P.times[i + 1], t_stop), kMagnusTol);
+            if (nsub > 1) b = std::min(b, t + hi_i / nsub);
+        }
+        b = std::min(b, t_stop);
+        if (b <= t + eps) b = std::min(P.times[std::min(i + 1, nt - 1)], t_stop);
+        return b;
+    }
+
+    // step doubling: one `step` of h from the current state (saved in aux[save]) into aux[save + 1], then two of h/2
+    // from the same state into the current state
+    template <typename Step>
+    void step_doubled(double a, double b, int save, const Step& step) {
+        flush();
+        ensure_aux_buffers(P);
+        copy_state(P.aux[save], P.buf[P.cur]);
+        step(a, b);
+        flush();
+        copy_state(P.aux[save + 1], P.buf[P.cur]);
+        copy_state(P.buf[P.cur], P.aux[save]);
+        const double mid = 0.5 * (a + b);
+        step(a, mid);
+        step(mid, b);
+        flush();
+    }
+
+    // step-length update from the check of [t, b] (e: its squared distance, ctol: its Chebyshev tolerance).  Returns
+    // false when the step is rejected, with the state the check saved in aux[save] restored
+    bool accept(double t, double b, double h_samples, double ctol, double e, int save) {
+        const int pw = extrap ? pw_base + 2 : pw_base;
+        const double scale = std::pow(2.0, pw) - 1.0;
+        const double err_big = std::sqrt(e) * std::pow(2.0, pw) / scale;
+        st.err_estimate += std::sqrt(e) / scale;
+        ++st.n_checks;
+        const double rate = err_big / std::max(b - t, 1e-30);
+        double factor = 2.0;
+        // differences at the level of truncation / rounding noise carry no information
+        const double noise = 50.0 * ctol + 1e-14;
+        if (err_big > noise) factor = std::pow(0.5 * rate_allowed / rate, 1.0 / pw);
+        factor = std::min(2.0, std::max(0.2, factor));
+        const bool controller_limited = h_samples >= 0.9 * Kc;  // not shortened by a cap / grading
+        Kc = std::min((double)Kmax, std::max(1.0 / 16.0, h_samples * factor));
+        // re-check soon after a big cut, and while a controller-limited step is still growing at the
+        // maximum rate (so that the step recovers quickly after a non-smooth stretch)
+        since_check = (factor < 0.7) ? check_every - 2 : ((factor >= 1.9 && controller_limited) ? check_every - 3 : 0);
+        // the state kept by a check is the pair of half steps, whose own error is err_big / 2^pw; if even
+        // that exceeds the step's share of the budget the step is REJECTED: restore the saved state and
+        // retry with the shortened step (at most 4 times in a row, then accept and let the budget absorb it)
+        const double kept_rate = std::sqrt(e) / scale / std::max(b - t, 1e-30);
+        if (kept_rate > rate_allowed && n_rejected < 4 && h_samples > 1.0 / 16.0 + 1e-12) {
+            copy_state(P.buf[P.cur], P.aux[save]);
+            st.err_estimate -= std::sqrt(e) / scale;
+            ++n_rejected; ++st.n_rejected;
+            since_check = 1 << 30;
+            return false;
+        }
+        n_rejected = 0;
+        return true;
+    }
+
+    // Richardson-extrapolated step: one CF4 step of h and two of h/2 from the same state,
+    // psi <- R2 + (R2 - R1) / (2^p - 1); the symmetric scheme gains two orders (6th for CF4).  Uses aux[0..3]
+    void extrap_step(double a, double b, double ctol) {
+        flush();
+        ensure_aux_buffers(P);
+        const double sc = std::pow(2.0, pw_base) - 1.0;
+        const long long total = P.D * (long long)P.B;
+        const long long nb = std::min<long long>((total + 255) / 256, (long long)P.sm_count * 16);
+        if (X.dual_ok) {
+            // the h branch and the h/2 branch start from the same state and are independent: they run as two
+            // chains sharing every kernel launch, each in its own buffers (no state copies at all)
+            const double mid = 0.5 * (a + b);
+            Program big, half;
+            add_step(P, big, X, a, b, order, ctol);
+            add_step(P, half, X, a, mid, order, ctol);
+            add_step(P, half, X, mid, b, order, ctol);
+            c2* Y = P.buf[P.cur].get();
+            c2* others[6]; int k = 0;
+            for (int i = 0; i < 3; ++i) if (i != P.cur) others[k++] = P.buf[i].get();
+            for (int i = 0; i < 4; ++i) others[k++] = P.aux[i].get();
+            Chain ch[2];
+            ch[0].prog = &half; ch[0].psi = Y; for (int i = 0; i < 3; ++i) ch[0].pool[i] = others[i];
+            ch[1].prog = &big;  ch[1].psi = Y; for (int i = 0; i < 3; ++i) ch[1].pool[i] = others[3 + i];
+            run_chains(P, ch, 2, X, st);
+            c2* res = ch[0].result();
+            axpby_kernel<<<(unsigned)nb, 256, 0, P.stream>>>(res, ch[1].result(), 1.0 + 1.0 / sc, -1.0 / sc, total);
+            CUDA_CHECK(cudaGetLastError());
+            st.n_launches += 1;
+            // make `res` the current state buffer (swap handles if it lives in the aux set)
+            bool found = false;
+            for (int i = 0; i < 3; ++i) if (P.buf[i].get() == res) { P.cur = i; found = true; }
+            if (!found)
+                for (int i = 0; i < 4; ++i) if (P.aux[i].get() == res) { std::swap(P.aux[i], P.buf[P.cur]); break; }
+            if (!one_uniform_state(P))
+                CUDA_CHECK(cudaStreamSynchronize(P.stream));  // tables of big/half were uploaded from this scope
+            return;
+        }
+        step_doubled(a, b, 0, [&](double x, double y) { add_step(P, prog, X, x, y, order, ctol); });
+        axpby_kernel<<<(unsigned)nb, 256, 0, P.stream>>>(P.buf[P.cur].get(), P.aux[1].get(), 1.0 + 1.0 / sc, -1.0 / sc, total);
+        CUDA_CHECK(cudaGetLastError());
+        st.n_launches += 1;
+    }
+
+    void run(double t) {
+        const size_t flush_doubles = (size_t)8 << 20;  // 64 MiB of tables per chunk
+        const bool can_aux = (P.D * (long long)P.B) <= (1LL << 31);
+        while (t < t_stop - eps) {
+            const int i = find_piece(P.times, t + eps);
+            const double b = step_end(t, i);
+            const double h_samples = (b - t) / (P.times[i + 1] - P.times[i]);
+            if (adaptive && since_check >= check_every && can_aux) {
+                // check: the step doubled, keeping the pair of half steps (the extrapolated step itself uses aux[0..3])
+                const double ctol = cheb_tol_for(b - t, true);
+                const int save = extrap ? 4 : 0;
+                if (extrap) step_doubled(t, b, save, [&](double x, double y) { extrap_step(x, y, ctol); });
+                else step_doubled(t, b, save, [&](double x, double y) { add_step(P, prog, X, x, y, order, ctol); });
+                if (!accept(t, b, h_samples, ctol, max_diff2(P.buf[P.cur], P.aux[save + 1]), save)) continue;
+            } else if (extrap && can_aux) {
+                extrap_step(t, b, adaptive ? cheb_tol_for(b - t, false) : 1e-13);
+                ++since_check;
+            } else {
+                add_step(P, prog, X, t, b, order, cheb_tol_for(b - t, false));
+                ++since_check;
+                if (prog.tables.size() > flush_doubles) flush();
+            }
+            ++st.n_steps; smooth_len += h_samples; ++smooth_steps;
+            t = b;
+        }
+        flush();
+        P.ctrl_Kc = Kc; P.ctrl_opts = options(); P.ctrl_t_end = t_stop;
+    }
+};
+
+static void propagate_magnus(Plan& P, double t_start, double t_stop, const pb200_run_opts* o, pb200_run_stats* stats) {
+    MagnusController M(P, t_start, t_stop, o);
+    EventPair evs;
+    evs.start(P.stream);
+    M.run(t_start);
+    M.st.gpu_ms = evs.stop_ms(P.stream);
+    M.st.mean_step_samples = M.smooth_steps ? M.smooth_len / M.smooth_steps : 0.0;
+    M.st.integrator = M.X.krylov ? 2 : 1;
+    if (stats) *stats = M.st;
 }
 
 static void propagate(Plan& P, double t_start, double t_stop, const pb200_run_opts* o, pb200_run_stats* stats) {
@@ -1613,299 +1926,7 @@ static void propagate(Plan& P, double t_start, double t_stop, const pb200_run_op
                      g_taylor_why);
         }
     }
-    const double gtol = (o && o->tol != 0.0) ? o->tol : (P.has_diss ? 1e-6 : 1e-8);
-    // Richardson extrapolation: on by default (extrapolate = 0 or 1), -1 switches it off
-    const bool extrap = !(o && o->extrapolate < 0);
-    const bool adaptive = gtol > 0.0;
-    // defaults of max_step_samples (adaptive + extrapolated / adaptive / fixed steps) and refine_window
-    constexpr int kMaxStepExtrap = 32, kMaxStepAdaptive = 16, kMaxStepFixed = 4, kRefineWindow = 8;
-    int Kmax = (o && o->max_step_samples > 0) ? o->max_step_samples
-                                               : (adaptive ? (extrap ? kMaxStepExtrap : kMaxStepAdaptive) : kMaxStepFixed);
-    int W = (o && o->refine_window >= 0) ? o->refine_window : kRefineWindow;
-    const double tol_user = (o && o->cheb_tol > 0) ? o->cheb_tol : 0.0;
-    double rtol = (o && o->rough_tol > 0) ? o->rough_tol : 1e-4;
-    int order = (o && o->magnus_order) ? o->magnus_order : 4;
-    int check_every = (o && o->check_every > 0) ? o->check_every : 12;
-    if (order != 2 && order != 4) fail(PB200_ERR_INVALID, "magnus_order must be 2 or 4");
-
-    pb200_run_stats st{};
-    const std::vector<PassGeom> passes = plan_passes(P.n, kStageTileBits, kMaxExtraBits);
-    if (!P.fine_cache.valid || P.fine_cache.window != W || P.fine_cache.rtol != rtol) {
-        P.fine_cache.fine = fine_intervals(P, W, rtol, 0.05, P.fine_cache.jump, P.fine_cache.dist);
-        for (size_t i = 0; i < P.fine_cache.fine.size(); ++i) if (P.fine_cache.jump[i]) P.fine_cache.fine[i] = 1;
-        P.fine_cache.window = W; P.fine_cache.rtol = rtol; P.fine_cache.valid = true;
-    }
-    const std::vector<char>& jump = P.fine_cache.jump;
-    const std::vector<int>& dist = P.fine_cache.dist;
-    const std::vector<char>& fine = P.fine_cache.fine;
-    const double magnus_tol = 1e-11;
-    const int nt = (int)P.times.size();
-    // error budget per unit of time: gtol over the whole sampling-time range
-    const double rate_allowed = adaptive ? gtol / std::max(thi - tlo, 1e-30) : 0.0;
-    // Chebyshev truncation per exponential: a fifth of the step's share of the error budget
-    // (a hundredth inside a step-doubling check so that the estimate is not truncation noise)
-    auto cheb_tol_for = [&](double h, bool check) {
-        if (tol_user > 0.0) return tol_user;
-        if (!adaptive) return 1e-12;
-        const double share = rate_allowed * h;
-        return std::min(1e-12, std::max(2e-15, (check ? 0.01 : 0.2) * share));
-    };
-
-    EventPair evs;
-    cudaEvent_t ev0 = evs.a, ev1 = evs.b;
-    CUDA_CHECK(cudaEventRecord(ev0, P.stream));
-
-    Program prog;
-    auto flush = [&]() {
-        if (prog.cheb.empty()) return;
-        run_program(P, prog, passes, st);
-        CUDA_CHECK(cudaStreamSynchronize(P.stream));  // tables are copied asynchronously from prog
-        prog = Program();
-    };
-    const size_t flush_doubles = (size_t)8 << 20;  // 64 MiB of tables per chunk
-    const size_t state_bytes = sizeof(c2) * (size_t)P.D * P.B;
-    auto copy_state = [&](const DevBuf<c2>& dst, const DevBuf<c2>& src) {
-        CUDA_CHECK(cudaMemcpyAsync(dst.get(), src.get(), state_bytes, cudaMemcpyDeviceToDevice, P.stream));
-    };
-    auto max_diff2 = [&](const DevBuf<c2>& x, const DevBuf<c2>& y) {
-        const int nb = std::min(P.B, 4096);
-        const long long blocks = std::min<long long>((P.D + 255) / 256, (long long)P.sm_count * 4);
-        dim3 grid((unsigned)std::max<long long>(blocks, 1), (unsigned)nb);
-        std::vector<double> d2(nb);
-        device_sum(P, P.d_scratch.get(), nb, d2.data(),
-                   [&] { diffnorm2_kernel<<<grid, 256, 0, P.stream>>>(x.get(), y.get(), P.D, P.d_scratch.get()); });
-        st.n_launches += 1;
-        double e = 0.0;
-        for (double v : d2) e = std::max(e, v);
-        return e;
-    };
-    // Richardson-extrapolated step: one CF4 step of h and two of h/2 from the same state,
-    // psi <- R2 + (R2 - R1) / (2^p - 1); the symmetric scheme gains two orders (6th for CF4)
-    // exponential: Chebyshev-Clenshaw (cost ~ full spectral width) or Lanczos (cost ~ populated spectral width);
-    // auto picks Lanczos when one sampling interval already spans a Chebyshev half-width near 1, i.e. for
-    // strongly blockaded registers whose high-energy states are not populated
-    {
-        constexpr double kKrylovRhoPerInterval = 0.9;
-        constexpr double kKrylovStateBytes = 64.0 * 1048576.0;
-        const int req = o ? o->integrator : 0;
-        bool kry = (req == 2);
-        if (req == 0) {
-            std::vector<cplx> q0, q1; std::vector<double> r0, r1;
-            const double tb = std::min(P.times[std::min(1, nt - 1)], t_stop);
-            moments_for_step(P, P.times[0], P.times[std::min(1, nt - 1)], q0, q1, r0, r1);
-            ExpParams E; E.g = q0; E.th = r0; E.w = P.times[std::min(1, nt - 1)] - P.times[0];
-            { double c0, c1; slm_moments(P, P.times[0], P.times[std::min(1, nt - 1)], c0, c1); E.wc = c0; }
-            double gm, rh1; std::vector<double> scratch_tab;
-            build_tables(P, E, gm, rh1, scratch_tab, is_d2path(P));
-            // ... or when the state no longer fits L2 (fewer, fatter iterations win once HBM-bound)
-            kry = rh1 > kKrylovRhoPerInterval || (double)P.D * P.B * 16.0 > kKrylovStateBytes;
-            (void)tb;
-        }
-        P.use_krylov = kry;
-    }
-    // spectral half-width of one step's exponential: Chebyshev / Lanczos
-    constexpr double kRhoCapChebyshev = 3.6, kRhoCapKrylov = 12.0;
-    const double rho_cap = P.use_krylov ? kRhoCapKrylov : kRhoCapChebyshev;
-    const bool dual_ok = dual_chain_ok(P, passes) && !P.has_diss && !P.use_krylov;
-    P.fwd_now = !P.use_krylov && !P.has_diss && fwd_eligible(P, passes);
-    if (P.fwd_now) plan_fwd_geometry(P);
-    // order of the one-step map whose error the controller / extrapolation sees: the Lindblad splitting is
-    // a symmetric 2nd-order scheme whatever the order of its unitary part
-    const int pw_base = P.has_diss ? 2 : ((order == 4) ? 4 : 2);
-    auto extrap_step = [&](double a, double b2, double ctol) {
-        flush();
-        ensure_aux_buffers(P);
-        const double mid = 0.5 * (a + b2);
-        const double sc = std::pow(2.0, pw_base) - 1.0;
-        const long long total = P.D * (long long)P.B;
-        const long long nb = std::min<long long>((total + 255) / 256, (long long)P.sm_count * 16);
-        if (dual_ok) {
-            // the h branch and the h/2 branch start from the same state and are independent: they run as two
-            // chains sharing every kernel launch, each in its own buffers (no state copies at all)
-            Program big, half;
-            add_step(P, big, a, b2, order, ctol);
-            add_step(P, half, a, mid, order, ctol);
-            add_step(P, half, mid, b2, order, ctol);
-            c2* X = P.buf[P.cur].get();
-            c2* others[6]; int k = 0;
-            for (int i = 0; i < 3; ++i) if (i != P.cur) others[k++] = P.buf[i].get();
-            for (int i = 0; i < 4; ++i) others[k++] = P.aux[i].get();
-            Chain ch[2];
-            ch[0].prog = &half; ch[0].psi = X; for (int i = 0; i < 3; ++i) ch[0].pool[i] = others[i];
-            ch[1].prog = &big;  ch[1].psi = X; for (int i = 0; i < 3; ++i) ch[1].pool[i] = others[3 + i];
-            run_chains(P, ch, 2, passes, st);
-            c2* res = ch[0].result();
-            axpby_kernel<<<(unsigned)nb, 256, 0, P.stream>>>(res, ch[1].result(), 1.0 + 1.0 / sc, -1.0 / sc, total);
-            CUDA_CHECK(cudaGetLastError());
-            st.n_launches += 1;
-            // make `res` the current state buffer (swap handles if it lives in the aux set)
-            bool found = false;
-            for (int i = 0; i < 3; ++i) if (P.buf[i].get() == res) { P.cur = i; found = true; }
-            if (!found)
-                for (int i = 0; i < 4; ++i) if (P.aux[i].get() == res) { std::swap(P.aux[i], P.buf[P.cur]); break; }
-            if (!(is_d2path(P) && P.all_uniform() && P.B == 1))
-                CUDA_CHECK(cudaStreamSynchronize(P.stream));  // tables of big/half were uploaded from this scope
-            return;
-        }
-        copy_state(P.aux[0], P.buf[P.cur]);
-        add_step(P, prog, a, b2, order, ctol);
-        flush();
-        copy_state(P.aux[1], P.buf[P.cur]);
-        copy_state(P.buf[P.cur], P.aux[0]);
-        add_step(P, prog, a, mid, order, ctol);
-        add_step(P, prog, mid, b2, order, ctol);
-        flush();
-        axpby_kernel<<<(unsigned)nb, 256, 0, P.stream>>>(P.buf[P.cur].get(), P.aux[1].get(), 1.0 + 1.0 / sc, -1.0 / sc, total);
-        CUDA_CHECK(cudaGetLastError());
-        st.n_launches += 1;
-    };
-    // current smooth-step length in sampling intervals (real: < 1 means sub-steps)
-    double Kc = adaptive ? std::min(extrap ? 8.0 : 4.0, (double)Kmax) : (double)Kmax;
-    int since_check = 1 << 30;  // force a check at the first smooth step
-    int n_rejected = 0;         // consecutive rejections of the current step
-    // a call that continues where the previous one stopped (same tolerances) inherits its step length: with "Full"
-    // evaluation times every sampling interval is its own call, and re-growing the step from scratch (and paying
-    // the 3x-cost check) on each of them would dominate the run
-    const double ctrl_key = gtol * 1e3 + (extrap ? 1.0 : 0.0) + 2.0 * order + 16.0 * Kmax;
-    if (adaptive && P.ctrl_Kc > 0.0 && P.ctrl_key == ctrl_key && std::fabs(P.ctrl_t_end - t_start) < 1e-9) {
-        Kc = std::min(P.ctrl_Kc, (double)Kmax);
-        since_check = check_every / 2;
-    }
-    double smooth_len = 0.0; long long smooth_steps = 0;
-    bool last_fine = false;
-    double t = t_start;
-    while (t < t_stop - eps) {
-        const int i = find_piece(P.times, t + eps);
-        const double hi_i = P.times[i + 1] - P.times[i];
-        double b;
-        // Every step is error-controlled.  "Fine" intervals (next to a non-smooth sample) are never merged with
-        // their neighbours; elsewhere up to Kc intervals form one step.  In both cases the step may be a
-        // fraction of an interval when the controller or the convergence-radius cap ask for it.
-        const bool is_fine = fine[i] != 0;
-        const bool smooth = true;
-        if (is_fine != last_fine) { since_check = 1 << 30; last_fine = is_fine; }  // re-validate on region change
-        double Kuse = is_fine ? std::min(Kc, 1.0) : Kc;
-        {   // keep the step inside the convergence radius of the Magnus expansion: the spectral
-            // half-width of int H dt over the step stays below rho_cap (~pi)
-            std::vector<cplx> q0, q1; std::vector<double> r0, r1;
-            moments_for_step(P, t, std::min(P.times[i + 1], t_stop), q0, q1, r0, r1);
-            ExpParams E; E.g = q0; E.th = r0; E.w = std::min(P.times[i + 1], t_stop) - t;
-            { double c0, c1; slm_moments(P, t, std::min(P.times[i + 1], t_stop), c0, c1); E.wc = c0; }
-            double gm, rh1; std::vector<double> scratch_tab;
-            build_tables(P, E, gm, rh1, scratch_tab, is_d2path(P));
-            const double frac = E.w / hi_i;  // fraction of a sampling interval covered by this probe
-            const double rho_per_sample = rh1 / std::max(frac, 1e-9);
-            Kuse = std::min(Kuse, rho_cap / std::max(rho_per_sample, 1e-12));
-        }
-        if (Kuse >= 1.0) {
-            int K = std::max(1, std::min((int)std::floor(Kuse + 1e-9), Kmax));
-            if (is_fine) {
-                b = P.times[i + 1];
-            } else {
-                // graded steps: no longer than half the distance to the nearest non-smooth sample on either side
-                K = std::max(1, std::min(K, dist[i] / 2));
-                int j = i, cnt = 0;
-                while (j < nt - 1 && !fine[j] && cnt < K && (cnt == 0 || 2 * (cnt + 1) <= std::max(dist[j], 2))) { ++j; ++cnt; }
-                b = P.times[j];
-            }
-        } else {
-            const int nsub = std::min(64, (int)std::ceil(1.0 / std::max(Kuse, 1.0 / 64.0) - 1e-9));
-            b = std::min(P.times[i + 1], t + hi_i / nsub);
-        }
-        if (jump[i] && order == 4) {  // a-priori sub-stepping of sample-to-sample jumps
-            const int nsub = jump_substeps(P, t, std::min(P.times[i + 1], t_stop), magnus_tol);
-            if (nsub > 1) b = std::min(b, t + hi_i / nsub);
-        }
-        b = std::min(b, t_stop);
-        if (b <= t + eps) b = std::min(P.times[std::min(i + 1, nt - 1)], t_stop);
-
-        const bool can_aux = (P.D * (long long)P.B) <= (1LL << 31);
-        const bool do_check = smooth && adaptive && since_check >= check_every && can_aux;
-        if (smooth && (do_check || (extrap && can_aux))) {
-            const double h_samples = (b - t) / hi_i;
-            const double ctol = adaptive ? cheb_tol_for(b - t, do_check) : 1e-13;
-            double e = 0.0;  // squared distance of the two solutions compared by a check
-            if (!extrap) {
-                // plain step-doubling check: one step of h against two of h/2 (keep the latter)
-                flush();
-                ensure_aux_buffers(P);
-                copy_state(P.aux[0], P.buf[P.cur]);
-                add_step(P, prog, t, b, order, ctol);
-                flush();
-                copy_state(P.aux[1], P.buf[P.cur]);
-                copy_state(P.buf[P.cur], P.aux[0]);
-                const double mid = 0.5 * (t + b);
-                add_step(P, prog, t, mid, order, ctol);
-                add_step(P, prog, mid, b, order, ctol);
-                flush();
-                e = max_diff2(P.buf[P.cur], P.aux[1]);
-            } else if (!do_check) {
-                extrap_step(t, b, ctol);
-            } else {
-                // check of the extrapolated scheme: E(h) against E(h/2) o E(h/2)
-                flush();
-                ensure_aux_buffers(P);
-                copy_state(P.aux[4], P.buf[P.cur]);
-                extrap_step(t, b, ctol);
-                copy_state(P.aux[5], P.buf[P.cur]);
-                copy_state(P.buf[P.cur], P.aux[4]);
-                const double mid = 0.5 * (t + b);
-                extrap_step(t, mid, ctol);
-                extrap_step(mid, b, ctol);
-                e = max_diff2(P.buf[P.cur], P.aux[5]);
-            }
-            if (do_check) {
-                const int pw = extrap ? pw_base + 2 : pw_base;
-                const double scale = std::pow(2.0, pw) - 1.0;
-                const double err_big = std::sqrt(e) * std::pow(2.0, pw) / scale;
-                st.err_estimate += std::sqrt(e) / scale;
-                ++st.n_checks;
-                const double rate = err_big / std::max(b - t, 1e-30);
-                double factor = 2.0;
-                // differences at the level of truncation / rounding noise carry no information
-                const double noise = 50.0 * ctol + 1e-14;
-                if (err_big > noise) factor = std::pow(0.5 * rate_allowed / rate, 1.0 / pw);
-                factor = std::min(2.0, std::max(0.2, factor));
-                const bool controller_limited = h_samples >= 0.9 * Kc;  // not shortened by a cap / grading
-                Kc = std::min((double)Kmax, std::max(1.0 / 16.0, h_samples * factor));
-                // re-check soon after a big cut, and while a controller-limited step is still growing at the
-                // maximum rate (so that the step recovers quickly after a non-smooth stretch)
-                since_check = (factor < 0.7) ? check_every - 2
-                                             : ((factor >= 1.9 && controller_limited) ? check_every - 3 : 0);
-                // the state kept by a check is the pair of half steps, whose own error is err_big / 2^pw; if even
-                // that exceeds the step's share of the budget the step is REJECTED: restore the saved state and
-                // retry with the shortened step (at most 4 times in a row, then accept and let the budget absorb it)
-                const double kept_rate = std::sqrt(e) / scale / std::max(b - t, 1e-30);
-                if (kept_rate > rate_allowed && n_rejected < 4 && h_samples > 1.0 / 16.0 + 1e-12) {
-                    copy_state(P.buf[P.cur], extrap ? P.aux[4] : P.aux[0]);
-                    st.err_estimate -= std::sqrt(e) / scale;
-                    ++n_rejected; ++st.n_rejected;
-                    since_check = 1 << 30;
-                    continue;
-                }
-                n_rejected = 0;
-            } else {
-                ++since_check;
-            }
-            ++st.n_steps; smooth_len += h_samples; ++smooth_steps;
-        } else {
-            add_step(P, prog, t, b, order, cheb_tol_for(b - t, false));
-            ++st.n_steps;
-            if (smooth) { ++since_check; smooth_len += (b - t) / hi_i; ++smooth_steps; }
-            if (prog.tables.size() > flush_doubles) flush();
-        }
-        t = b;
-    }
-    flush();
-    P.ctrl_Kc = Kc; P.ctrl_key = ctrl_key; P.ctrl_t_end = t_stop;
-    CUDA_CHECK(cudaEventRecord(ev1, P.stream));
-    CUDA_CHECK(cudaEventSynchronize(ev1));
-    float ms = 0.f;
-    CUDA_CHECK(cudaEventElapsedTime(&ms, ev0, ev1));
-    st.gpu_ms = ms;
-    st.mean_step_samples = smooth_steps ? smooth_len / smooth_steps : 0.0;
-    st.integrator = P.use_krylov ? 2 : 1;
-    if (stats) *stats = st;
+    propagate_magnus(P, t_start, t_stop, o, stats);
 }
 
 // ---- time-dependent Taylor propagator (one drive time shape, its phase constant or moving, d = 2) -----------------
@@ -2857,7 +2878,7 @@ struct ShardEvents {
 template <class Next>
 static float taylor_launch_steps(const std::vector<Plan*>& G, const PassGeom& geo, bool tiled, Next&& next,
                                  long long& launches) {
-    const int count = (int)G.size(), sb = G[0]->shard_bits;
+    const int count = (int)G.size(), sb = count > 1 ? G[0]->shard_bits : 0;   // a whole state has no peers
     // plan r, its device current (a whole state's already is)
     auto use = [&](int r) -> Plan& {
         if (count > 1) CUDA_CHECK(cudaSetDevice(G[r]->desc.device));
@@ -2936,49 +2957,34 @@ static ExpParams params_at(const Plan& P, double t) {
     return E;
 }
 
-// one plain H-apply: out_buf = H(t) in_buf (device buffers [B][D])
-static void apply_h_device(Plan& P, double t, const c2* in, c2* out, long long& launches) {
-    const bool d2path = is_d2path(P);
-    const bool uniform = d2path && P.all_uniform() && P.B == 1;
-    ExpParams E = params_at(P, t);
-    std::vector<double> host;
-    const int N = P.n;
-    // unscaled tables: rho = 1, gamma0 = 0
-    if (d2path) {
-        const int stride = d2_table_stride(N);
-        host.assign((size_t)P.B * stride, 0.0);
-        for (int b = 0; b < P.B; ++b) {
-            double* tb = host.data() + (size_t)b * stride;
-            for (int k = 0; k < N; ++k) {
-                const int p = N - 1 - k;
-                tb[2 * p] = E.g[pidx(P, b, 0, k)].real(); tb[2 * p + 1] = E.g[pidx(P, b, 0, k)].imag();
-                tb[2 * N + p] = E.th[pidx(P, b, 0, k)];
-            }
-            tb[3 * N] = 1.0; tb[3 * N + 1] = 0.0;
-        }
-    } else {
-        const int stride = gen_table_stride(N, P.n_drives);
-        host.assign((size_t)P.B * stride, 0.0);
-        for (int b = 0; b < P.B; ++b) {
-            double* tb = host.data() + (size_t)b * stride;
-            for (int q = 0; q < P.n_drives; ++q)
-                for (int k = 0; k < N; ++k) {
-                    tb[q * 3 * N + 2 * k] = E.g[pidx(P, b, q, k)].real();
-                    tb[q * 3 * N + 2 * k + 1] = E.g[pidx(P, b, q, k)].imag();
-                    tb[q * 3 * N + 2 * N + k] = E.th[pidx(P, b, q, k)];
-                }
-            tb[stride - 3] = E.wc; tb[stride - 2] = 1.0; tb[stride - 1] = 0.0;
-        }
+// one plain H(t)-apply as a stage: H(t) unscaled (rho = 1, gamma0 = 0) in the device table and in the uniform drive
+struct ApplyH {
+    bool uniform, real_g;
+    UniformDrive ud{};
+    std::vector<PassGeom> passes;
+
+    void launch(Plan& P, const c2* in, c2* out, long long& launches) const {
+        launch_stage(P, passes, in, nullptr, nullptr, out, StageCoef{{0, 0}, {0, 0}, {1, 0}}, uniform, real_g, ud,
+                     P.d_table.get(), launches);
     }
+};
+
+// out = H(t) in (device buffers [B][D]); returns the set-up, which stays valid until the device table is rewritten
+static ApplyH apply_h_device(Plan& P, double t, const c2* in, c2* out, long long& launches) {
+    const ExpParams E = params_at(P, t);
+    double gamma0, rho; std::vector<double> host;
+    build_tables(P, E, gamma0, rho, host, is_d2path(P), /*scaled=*/false);
     ensure_table_capacity(P, host.size());
     CUDA_CHECK(cudaMemcpyAsync(P.d_table.get(), host.data(), host.size() * sizeof(double), cudaMemcpyHostToDevice, P.stream));
     CUDA_CHECK(cudaStreamSynchronize(P.stream));
-    UniformDrive ud{};
-    ud.g = {E.g[0].real(), E.g[0].imag()}; ud.theta = E.th[0]; ud.w = 1.0; ud.gamma = 0.0;
-    StageCoef sc{{0, 0}, {0, 0}, {1, 0}};
-    const std::vector<PassGeom> passes = plan_passes(P.n, kStageTileBits, kMaxExtraBits);
-    launch_stage(P, passes, in, nullptr, nullptr, out, sc, uniform, E.g[0].imag() == 0.0, ud, P.d_table.get(), launches);
+    ApplyH A;
+    A.uniform = one_uniform_state(P);
+    A.real_g = E.g[0].imag() == 0.0;
+    A.ud.g = {E.g[0].real(), E.g[0].imag()}; A.ud.theta = E.th[0]; A.ud.w = 1.0; A.ud.gamma = 0.0;
+    A.passes = plan_passes(P.n, kStageTileBits, kMaxExtraBits);
+    A.launch(P, in, out, launches);
     CUDA_CHECK(cudaGetLastError());
+    return A;
 }
 
 }  // namespace pb200
@@ -3479,6 +3485,7 @@ int pb200_plan_set_slm_mask(pb200_plan* h, const uint8_t* masked, const double* 
         if (masked[k]) P.slm_bits |= 1ULL << k;
     P.slm_coef = make_interpolant<double>(P.times.data(), coeff, nt, P.desc.interp_order);
     P.has_slm = P.slm_bits != 0;
+    P.fine_cache.valid = false;   // the 0 -> 1 switch of the mask is a jump interval
     PB200_CATCH
 }
 
@@ -3866,27 +3873,14 @@ int pb200_bench_apply(pb200_plan* h, double t_us, int32_t reps, double* ms_out, 
     c2* in = P.buf[P.cur].get();
     c2* outb = P.buf[(P.cur + 1) % 3].get();
     long long launches = 0;
-    apply_h_device(P, t_us, in, outb, launches);  // warm-up + table upload
+    const ApplyH A = apply_h_device(P, t_us, in, outb, launches);  // warm-up + table upload
     CUDA_CHECK(cudaStreamSynchronize(P.stream));
-    const bool d2path = is_d2path(P);
-    const bool uniform = d2path && P.all_uniform() && P.B == 1;
-    ExpParams E = params_at(P, t_us);
-    UniformDrive ud{};
-    ud.g = {E.g[0].real(), E.g[0].imag()}; ud.theta = E.th[0]; ud.w = 1.0; ud.gamma = 0.0;
-    StageCoef sc{{0, 0}, {0, 0}, {1, 0}};
-    const std::vector<PassGeom> passes = plan_passes(P.n, kStageTileBits, kMaxExtraBits);
     EventPair evs;
-    cudaEvent_t e0 = evs.a, e1 = evs.b;
     launches = 0;
-    CUDA_CHECK(cudaEventRecord(e0, P.stream));
-    for (int r = 0; r < reps; ++r)
-        launch_stage(P, passes, in, nullptr, nullptr, outb, sc, uniform, E.g[0].imag() == 0.0, ud, P.d_table.get(), launches);
-    CUDA_CHECK(cudaEventRecord(e1, P.stream));
-    CUDA_CHECK(cudaEventSynchronize(e1));
+    evs.start(P.stream);
+    for (int r = 0; r < reps; ++r) A.launch(P, in, outb, launches);
+    *ms_out = evs.stop_ms(P.stream);
     CUDA_CHECK(cudaGetLastError());
-    float ms = 0.f;
-    CUDA_CHECK(cudaEventElapsedTime(&ms, e0, e1));
-    *ms_out = ms;
     if (launches_out) *launches_out = launches;
     PB200_CATCH
 }
