@@ -713,9 +713,8 @@ static void plan_fwd_passes(const Plan& P, PassGeom geo[3]) {
     geo[1] = b;
 }
 
-static void launch_stage_fwd(Plan& P, const ExpChoice& X, const StageIO* io, int n, long long& launches) {
-    bool real_g = true;
-    for (int c = 0; c < n; ++c) real_g = real_g && io[c].real_g;
+// real_g: every chain's exponential is real (decided by run_chains before the chains emitted their stages)
+static void launch_stage_fwd(Plan& P, const ExpChoice& X, const StageIO* io, int n, bool real_g, long long& launches) {
     constexpr int TB = kStageTileBits, RB = kStageRegBits;
     StageArgs2 m{};
     for (int c = 0; c < n; ++c) {
@@ -862,6 +861,7 @@ struct Chain {
     c2* scratch[2] = {nullptr, nullptr};
     long long applies = 0; double max_rho = 0.0;
     int fwd_parity = 0; bool fwd_valid = false;   // partner-sum forwarding: geometry of the next stage, sums available
+    bool fwd_q = false;                           // the forwarded sums include the Q plane (a complex launch wrote them)
 
     bool done() const { return e >= prog->cheb.size(); }
     c2* result() const { return psi; }
@@ -877,8 +877,10 @@ struct Chain {
         for (int i = 0; i < 3 && k < 2; ++i)
             if (pool[i] != psi) scratch[k++] = pool[i];
     }
-    // fill io for the next stage and advance; requires !done()
-    void next(const Plan& P, bool uniform, StageIO& io) {
+    bool next_real_g() const { return prog->real_g[e] != 0; }
+    // fill io for the next stage and advance; requires !done().  `launch_real`: the stage runs in a launch of the real
+    // forwarding kernel, which writes and reads only the P plane of the forwarded sums
+    void next(const Plan& P, bool uniform, bool launch_real, StageIO& io) {
         if (j < 0) begin_exponential();
         const std::vector<cplx>& a = prog->cheb[e];
         const cplx ph = std::exp(cplx(0.0, -prog->gamma0[e]));
@@ -894,11 +896,15 @@ struct Chain {
         io.ud = prog->ud[e];
         io.table = uniform ? nullptr : P.d_table.get() + table_base + prog->offset[e];
         io.real_g = prog->real_g[e] != 0;
-        // partner-sum forwarding: this stage's geometry and whether a later stage of the chain consumes its sums
+        // partner-sum forwarding: this stage's geometry and whether a later stage of the chain consumes its sums.  A
+        // complex launch also reads the Q plane, which a real launch does not write: after a real launch the first
+        // complex stage gathers all its partners itself, as the first stage of a chain does
+        if (!launch_real && !fwd_q) fwd_valid = false;
         io.fwd_role = !fwd_valid ? 0 : (fwd_parity ? 1 : 2);
         io.fwd_emit = !(j == 0 && e + 1 == prog->cheb.size());
         fwd_parity = (io.fwd_role == 1) ? 0 : 1;
         fwd_valid = io.fwd_emit;
+        fwd_q = !launch_real;
         // shift the recurrence
         if (b1_buf == psi) { b2_kind = 2; kappa = b1_scale; b2_buf = nullptr; }
         else { b2_kind = 1; b2_buf = const_cast<c2*>(b1_buf); }
@@ -936,9 +942,15 @@ static void run_chains(Plan& P, Chain* chains, int n, const ExpChoice& X, pb200_
         for (int c = 0; c < n; ++c)
             if (!P.wbuf[c]) P.wbuf[c].reset(P, (size_t)P.D * P.B * 2);
     if (P.has_diss && n != 1) fail(PB200_ERR_STATE, "internal: Lindblad splitting runs one chain at a time");
+    // PB200_MAGNUS_LOG: one line per forwarding stage and chain (what kernel and which forwarded sums it used)
+    const bool log_fwd = X.fwd && env_int("PB200_MAGNUS_LOG", 0) != 0;
+    if (log_fwd) fprintf(stderr, "magnus fwd chains=%d\n", n);
     while (true) {
         int k = 0;
         size_t e_before = 0;
+        bool real_g = true;   // the stages of this launch all belong to real exponentials
+        for (int c = 0; c < n; ++c)
+            if (!chains[c].done()) real_g = real_g && chains[c].next_real_g();
         for (int c = 0; c < n; ++c)
             if (!chains[c].done()) {
                 if (P.has_diss) {
@@ -947,10 +959,14 @@ static void run_chains(Plan& P, Chain* chains, int n, const ExpChoice& X, pb200_
                         apply_dissipator(P, chains[c].psi, chains[c].prog->pre_diss[e_before], launches);
                 }
                 io[k].wbuf = P.wbuf[c].get();
-                chains[c].next(P, uniform, io[k++]);
+                chains[c].next(P, uniform, real_g, io[k]);
+                if (log_fwd)
+                    fprintf(stderr, "magnus fwd stage chain=%d exp_real=%d launch_real=%d role=%d\n", c,
+                            (int)io[k].real_g, (int)real_g, io[k].fwd_role);
+                ++k;
             }
         if (k == 0) break;
-        if (X.fwd) launch_stage_fwd(P, X, io, k, launches);
+        if (X.fwd) launch_stage_fwd(P, X, io, k, real_g, launches);
         else launch_stage_multi(P, X.passes, io, k, uniform, launches);
         if (P.has_diss && chains[0].e != e_before && chains[0].prog->post_diss[e_before] > 0.0)
             apply_dissipator(P, chains[0].psi, chains[0].prog->post_diss[e_before], launches);
