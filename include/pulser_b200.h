@@ -279,6 +279,46 @@ int pb200_state_copy(pb200_plan* dst, int32_t dst_traj, pb200_plan* src, int32_t
 /* Device pointer of the current state buffer (complex128 [n_traj][D]). */
 int pb200_state_device_ptr(pb200_plan* plan, void** dptr);
 
+/* ---- density matrices ------------------------------------------------------ */
+/* Reductions of the density matrices of a plan with a dissipator
+ * (pb200_plan_set_dissipator): the plan holds vec(rho_b)[r*D + c] = rho_b[r, c]
+ * for N = n_qudits / 2 physical qudits, D = dim^N.  They give the observables of
+ * a master-equation run (default_observables.py:184-561 on a density matrix)
+ * without copying rho to the host.  Values are NOT divided by the trace; the
+ * caller normalises.  A plan without a dissipator is refused
+ * (PB200_ERR_UNSUPPORTED). */
+/* trace[c] = Re Tr rho_{traj0+c} */
+int pb200_density_trace(pb200_plan* plan, int32_t traj0, int32_t count,
+                        double* trace);
+/* occ[count][N]: occ[c][k] = sum_r rho_rr [digit_k(r) == digit] */
+int pb200_density_occupation(pb200_plan* plan, int32_t traj0, int32_t count,
+                             int32_t digit, double* occ);
+/* corr[count][N][N] = Tr(n_i n_j rho), n_k = |digit><digit| on qudit k */
+int pb200_density_correlation(pb200_plan* plan, int32_t traj0, int32_t count,
+                              int32_t digit, double* corr);
+/* out[c] = Tr(op rho_{traj0+c}) as (re, im), op as in pb200_state_expect;
+ * term t reads rho[shift_t(r), r], one element per (term, r). */
+int pb200_density_expect(pb200_plan* plan, int32_t traj0, int32_t count,
+                         const pb200_op_terms* op, double* out);
+/* energy[c] = Re Tr(H rho_{traj0+c}), h2[c] = Re Tr(H^2 rho_{traj0+c}) with
+ * H = H(t_us) of `ham`: a single-trajectory state-vector plan of the same
+ * register and basis on the same device (the noiseless Hamiltonian handed to the
+ * observables).  Reads the diagonal, the drive transitions and the interaction
+ * diagonal of H: O(D (1 + N n_drives)^2) loads, never the whole matrix.  XY
+ * registers are refused (PB200_ERR_UNSUPPORTED). */
+int pb200_density_energy(pb200_plan* plan, pb200_plan* ham, double t_us,
+                         int32_t traj0, int32_t count, double* energy,
+                         double* h2);
+/* out[c] = <phi|rho_{traj0+c}|phi> as (re, im); phi: complex128[D] on the
+ * host (Fidelity observable).  One pass over the D^2 entries. */
+int pb200_density_overlap(pb200_plan* plan, int32_t traj0, int32_t count,
+                          const double* phi, double* out);
+/* Bitstring shots of trajectory `traj` drawn from diag(rho) with the recipe and
+ * the caller's uniforms of pb200_state_sample (negative rounding noise on the
+ * diagonal counts as 0). */
+int pb200_density_sample(pb200_plan* plan, int32_t traj, int32_t one_digit,
+                         const double* uniforms, int32_t n_shots, int64_t* out);
+
 /* ---- hot path ------------------------------------------------------------ */
 /* Advance every trajectory from t_start to t_stop (microseconds, inside the
  * sampling-time range).  Replaces the qutip.sesolve call at

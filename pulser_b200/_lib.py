@@ -125,6 +125,14 @@ def _load() -> C.CDLL:
             C.c_int, [vp, C.c_int32, C.c_int32, dp, C.c_int32, C.POINTER(C.c_int64)]),
         "pb200_state_copy": (C.c_int, [vp, C.c_int32, vp, C.c_int32]),
         "pb200_state_device_ptr": (C.c_int, [vp, C.POINTER(vp)]),
+        "pb200_density_trace": (C.c_int, [vp, C.c_int32, C.c_int32, dp]),
+        "pb200_density_occupation": (C.c_int, [vp, C.c_int32, C.c_int32, C.c_int32, dp]),
+        "pb200_density_correlation": (C.c_int, [vp, C.c_int32, C.c_int32, C.c_int32, dp]),
+        "pb200_density_expect": (C.c_int, [vp, C.c_int32, C.c_int32, C.POINTER(OpTermsDesc), dp]),
+        "pb200_density_energy": (C.c_int, [vp, vp, C.c_double, C.c_int32, C.c_int32, dp, dp]),
+        "pb200_density_overlap": (C.c_int, [vp, C.c_int32, C.c_int32, dp, dp]),
+        "pb200_density_sample": (
+            C.c_int, [vp, C.c_int32, C.c_int32, dp, C.c_int32, C.POINTER(C.c_int64)]),
         "pb200_propagate": (
             C.c_int, [vp, C.c_double, C.c_double, C.POINTER(RunOpts), C.POINTER(RunStats)]),
         "pb200_apply_h": (C.c_int, [vp, C.c_int32, C.c_double, dp, dp]),
@@ -173,6 +181,8 @@ EXPORTED_SYMBOLS = [
     "pb200_host_taylor_shapes",
     "pb200_plan_create_shard", "pb200_shards_link", "pb200_shards_propagate", "pb200_shards_apply_h", "pb200_shards_energy",
     "pb200_shards_expect",
+    "pb200_density_trace", "pb200_density_occupation", "pb200_density_correlation", "pb200_density_expect",
+    "pb200_density_energy", "pb200_density_overlap", "pb200_density_sample",
 ]
 
 lib = _load()

@@ -88,6 +88,8 @@ class B200State(State[complex, float]):
             if set(self.eigenstates) != set(other.eigenstates):
                 raise ValueError(msg)
             raise NotImplementedError(msg)
+        if isinstance(other, DeviceDensityView) and not isinstance(self, _DeviceResident) and self.is_ket:
+            return other.overlap(self)  # <phi|rho|phi> on the device (Fidelity.apply calls target.overlap(state))
         a, b = self._state, other._state
         if a.ndim == 1 and b.ndim == 1:
             return float(np.abs(np.vdot(a, b)) ** 2)
@@ -253,25 +255,106 @@ class DeviceStateView(_DeviceResident, B200State):
         the global ``np.random`` stream, the recipe of ``qutip_result.py:101-158``); same distribution as
         ``B200State.sample`` without the host-side probability dictionary."""
         one_state = one_state or self.infer_one_state()
-        counts = self._plan.sample(int(num_shots), one_state, self._traj)
-        if p_false_pos == 0.0 and p_false_neg == 0.0:
-            return counts
-        keys = list(counts)
-        bitstr_arr = np.repeat(np.array([list(k) for k in keys], dtype=int), [counts[k] for k in keys], axis=0)
-        flip_probs = np.where(bitstr_arr == 1, p_false_neg, p_false_pos)
-        flips = np.random.uniform(size=flip_probs.shape) < flip_probs
-        new_counts: Counter = Counter(map(tuple, bitstr_arr ^ flips))
-        return Counter({"".join(map(str, k)): v for k, v in new_counts.items()})
+        return _spam_flips(self._plan.sample(int(num_shots), one_state, self._traj), p_false_pos, p_false_neg)
 
     def __repr__(self) -> str:
         return f"DeviceStateView(eigenstates={self.eigenstates}, n_qudits={self.n_qudits})"
 
 
-class _HPsiView(_DeviceResident, B200State):
-    """``H(t)|psi>`` of a device-resident state: its squared norm is known from the fused device reduction,
-    the vector itself is only formed (one more H-apply, fetched to the host) if somebody asks for it."""
+def _spam_flips(counts: Counter, p_false_pos: float, p_false_neg: float) -> Counter:
+    """Measurement errors on device-drawn shots: every bit of every shot flips with ``p_false_neg`` (a 1) or
+    ``p_false_pos`` (a 0), with the uniforms of ``B200State.sample`` (qutip_state.py:169-218)."""
+    if p_false_pos == 0.0 and p_false_neg == 0.0:
+        return counts
+    keys = list(counts)
+    bitstr_arr = np.repeat(np.array([list(k) for k in keys], dtype=int), [counts[k] for k in keys], axis=0)
+    flip_probs = np.where(bitstr_arr == 1, p_false_neg, p_false_pos)
+    flips = np.random.uniform(size=flip_probs.shape) < flip_probs
+    new_counts: Counter = Counter(map(tuple, bitstr_arr ^ flips))
+    return Counter({"".join(map(str, k)): v for k, v in new_counts.items()})
 
-    def __init__(self, source: DeviceStateView, ham: "DeviceHamiltonian", norm2: float):
+
+class DeviceDensityView(_DeviceResident, B200State):
+    """The current density matrix of one trajectory of a ``LindbladPlan``, left on the GPU.
+
+    The master-equation counterpart of ``DeviceStateView``: ``Occupation`` / ``CorrelationMatrix``, ``Expectation``
+    of an operator with monomial terms, ``Energy*`` (with ``DeviceHamiltonian``), ``Fidelity`` and ``BitStrings``
+    reduce on the device (``pb200_density_*``), every value divided by the device trace.  Anything else reads a host
+    copy (``to_array``), fetched once.  ``copy.deepcopy`` (``StateResult``) gives a plain ``B200State``, so a stored
+    state never follows the plan as it moves on.
+    """
+
+    def __init__(self, plan: Any, *, eigenstates: Sequence[str], traj: int = 0, trace: float | None = None):
+        State.__init__(self, eigenstates=eigenstates)
+        self._plan = plan
+        self._traj = int(traj)
+        self._host: np.ndarray | None = None
+        self._trace = float(plan.density_trace(self._traj, 1)[0]) if trace is None else float(trace)
+        self._corr: dict[int, np.ndarray] = {}
+        self._energy: dict[tuple[int, float], tuple[float, float]] = {}
+
+    @property
+    def _state(self) -> np.ndarray:  # host copy, normalised like qutip_backend.py:268-272
+        if self._host is None:
+            self._host = self._plan.get_rho()[self._traj] / self._trace
+        return self._host
+
+    @property
+    def is_ket(self) -> bool:
+        return False
+
+    @property
+    def n_qudits(self) -> int:
+        return int(self._plan.n)
+
+    def _projector_expect(self, coeff, letter, targets):
+        if len(targets) == 0:
+            return complex(coeff)
+        if len(targets) > 2:
+            return None
+        digit = self.eigenstates.index(letter)
+        if digit not in self._corr:
+            self._corr[digit] = self._plan.density_correlation(digit, self._traj, 1)[0] / self._trace
+        idx = sorted(targets)
+        return complex(coeff) * float(self._corr[digit][idx[0], idx[-1]])
+
+    def _terms_expect(self, terms: OpTerms) -> complex | None:
+        return complex(self._plan.density_expect(terms, self._traj, 1)[0]) / self._trace
+
+    def _energy_moments(self, plan: Any, t_us: float) -> tuple[float, float]:
+        """``Tr(H rho)``, ``Tr(H^2 rho)`` over the trace, ``H = H(t_us)`` of the single-state plan ``plan``."""
+        key = (id(plan), t_us)
+        if key not in self._energy:
+            e, e2 = self._plan.density_energy(plan, t_us, self._traj, 1)
+            self._energy[key] = (float(e[0]) / self._trace, float(e2[0]) / self._trace)
+        return self._energy[key]
+
+    def overlap(self, other: "B200State") -> float:
+        if isinstance(other, B200State) and not isinstance(other, _DeviceResident) and other.is_ket \
+                and other.eigenstates == self.eigenstates and other.n_qudits == self.n_qudits:
+            return float(self._plan.density_overlap(other._state, self._traj, 1)[0].real / self._trace)
+        return B200State.overlap(self, other)
+
+    def sample(self, *, num_shots: int, one_state: str | None = None, p_false_pos: float = 0.0,
+               p_false_neg: float = 0.0) -> Counter:
+        """Shots drawn on the device from ``diag rho`` (``pb200_density_sample``, the recipe of
+        ``DeviceStateView.sample``), then the same measurement errors."""
+        one_state = one_state or self.infer_one_state()
+        return _spam_flips(self._plan.density_sample(int(num_shots), one_state, self._traj), p_false_pos, p_false_neg)
+
+    def __deepcopy__(self, memo: dict) -> B200State:
+        return B200State(self._state.copy(), eigenstates=self.eigenstates)
+
+    def __repr__(self) -> str:
+        return f"DeviceDensityView(eigenstates={self.eigenstates}, n_qudits={self.n_qudits})"
+
+
+class _HPsiView(_DeviceResident, B200State):
+    """``H(t)|psi>`` (or ``H(t) rho H(t)``) of a device-resident state: its squared norm (trace) is known from the
+    fused device reduction, the state itself is only formed (more H-applies, fetched to the host) if somebody asks
+    for it."""
+
+    def __init__(self, source: DeviceStateView | DeviceDensityView, ham: "DeviceHamiltonian", norm2: float):
         State.__init__(self, eigenstates=source.eigenstates)
         self._source, self._ham, self._weight = source, ham, norm2
         self._host: np.ndarray | None = None
@@ -279,12 +362,13 @@ class _HPsiView(_DeviceResident, B200State):
     @property
     def _state(self) -> np.ndarray:
         if self._host is None:
-            self._host = self._ham._matvec(self._source._state)
+            out = self._ham._matvec(self._source._state)
+            self._host = out if self._source.is_ket else self._ham._matvec(out.conj().T).conj().T
         return self._host
 
     @property
     def is_ket(self) -> bool:
-        return True
+        return self._source.is_ket
 
     @property
     def n_qudits(self) -> int:
@@ -384,7 +468,7 @@ class B200Operator(Operator[complex, complex, B200State]):
             val = state._projector_expect(*self._pattern)
             if val is not None:
                 return val.real if val.imag == 0.0 else val
-        if self._terms is not None and isinstance(state, _DeviceResident) and state.is_ket:
+        if self._terms is not None and isinstance(state, _DeviceResident):
             val = state._terms_expect(self._terms)
             if val is not None:
                 return val.real if self._isherm else val
@@ -511,7 +595,7 @@ class DeviceHamiltonian(B200Operator):
         raise NotImplementedError("DeviceHamiltonian is matrix-free")
 
     def expect(self, state: B200State, /) -> complex:
-        if isinstance(state, DeviceStateView):
+        if isinstance(state, (DeviceStateView, DeviceDensityView)):
             self._validate_other(state, B200State, "B200Operator.expect()")
             mom = state._energy_moments(self._plan, self._t)
             if mom is not None:
@@ -519,7 +603,7 @@ class DeviceHamiltonian(B200Operator):
         return super().expect(state)
 
     def apply_to(self, state: B200State, /) -> B200State:
-        if isinstance(state, DeviceStateView):
+        if isinstance(state, (DeviceStateView, DeviceDensityView)):
             self._validate_other(state, B200State, "B200Operator.apply_to()")
             mom = state._energy_moments(self._plan, self._t)
             if mom is not None:
@@ -781,6 +865,75 @@ class B200Backend(EmulatorBackend):
                 out.extend(results)
         return out
 
+    def _streams_density(self) -> bool:
+        """A master-equation run whose density matrices stay on the device (``_stream_density``): the plan class
+        provides the density reductions, and the register is not XY (``pb200_density_energy`` has no exchange
+        term).  Otherwise the stored density matrices are replayed."""
+        from . import lindblad
+
+        sim = self._sim_obj
+        return (sim._has_collapse_ops() and not sim._use_mcwf() and hasattr(lindblad.LindbladPlan, "density_trace")
+                and sim._hamiltonian_data.basis_data.interaction_type != "XY")
+
+    def _stream_density(self, hplan: Any, atom_order: tuple) -> list[Results]:
+        """Master equation: the density matrices of the trajectories (one without stochastic noise) are evolved in
+        device batches through the evaluation times, and every observable sees a ``DeviceDensityView`` of its
+        trajectory, so no density matrix is stored per evaluation time.  The Hamiltonian handed over is the noiseless
+        one (``qutip_backend.py:258-264``).  One ``Results`` per trajectory repetition, like the replay path; within a
+        batch the observables are visited time-major, as in ``_stream_noisy``."""
+        from . import lindblad
+
+        sim, config = self._sim_obj, self._config
+        eig = sim._hamiltonian_data.basis_data.eigenbasis
+        opts = {"max_step": 0, "cheb_tol": 0.0, "refine_window": -1, "tol": 0.0}
+        times = sim._eval_times_array
+        if _has_stochastic_noise(sim.noise_model):
+            pending = sim._pending_trajectories()
+            if not pending:
+                return []
+            chunks = pending.batches(sim._auto_batch(pending[0][0].hilbert_dim, len(pending), stored_states=False))
+            n_trajectories = sim.n_trajectories
+        else:
+            chunks, n_trajectories = [[(sim._current_spec, 1)]], 1
+        out: list[Results] = []
+        traj_nb = 0
+        for chunk in chunks:
+            if config.print_progress:
+                for _, reps in chunk:
+                    if reps == 1:
+                        print(f"Emulating Trajectory {traj_nb+1}/{n_trajectories}")
+                    else:
+                        print("Emulating Trajectories " f"[{traj_nb+1} - {traj_nb+reps}]/{n_trajectories}")
+                    traj_nb += reps
+            per_traj = [[Results(atom_order=atom_order, total_duration=sim.total_duration_ns) for _ in range(reps)]
+                        for _, reps in chunk]
+            stats: dict = {}
+            with lindblad.LindbladPlan([s for s, _ in chunk], sim._interp_order, sim._gpu) as plan:
+                plan.set_state(sim._initial_state.full().reshape(-1))
+                prev = float(times[0])
+                for t_us in times:
+                    t_us = float(t_us)
+                    if t_us > prev:
+                        st = plan.propagate(prev, t_us, **opts)
+                        for k, v in st.items():
+                            stats[k] = max(stats.get(k, 0), v) if k == "max_rho" else stats.get(k, 0) + v
+                        prev = t_us
+                    t = t_us / (sim._tot_duration * 1e-3)
+                    ham = DeviceHamiltonian(hplan, t_us, eig)
+                    traces = plan.density_trace()
+                    for i, results in enumerate(per_traj):
+                        state = DeviceDensityView(plan, eigenstates=eig, traj=i, trace=float(traces[i]))
+                        for res in results:
+                            for callback in config.callbacks:
+                                callback(config=config, t=t, state=state, hamiltonian=ham, result=res)
+                            for obs in config.observables:
+                                obs(config=config, t=t, state=state, hamiltonian=ham, result=res)
+            sim.last_run_stats = stats
+            sim._current_spec = chunk[-1][0]
+            for results in per_traj:
+                out.extend(results)
+        return out
+
     def _run_sharded(self, devices: list[int]) -> Results:
         """Noiseless sequence on a state vector split over ``devices`` (``B200Config(devices=...)``), streamed through
         the evaluation times like the single-plan run."""
@@ -828,6 +981,10 @@ class B200Backend(EmulatorBackend):
                 self._stream(hplan, res)
                 return res
             if not _has_stochastic_noise(sim.noise_model):
+                if self._streams_density():
+                    sim._validate_options({})
+                    sim._check_supported()
+                    return self._stream_density(hplan, atom_order)[0]
                 with warnings.catch_warnings():
                     warnings.simplefilter("ignore", DeprecationWarning)
                     single = sim.run(**opts)
@@ -840,6 +997,10 @@ class B200Backend(EmulatorBackend):
             if not sim._has_collapse_ops() or sim._use_mcwf():
                 # pure states: observables reduce on the device, nothing is stored per evaluation time
                 streamed = self._stream_noisy(hplan, atom_order)
+                return Results.aggregate(streamed, **_state_aggregators(streamed))
+            if self._streams_density():
+                # density matrices: observables reduce on the device, nothing is stored per evaluation time
+                streamed = self._stream_density(hplan, atom_order)
                 return Results.aggregate(streamed, **_state_aggregators(streamed))
             for cleanres, reps in sim._noisy_runs(print_progress=self._config.print_progress, batch=0,
                                                   opts={"max_step": 0, "cheb_tol": 0.0, "refine_window": -1, "tol": 0.0}):

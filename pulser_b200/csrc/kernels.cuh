@@ -1794,15 +1794,30 @@ __global__ void dint_bounds_kernel(const double* dint, int n, int dim, int rstat
 }
 
 // ---- measurement: bitstring weights, occupations, sampling ---------------------------------------------------
-// weights[b(s)] += |psi_s|^2 with bit k of b = [digit_k(s) == one_digit], qudit 0 = most significant bit
+// The weight of basis state s in trajectory traj: |psi_s|^2 of a ket (RHO = false: D amplitudes per trajectory), or
+// the diagonal element Re rho_ss of a density matrix (RHO = true: vec(rho)[r D + c] = rho_rc, D^2 entries per
+// trajectory, D = the dimension of the physical register).
+template <bool RHO>
+__device__ __forceinline__ double basis_weight(const c2* p, long long traj, long long D, long long s) {
+    if constexpr (RHO) {
+        return p[traj * D * D + s * (D + 1)].x;
+    } else {
+        const c2 v = p[traj * D + s];
+        return v.x * v.x + v.y * v.y;
+    }
+}
+
+// weights[b(s)] += |psi_s|^2 (or rho_ss) with bit k of b = [digit_k(s) == one_digit], qudit 0 = most significant bit
 // (QutipResult._weights, qutip_result.py:101-158: reversal for ground-rydberg and the 3/4-level
 // marginalisation are both this rule).  A shard (d = 2) covers an aligned block of 2^L = D bitstrings: weights[b mod D].
+// A density matrix's diagonal may carry rounding noise below zero: it is clipped so the cumulative sum stays monotone.
+template <bool RHO>
 __global__ void bitstring_weights_kernel(const c2* psi, double* weights, long long D, int n, int dim, int one_digit,
                                          long long off) {
     for (long long s = blockIdx.x * (long long)blockDim.x + threadIdx.x; s < D;
          s += (long long)gridDim.x * blockDim.x) {
-        const c2 v = psi[s];
-        const double p = v.x * v.x + v.y * v.y;
+        double p = basis_weight<RHO>(psi, 0, D, s);
+        if constexpr (RHO) p = fmax(p, 0.0);
         long long rem = off + s, b = 0;
         for (int k = n - 1; k >= 0; --k) {  // qudit k <-> bit n-1-k
             if ((int)(rem % dim) == one_digit) b |= 1LL << (n - 1 - k);
@@ -1813,7 +1828,8 @@ __global__ void bitstring_weights_kernel(const c2* psi, double* weights, long lo
     }
 }
 
-// occ[k] += sum_s |psi_s|^2 [digit_k(s) == digit]   (Occupation observable / <n_k>)
+// occ[k] += sum_s |psi_s|^2 [digit_k(s) == digit]   (Occupation observable / <n_k>; rho_ss for RHO)
+template <bool RHO>
 __global__ void occupation_kernel(const c2* psi, double* occ, long long D, int n, int dim, int digit, long long off) {
     extern __shared__ double socc[];
     for (int i = threadIdx.x; i < n; i += blockDim.x) socc[i] = 0.0;
@@ -1821,8 +1837,7 @@ __global__ void occupation_kernel(const c2* psi, double* occ, long long D, int n
     const long long traj = blockIdx.y;
     for (long long s = blockIdx.x * (long long)blockDim.x + threadIdx.x; s < D;
          s += (long long)gridDim.x * blockDim.x) {
-        const c2 v = psi[traj * D + s];
-        const double p = v.x * v.x + v.y * v.y;
+        const double p = basis_weight<RHO>(psi, traj, D, s);
         if (p == 0.0) continue;
         long long rem = off + s;
         for (int k = n - 1; k >= 0; --k) {
@@ -1837,6 +1852,8 @@ __global__ void occupation_kernel(const c2* psi, double* occ, long long D, int n
 // corr[traj][i*n+j] (i <= j) += sum_s |psi_s|^2 [digit_i(s) == digit][digit_j(s) == digit]
 // (CorrelationMatrix observable <n_i n_j>; the diagonal is the occupation).  A block stages 2048 probabilities and
 // their per-qudit match masks in shared memory; each warp then reduces a subset of the n(n+1)/2 pairs over them.
+// RHO: the weights are the diagonal rho_ss.
+template <bool RHO>
 __global__ void __launch_bounds__(256) correlation_kernel(const c2* psi, double* corr, long long D, int n, int dim, int digit,
                                                           long long off) {
     constexpr int CH = 2048;
@@ -1851,8 +1868,7 @@ __global__ void __launch_bounds__(256) correlation_kernel(const c2* psi, double*
             double p = 0.0;
             unsigned long long m = 0ull;
             if (s < D) {
-                const c2 v = psi[traj * D + s];
-                p = v.x * v.x + v.y * v.y;
+                p = basis_weight<RHO>(psi, traj, D, s);
                 long long rem = off + s;
                 for (int k = n - 1; k >= 0; --k) {
                     if ((int)(rem % dim) == digit) m |= 1ull << k;
@@ -1938,14 +1954,17 @@ __device__ __forceinline__ void exp_reduce(double re, double im, double* acc) {
     }
 }
 
-// acc[traj] += sum_terms (blockIdx.y = trajectory; D = 2^local_bits amplitudes per trajectory; 256 threads)
+// acc[traj] += sum_terms (blockIdx.y = trajectory; D = 2^local_bits amplitudes per trajectory; 256 threads).
+// RHO: src.p[0] holds density matrices of D^2 entries (no shards) and the term reads Tr(term rho) =
+// sum_g term[g, g ^ f] rho[g ^ f, g]: one element per (mask, g), never the whole matrix.
+template <bool RHO>
 __global__ void __launch_bounds__(256) expect_terms_d2_kernel(const __grid_constant__ ExpSrc src, long long D,
                                                               const ExpD2Term* terms, const ExpGenSite* gens,
                                                               const int* chunk_t, const int* chunk_s, int n_chunks,
                                                               double* acc) {
     __shared__ ExpD2Term st[kExpChunkTerms];
     __shared__ ExpGenSite sg[kExpChunkSites];
-    const long long traj_off = (long long)blockIdx.y * D;
+    const long long traj_off = (long long)blockIdx.y * (RHO ? D * D : D);
     const c2* own = src.p[src.shard] + traj_off;
     const unsigned long long off = (unsigned long long)src.shard << src.local_bits;
     const unsigned long long lmask = (unsigned long long)D - 1ull;
@@ -1957,17 +1976,21 @@ __global__ void __launch_bounds__(256) expect_terms_d2_kernel(const __grid_const
         for (int i = threadIdx.x; i < ns; i += blockDim.x) sg[i] = gens[s0 + i];
         __syncthreads();
         for (long long s = blockIdx.x * (long long)blockDim.x + threadIdx.x; s < D; s += (long long)gridDim.x * blockDim.x) {
-            const c2 v = own[s];
+            const c2 v = RHO ? c2{0.0, 0.0} : own[s];
             const unsigned long long g = off | (unsigned long long)s;
             unsigned long long fcur = ~0ull;
-            c2 q = {0.0, 0.0};  // conj(psi_g) psi_{g ^ f}
+            c2 q = {0.0, 0.0};  // conj(psi_g) psi_{g ^ f}, or rho[g ^ f, g]
             for (int t = 0; t < nt; ++t) {
                 const ExpD2Term& T = st[t];
                 if (T.f != fcur) {  // uniform across the block: the loads of a warp are coalesced
                     fcur = T.f;
-                    c2 p = v;
-                    if (fcur) p = src.p[src.shard ^ (int)(fcur >> src.local_bits)][traj_off + (long long)((unsigned long long)s ^ (fcur & lmask))];
-                    q = {v.x * p.x + v.y * p.y, v.x * p.y - v.y * p.x};
+                    if constexpr (RHO) {
+                        q = own[(long long)((unsigned long long)s ^ fcur) * D + s];
+                    } else {
+                        c2 p = v;
+                        if (fcur) p = src.p[src.shard ^ (int)(fcur >> src.local_bits)][traj_off + (long long)((unsigned long long)s ^ (fcur & lmask))];
+                        q = {v.x * p.x + v.y * p.y, v.x * p.y - v.y * p.x};
+                    }
                 }
                 if ((g & T.care) != T.val) continue;
                 c2 c = T.c;
@@ -1986,12 +2009,14 @@ __global__ void __launch_bounds__(256) expect_terms_d2_kernel(const __grid_const
 struct ExpTerm { c2 c; int s0, sn; };
 struct ExpSite { long long stride; int shift, pad; c2 w[4]; };
 
+// RHO: psi holds density matrices of D^2 entries; the term with partner s' reads rho[s', s]
+template <bool RHO>
 __global__ void __launch_bounds__(256) expect_terms_kernel(const c2* psi, long long D, int dim, const ExpTerm* terms,
                                                            const ExpSite* sites, const int* chunk_t, const int* chunk_s,
                                                            int n_chunks, double* acc) {
     __shared__ ExpTerm st[kExpChunkTerms];
     __shared__ ExpSite ss[kExpChunkSites];
-    const c2* v_traj = psi + (long long)blockIdx.y * D;
+    const c2* v_traj = psi + (long long)blockIdx.y * (RHO ? D * D : D);
     double re = 0.0, im = 0.0;
     for (int ch = 0; ch < n_chunks; ++ch) {
         const int t0 = chunk_t[ch], nt = chunk_t[ch + 1] - t0, s0 = chunk_s[ch], ns = chunk_s[ch + 1] - s0;
@@ -2000,7 +2025,7 @@ __global__ void __launch_bounds__(256) expect_terms_kernel(const c2* psi, long l
         for (int i = threadIdx.x; i < ns; i += blockDim.x) ss[i] = sites[s0 + i];
         __syncthreads();
         for (long long s = blockIdx.x * (long long)blockDim.x + threadIdx.x; s < D; s += (long long)gridDim.x * blockDim.x) {
-            const c2 v = v_traj[s];
+            const c2 v = RHO ? c2{0.0, 0.0} : v_traj[s];
             for (int t = 0; t < nt; ++t) {
                 const ExpTerm& T = st[t];
                 c2 c = T.c;
@@ -2014,14 +2039,116 @@ __global__ void __launch_bounds__(256) expect_terms_kernel(const c2* psi, long l
                     sp += (long long)(b - a) * S.stride;
                 }
                 if (c.x == 0.0 && c.y == 0.0) continue;
-                const c2 p = v_traj[sp];
-                const c2 q = {v.x * p.x + v.y * p.y, v.x * p.y - v.y * p.x};
+                c2 q;
+                if constexpr (RHO) {
+                    q = v_traj[sp * D + s];
+                } else {
+                    const c2 p = v_traj[sp];
+                    q = {v.x * p.x + v.y * p.y, v.x * p.y - v.y * p.x};
+                }
                 re = fma(c.x, q.x, re); re = fma(-c.y, q.y, re);
                 im = fma(c.x, q.y, im); im = fma(c.y, q.x, im);
             }
         }
     }
     exp_reduce(re, im, acc);
+}
+
+// ---- reductions of density matrices vec(rho)[r D + c] = rho[r, c] (D^2 entries per trajectory, blockIdx.y) -------
+// acc[2 traj] += Re Tr rho
+__global__ void __launch_bounds__(256) density_trace_kernel(const c2* rho, long long D, double* acc) {
+    double tr = 0.0;
+    for (long long r = blockIdx.x * (long long)blockDim.x + threadIdx.x; r < D; r += (long long)gridDim.x * blockDim.x)
+        tr += basis_weight<true>(rho, blockIdx.y, D, r);
+    exp_reduce(tr, 0.0, acc);
+}
+
+// acc[traj] += <phi| rho |phi> = sum_{r,c} conj(phi_r) rho[r, c] phi_c (complex): a block per row at a time
+__global__ void __launch_bounds__(256) density_overlap_kernel(const c2* phi, const c2* rho, long long D, double* acc) {
+    const c2* m = rho + (long long)blockIdx.y * D * D;
+    double re = 0.0, im = 0.0;
+    for (long long r = blockIdx.x; r < D; r += gridDim.x) {
+        double sr = 0.0, si = 0.0;  // sum_c rho[r, c] phi_c
+        for (long long c = threadIdx.x; c < D; c += blockDim.x) {
+            const c2 a = m[r * D + c], b = phi[c];
+            sr = fma(a.x, b.x, sr); sr = fma(-a.y, b.y, sr);
+            si = fma(a.x, b.y, si); si = fma(a.y, b.x, si);
+        }
+        const c2 p = phi[r];  // conj(p) (sr + i si)
+        re = fma(p.x, sr, re); re = fma(p.y, si, re);
+        im = fma(p.x, si, im); im = fma(-p.y, sr, im);
+    }
+    exp_reduce(re, im, acc);
+}
+
+// H(t) of a single-state plan in the form the density reductions read it: per drive q and qudit k the element
+// g[q][k] = H[.. to_q .., .. from_q ..] (conj(g) on the transposed pair) and the detuning th[q][k] entering as
+// -th |from_q><from_q|_k; dint = the interaction diagonal (nullptr when there is none).  No XY exchange term.
+constexpr int kDensityMaxQudits = 20;
+struct DensityH {
+    c2 g[PB200_MAX_DRIVES_K][kDensityMaxQudits];
+    double th[PB200_MAX_DRIVES_K][kDensityMaxQudits];
+    int to[PB200_MAX_DRIVES_K], from[PB200_MAX_DRIVES_K];
+    int n, dim, n_drives;
+    const double* dint;
+};
+
+// (H rho)[a, r] = sum_b H[a, b] rho[b, r] over the diagonal and the drive transitions of a; diag = H[a, a]
+__device__ __forceinline__ c2 density_h_row(const DensityH& h, const c2* m, long long D, long long a, long long r,
+                                            double& diag) {
+    diag = h.dint ? h.dint[a] : 0.0;
+    double yr = 0.0, yi = 0.0;
+    long long rem = a, st = 1;
+    for (int k = h.n - 1; k >= 0; --k) {  // qudit k has stride dim^(n-1-k)
+        const int digit = (int)(rem % h.dim);
+        rem /= h.dim;
+        for (int q = 0; q < h.n_drives; ++q) {
+            const c2 g = h.g[q][k];
+            if (digit == h.to[q]) {
+                const c2 v = m[(a + (long long)(h.from[q] - h.to[q]) * st) * D + r];
+                yr = fma(g.x, v.x, yr); yr = fma(-g.y, v.y, yr);
+                yi = fma(g.x, v.y, yi); yi = fma(g.y, v.x, yi);
+            } else if (digit == h.from[q]) {
+                const c2 v = m[(a + (long long)(h.to[q] - h.from[q]) * st) * D + r];
+                yr = fma(g.x, v.x, yr); yr = fma(g.y, v.y, yr);
+                yi = fma(g.x, v.y, yi); yi = fma(-g.y, v.x, yi);
+                diag -= h.th[q][k];
+            }
+        }
+        st *= h.dim;
+    }
+    const c2 v = m[a * D + r];
+    return {fma(diag, v.x, yr), fma(diag, v.y, yi)};
+}
+
+// acc[2 traj] += Re Tr(H rho), acc[2 traj + 1] += Re Tr(H^2 rho):  per diagonal index r,
+// (H rho)[r, r] and sum_a H[r, a] (H rho)[a, r] over a = r and the drive partners of r
+__global__ void __launch_bounds__(256) density_energy_kernel(const c2* rho, long long D, const __grid_constant__ DensityH h,
+                                                             double* acc) {
+    const c2* m = rho + (long long)blockIdx.y * D * D;
+    double e1 = 0.0, e2 = 0.0;
+    for (long long r = blockIdx.x * (long long)blockDim.x + threadIdx.x; r < D; r += (long long)gridDim.x * blockDim.x) {
+        double diag, unused;
+        const c2 y = density_h_row(h, m, D, r, r, diag);
+        e1 += y.x;
+        e2 = fma(diag, y.x, e2);
+        long long rem = r, st = 1;
+        for (int k = h.n - 1; k >= 0; --k) {
+            const int digit = (int)(rem % h.dim);
+            rem /= h.dim;
+            for (int q = 0; q < h.n_drives; ++q) {
+                c2 g = h.g[q][k];  // H[r, a]
+                long long a;
+                if (digit == h.to[q]) a = r + (long long)(h.from[q] - h.to[q]) * st;
+                else if (digit == h.from[q]) { a = r + (long long)(h.to[q] - h.from[q]) * st; g.y = -g.y; }
+                else continue;
+                const c2 ya = density_h_row(h, m, D, a, r, unused);
+                e2 = fma(g.x, ya.x, e2); e2 = fma(-g.y, ya.y, e2);
+            }
+            st *= h.dim;
+        }
+    }
+    exp_reduce(e1, e2, acc);
 }
 
 // indices[i] = first j with cum[j] >= u[i] * total  (np.searchsorted(cumsum(w / sum w), rnd), side="left")

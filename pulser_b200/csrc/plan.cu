@@ -1570,7 +1570,7 @@ static void propagate_mcwf(Plan& P, double t_start, double t_stop, const pb200_r
                 const long long nb = std::min<long long>((P.D + 255) / 256, (long long)P.sm_count * 4);
                 device_sum(P, d_occ.get(), occ.size(), occ.data(), [&] {
                     for (int dgt = 0; dgt < P.dim; ++dgt)
-                        occupation_kernel<<<(unsigned)std::max<long long>(nb, 1), 256, sizeof(double) * P.n, P.stream>>>(
+                        occupation_kernel<false><<<(unsigned)std::max<long long>(nb, 1), 256, sizeof(double) * P.n, P.stream>>>(
                             psi, d_occ.get() + (size_t)dgt * P.n, P.D, P.n, P.dim, dgt, 0LL);
                 });
             }
@@ -3213,22 +3213,78 @@ static DevBuf<char> upload_exp(const ExpHost& H, const Plan& P) {
     return X;
 }
 
-// acc[2 c] += <psi_c| op |psi_c> for `count` trajectories; src.p[src.shard] + c D is trajectory c (d = 2), psi (d > 2);
-// X = the device copy of H
-static void launch_expect(const Plan& P, const ExpHost& H, const char* X, const ExpSrc& src, const c2* psi, int count,
-                          double* d_acc) {
-    const long long blocks = std::min<long long>((P.D + 255) / 256, (long long)P.sm_count * 8);
+// acc[2 c] += <psi_c| op |psi_c> for `count` trajectories of D amplitudes; src.p[src.shard] + c D is trajectory c
+// (d = 2), psi (d > 2); X = the device copy of H.  RHO: Tr(op rho_c) of density matrices of D^2 entries instead
+template <bool RHO>
+static void launch_expect(const Plan& P, long long D, const ExpHost& H, const char* X, const ExpSrc& src, const c2* psi,
+                          int count, double* d_acc) {
+    const long long blocks = std::min<long long>((D + 255) / 256, (long long)P.sm_count * 8);
     const dim3 grid((unsigned)std::max<long long>(blocks, 1), (unsigned)count);
     const int* ct = reinterpret_cast<const int*>(X + H.off_ct);
     const int* cs = reinterpret_cast<const int*>(X + H.off_cs);
     if (H.d2)
-        expect_terms_d2_kernel<<<grid, 256, 0, P.stream>>>(src, P.D, reinterpret_cast<const ExpD2Term*>(X),
+        expect_terms_d2_kernel<RHO><<<grid, 256, 0, P.stream>>>(src, D, reinterpret_cast<const ExpD2Term*>(X),
                                                            reinterpret_cast<const ExpGenSite*>(X + H.off_sites), ct, cs,
                                                            H.n_chunks, d_acc);
     else
-        expect_terms_kernel<<<grid, 256, 0, P.stream>>>(psi, P.D, P.dim, reinterpret_cast<const ExpTerm*>(X),
+        expect_terms_kernel<RHO><<<grid, 256, 0, P.stream>>>(psi, D, P.dim, reinterpret_cast<const ExpTerm*>(X),
                                                         reinterpret_cast<const ExpSite*>(X + H.off_sites), ct, cs,
                                                         H.n_chunks, d_acc);
+}
+
+// occ[count][n] of `count` trajectories at src (RHO: density matrices of D^2 entries) of D basis states
+template <bool RHO>
+static void reduce_occupation(const Plan& P, const c2* src, long long D, int n, int count, int digit, double* occ) {
+    CUDA_CHECK(cudaSetDevice(P.desc.device));
+    DevBuf<double> d_occ(P, (size_t)count * n);
+    const long long blocks = std::min<long long>((D + 255) / 256, (long long)P.sm_count * 4);
+    dim3 grid((unsigned)std::max<long long>(blocks, 1), (unsigned)count);
+    device_sum(P, d_occ.get(), d_occ.size(), occ, [&] {
+        occupation_kernel<RHO><<<grid, 256, sizeof(double) * n, P.stream>>>(src, d_occ.get(), D, n, P.dim, digit,
+                                                                          P.shard_offset());
+    });
+}
+
+// corr[count][n][n] (symmetric) of `count` trajectories at src, as reduce_occupation
+template <bool RHO>
+static void reduce_correlation(const Plan& P, const c2* src, long long D, int n, int count, int digit, double* corr) {
+    CUDA_CHECK(cudaSetDevice(P.desc.device));
+    const size_t nn = (size_t)n * n;
+    DevBuf<double> d_c(P, count * nn);
+    const long long blocks = std::min<long long>((D + 2047) / 2048, (long long)P.sm_count * 4);
+    dim3 grid((unsigned)std::max<long long>(blocks, 1), (unsigned)count);
+    device_sum(P, d_c.get(), d_c.size(), corr, [&] {
+        correlation_kernel<RHO><<<grid, 256, 0, P.stream>>>(src, d_c.get(), D, n, P.dim, digit, P.shard_offset());
+    });
+    for (int c = 0; c < count; ++c)  // the kernel fills i <= j
+        for (int i = 0; i < n; ++i)
+            for (int j = 0; j < i; ++j) corr[c * nn + (size_t)i * n + j] = corr[c * nn + (size_t)j * n + i];
+}
+
+// Bitstring shots of one state (RHO: of one density matrix's diagonal) of D basis states on n qudits: the weights of
+// the 2^nbits bitstrings, their inclusive prefix sum and one binary search per uniform (pb200_state_sample).
+template <bool RHO>
+static void sample_bitstrings(const Plan& P, const c2* src, long long D, int n, int nbits, int one_digit,
+                              const double* uniforms, int n_shots, int64_t* out) {
+    if (nbits > 30) fail(PB200_ERR_UNSUPPORTED, "bitstring sampling: at most 30 qudits (32-bit item count of the prefix scan)");
+    CUDA_CHECK(cudaSetDevice(P.desc.device));
+    const long long M = 1LL << nbits;
+    DevBuf<double> d_w(P, (size_t)M), d_u(P, (size_t)n_shots);
+    DevBuf<long long> d_idx(P, (size_t)n_shots);
+    CUDA_CHECK(cudaMemsetAsync(d_w.get(), 0, sizeof(double) * (size_t)M, P.stream));
+    CUDA_CHECK(cudaMemcpyAsync(d_u.get(), uniforms, sizeof(double) * (size_t)n_shots, cudaMemcpyHostToDevice, P.stream));
+    const long long blocks = std::min<long long>((D + 255) / 256, (long long)P.sm_count * 8);
+    bitstring_weights_kernel<RHO><<<(unsigned)std::max<long long>(blocks, 1), 256, 0, P.stream>>>(
+        src, d_w.get(), D, n, P.dim, one_digit, P.shard_offset());
+    CUDA_CHECK(cudaGetLastError());
+    size_t tmp_bytes = 0;
+    CUDA_CHECK(cub::DeviceScan::InclusiveSum(nullptr, tmp_bytes, d_w.get(), d_w.get(), (int)M, P.stream));
+    DevBuf<char> d_tmp(P, tmp_bytes);
+    CUDA_CHECK(cub::DeviceScan::InclusiveSum(d_tmp.get(), tmp_bytes, d_w.get(), d_w.get(), (int)M, P.stream));
+    search_sorted_kernel<<<(n_shots + 255) / 256, 256, 0, P.stream>>>(d_w.get(), M, d_u.get(), d_idx.get(), n_shots);
+    CUDA_CHECK(cudaGetLastError());
+    CUDA_CHECK(cudaMemcpyAsync(out, d_idx.get(), sizeof(long long) * (size_t)n_shots, cudaMemcpyDeviceToHost, P.stream));
+    CUDA_CHECK(cudaStreamSynchronize(P.stream));
 }
 
 #define PB200_TRY try {
@@ -3678,15 +3734,7 @@ int pb200_state_occupation(pb200_plan* h, int32_t traj0, int32_t count, int32_t 
     Plan& P = h->p;
     check_traj_range(P, traj0, count, "pb200_state_occupation");
     if (digit < 0 || digit >= P.dim) fail(PB200_ERR_INVALID, "digit out of range");
-    CUDA_CHECK(cudaSetDevice(P.desc.device));
-    DevBuf<double> d_occ(P, (size_t)count * P.n);
-    const long long blocks = std::min<long long>((P.D + 255) / 256, (long long)P.sm_count * 4);
-    dim3 grid((unsigned)std::max<long long>(blocks, 1), (unsigned)count);
-    device_sum(P, d_occ.get(), d_occ.size(), occ, [&] {
-        occupation_kernel<<<grid, 256, sizeof(double) * P.n, P.stream>>>(P.buf[P.cur].get() + (size_t)traj0 * P.D,
-                                                                           d_occ.get(), P.D, P.n, P.dim, digit,
-                                                                           P.shard_offset());
-    });
+    reduce_occupation<false>(P, P.buf[P.cur].get() + (size_t)traj0 * P.D, P.D, P.n, count, digit, occ);
     PB200_CATCH
 }
 
@@ -3697,18 +3745,7 @@ int pb200_state_correlation(pb200_plan* h, int32_t traj0, int32_t count, int32_t
     check_traj_range(P, traj0, count, "pb200_state_correlation");
     if (digit < 0 || digit >= P.dim) fail(PB200_ERR_INVALID, "digit out of range");
     if (P.n > 40) fail(PB200_ERR_UNSUPPORTED, "too many qudits for the correlation matrix");
-    CUDA_CHECK(cudaSetDevice(P.desc.device));
-    const size_t nn = (size_t)P.n * P.n;
-    DevBuf<double> d_c(P, count * nn);
-    const long long blocks = std::min<long long>((P.D + 2047) / 2048, (long long)P.sm_count * 4);
-    dim3 grid((unsigned)std::max<long long>(blocks, 1), (unsigned)count);
-    device_sum(P, d_c.get(), d_c.size(), corr, [&] {
-        correlation_kernel<<<grid, 256, 0, P.stream>>>(P.buf[P.cur].get() + (size_t)traj0 * P.D, d_c.get(), P.D, P.n, P.dim,
-                                                       digit, P.shard_offset());
-    });
-    for (int c = 0; c < count; ++c)  // the kernel fills i <= j
-        for (int i = 0; i < P.n; ++i)
-            for (int j = 0; j < i; ++j) corr[c * nn + (size_t)i * P.n + j] = corr[c * nn + (size_t)j * P.n + i];
+    reduce_correlation<false>(P, P.buf[P.cur].get() + (size_t)traj0 * P.D, P.D, P.n, count, digit, corr);
     PB200_CATCH
 }
 
@@ -3771,7 +3808,7 @@ int pb200_state_expect(pb200_plan* h, int32_t traj0, int32_t count, const pb200_
     const c2* psi = P.buf[P.cur].get() + (size_t)traj0 * P.D;
     ExpSrc src{};
     src.p[0] = psi; src.shard = 0; src.local_bits = P.n;
-    device_sum(P, d_acc.get(), d_acc.size(), out, [&] { launch_expect(P, H, X.get(), src, psi, count, d_acc.get()); });
+    device_sum(P, d_acc.get(), d_acc.size(), out, [&] { launch_expect<false>(P, P.D, H, X.get(), src, psi, count, d_acc.get()); });
     PB200_CATCH
 }
 
@@ -3784,26 +3821,8 @@ int pb200_state_sample(pb200_plan* h, int32_t traj, int32_t one_digit, const dou
     if (traj < 0 || traj >= P.B) fail(PB200_ERR_INVALID, "trajectory out of range");
     if (one_digit < 0 || one_digit >= P.dim) fail(PB200_ERR_INVALID, "one_digit out of range");
     // a shard samples its own slice: M = its 2^L bitstrings, out[i] = the low L bits of the global bitstring
-    const int nbits = P.n - P.shard_bits;
-    if (nbits > 30) fail(PB200_ERR_UNSUPPORTED, "bitstring sampling: at most 30 qudits (32-bit item count of the prefix scan)");
-    CUDA_CHECK(cudaSetDevice(P.desc.device));
-    const long long M = 1LL << nbits;
-    DevBuf<double> d_w(P, (size_t)M), d_u(P, (size_t)n_shots);
-    DevBuf<long long> d_idx(P, (size_t)n_shots);
-    CUDA_CHECK(cudaMemsetAsync(d_w.get(), 0, sizeof(double) * (size_t)M, P.stream));
-    CUDA_CHECK(cudaMemcpyAsync(d_u.get(), uniforms, sizeof(double) * (size_t)n_shots, cudaMemcpyHostToDevice, P.stream));
-    const long long blocks = std::min<long long>((P.D + 255) / 256, (long long)P.sm_count * 8);
-    bitstring_weights_kernel<<<(unsigned)std::max<long long>(blocks, 1), 256, 0, P.stream>>>(
-        P.buf[P.cur].get() + (size_t)traj * P.D, d_w.get(), P.D, P.n, P.dim, one_digit, P.shard_offset());
-    CUDA_CHECK(cudaGetLastError());
-    size_t tmp_bytes = 0;
-    CUDA_CHECK(cub::DeviceScan::InclusiveSum(nullptr, tmp_bytes, d_w.get(), d_w.get(), (int)M, P.stream));
-    DevBuf<char> d_tmp(P, tmp_bytes);
-    CUDA_CHECK(cub::DeviceScan::InclusiveSum(d_tmp.get(), tmp_bytes, d_w.get(), d_w.get(), (int)M, P.stream));
-    search_sorted_kernel<<<(n_shots + 255) / 256, 256, 0, P.stream>>>(d_w.get(), M, d_u.get(), d_idx.get(), n_shots);
-    CUDA_CHECK(cudaGetLastError());
-    CUDA_CHECK(cudaMemcpyAsync(out, d_idx.get(), sizeof(long long) * (size_t)n_shots, cudaMemcpyDeviceToHost, P.stream));
-    CUDA_CHECK(cudaStreamSynchronize(P.stream));
+    sample_bitstrings<false>(P, P.buf[P.cur].get() + (size_t)traj * P.D, P.D, P.n, P.n - P.shard_bits, one_digit,
+                             uniforms, n_shots, out);
     PB200_CATCH
 }
 
@@ -3831,6 +3850,159 @@ int pb200_state_device_ptr(pb200_plan* h, void** dptr) {
     PB200_TRY
     if (!h || !dptr) fail(PB200_ERR_INVALID, "null argument");
     *dptr = h->p.buf[h->p.cur].get();
+    PB200_CATCH
+}
+
+// ---- reductions of density matrices (plans with a dissipator) ------------------------------------------------------
+// The plan holds vec(rho) of N = n / 2 physical qudits: D = dim^N, trajectory b at buf + b D^2.
+struct DensityGeom { int n; long long D; };
+
+static DensityGeom density_geom(const Plan& P, const char* who) {
+    if (!P.has_diss)
+        fail(PB200_ERR_UNSUPPORTED, "%s: the plan holds state vectors, not a density matrix (no dissipator)", who);
+    if (!P.state_set) fail(PB200_ERR_STATE, "%s: no state set", who);
+    DensityGeom G{P.n / 2, 1};
+    for (int k = 0; k < G.n; ++k) G.D *= P.dim;
+    return G;
+}
+
+static const c2* density_at(const Plan& P, const DensityGeom& G, int traj) {
+    return P.buf[P.cur].get() + (size_t)traj * G.D * G.D;
+}
+
+int pb200_density_trace(pb200_plan* h, int32_t traj0, int32_t count, double* trace) {
+    PB200_TRY
+    if (!h || !trace) fail(PB200_ERR_INVALID, "pb200_density_trace: null argument");
+    Plan& P = h->p;
+    const DensityGeom G = density_geom(P, "pb200_density_trace");
+    check_traj_range(P, traj0, count, "pb200_density_trace");
+    CUDA_CHECK(cudaSetDevice(P.desc.device));
+    DevBuf<double> d_acc(P, 2 * (size_t)count);
+    std::vector<double> acc(2 * (size_t)count);
+    const long long blocks = std::min<long long>((G.D + 255) / 256, (long long)P.sm_count * 4);
+    dim3 grid((unsigned)std::max<long long>(blocks, 1), (unsigned)count);
+    device_sum(P, d_acc.get(), acc.size(), acc.data(), [&] {
+        density_trace_kernel<<<grid, 256, 0, P.stream>>>(density_at(P, G, traj0), G.D, d_acc.get());
+    });
+    for (int c = 0; c < count; ++c) trace[c] = acc[2 * (size_t)c];
+    PB200_CATCH
+}
+
+int pb200_density_occupation(pb200_plan* h, int32_t traj0, int32_t count, int32_t digit, double* occ) {
+    PB200_TRY
+    if (!h || !occ) fail(PB200_ERR_INVALID, "pb200_density_occupation: null argument");
+    Plan& P = h->p;
+    const DensityGeom G = density_geom(P, "pb200_density_occupation");
+    check_traj_range(P, traj0, count, "pb200_density_occupation");
+    if (digit < 0 || digit >= P.dim) fail(PB200_ERR_INVALID, "pb200_density_occupation: digit out of range");
+    reduce_occupation<true>(P, density_at(P, G, traj0), G.D, G.n, count, digit, occ);
+    PB200_CATCH
+}
+
+int pb200_density_correlation(pb200_plan* h, int32_t traj0, int32_t count, int32_t digit, double* corr) {
+    PB200_TRY
+    if (!h || !corr) fail(PB200_ERR_INVALID, "pb200_density_correlation: null argument");
+    Plan& P = h->p;
+    const DensityGeom G = density_geom(P, "pb200_density_correlation");
+    check_traj_range(P, traj0, count, "pb200_density_correlation");
+    if (digit < 0 || digit >= P.dim) fail(PB200_ERR_INVALID, "pb200_density_correlation: digit out of range");
+    reduce_correlation<true>(P, density_at(P, G, traj0), G.D, G.n, count, digit, corr);
+    PB200_CATCH
+}
+
+int pb200_density_expect(pb200_plan* h, int32_t traj0, int32_t count, const pb200_op_terms* op, double* out) {
+    PB200_TRY
+    NvtxRange nvtx_range("pb200_density_expect");
+    if (!h || !out) fail(PB200_ERR_INVALID, "pb200_density_expect: null argument");
+    Plan& P = h->p;
+    const DensityGeom G = density_geom(P, "pb200_density_expect");
+    check_traj_range(P, traj0, count, "pb200_density_expect");
+    check_op_terms(op, G.n, P.dim, "pb200_density_expect");
+    std::fill(out, out + 2 * (size_t)count, 0.0);
+    const ExpHost H = exp_host(op, G.n, P.dim, G.n);
+    if (H.n_chunks == 0) return PB200_OK;
+    CUDA_CHECK(cudaSetDevice(P.desc.device));
+    const DevBuf<char> X = upload_exp(H, P);
+    DevBuf<double> d_acc(P, 2 * (size_t)count);
+    const c2* rho = density_at(P, G, traj0);
+    ExpSrc src{};
+    src.p[0] = rho; src.shard = 0; src.local_bits = G.n;
+    device_sum(P, d_acc.get(), d_acc.size(), out, [&] { launch_expect<true>(P, G.D, H, X.get(), src, rho, count, d_acc.get()); });
+    PB200_CATCH
+}
+
+int pb200_density_energy(pb200_plan* h, pb200_plan* ham, double t_us, int32_t traj0, int32_t count, double* energy,
+                         double* h2) {
+    PB200_TRY
+    NvtxRange nvtx_range("pb200_density_energy");
+    if (!h || !ham || !energy || !h2) fail(PB200_ERR_INVALID, "pb200_density_energy: null argument");
+    Plan& P = h->p;
+    const Plan& Q = ham->p;
+    const DensityGeom G = density_geom(P, "pb200_density_energy");
+    check_traj_range(P, traj0, count, "pb200_density_energy");
+    if (P.has_xy || Q.has_xy)
+        fail(PB200_ERR_UNSUPPORTED, "pb200_density_energy: XY registers (the exchange term is not evaluated)");
+    if (Q.has_diss || Q.has_collapse || Q.shard_bits || Q.B != 1)
+        fail(PB200_ERR_INVALID, "pb200_density_energy: the Hamiltonian plan must be a single-state plan without noise");
+    if (Q.n != G.n || Q.dim != P.dim)
+        fail(PB200_ERR_INVALID, "pb200_density_energy: the Hamiltonian plan has %d qudits of dimension %d, the density "
+             "matrix %d of dimension %d", Q.n, Q.dim, G.n, P.dim);
+    if (Q.desc.device != P.desc.device) fail(PB200_ERR_UNSUPPORTED, "pb200_density_energy: plans on different devices");
+    if (G.n > kDensityMaxQudits) fail(PB200_ERR_UNSUPPORTED, "pb200_density_energy: at most %d qudits", kDensityMaxQudits);
+    check_drives_set(Q, "pb200_density_energy");
+    const ExpParams E = params_at(Q, t_us);
+    DensityH dh{};
+    dh.n = G.n; dh.dim = Q.dim; dh.n_drives = Q.n_drives;
+    for (int q = 0; q < Q.n_drives; ++q) {
+        dh.to[q] = Q.desc.drives[q].state_to;
+        dh.from[q] = Q.desc.drives[q].state_from;
+        for (int k = 0; k < G.n; ++k) {
+            const cplx g = E.g[pidx(Q, 0, q, k)];
+            dh.g[q][k] = {g.real(), g.imag()};
+            dh.th[q][k] = E.th[pidx(Q, 0, q, k)];
+        }
+    }
+    dh.dint = Q.has_interaction ? Q.dint.get() : nullptr;  // complete: pb200_plan_set_interaction synchronises
+    CUDA_CHECK(cudaSetDevice(P.desc.device));
+    DevBuf<double> d_acc(P, 2 * (size_t)count);
+    std::vector<double> acc(2 * (size_t)count);
+    const long long blocks = (G.D + 255) / 256;
+    dim3 grid((unsigned)std::max<long long>(blocks, 1), (unsigned)count);
+    device_sum(P, d_acc.get(), acc.size(), acc.data(), [&] {
+        density_energy_kernel<<<grid, 256, 0, P.stream>>>(density_at(P, G, traj0), G.D, dh, d_acc.get());
+    });
+    for (int c = 0; c < count; ++c) { energy[c] = acc[2 * (size_t)c]; h2[c] = acc[2 * (size_t)c + 1]; }
+    PB200_CATCH
+}
+
+int pb200_density_overlap(pb200_plan* h, int32_t traj0, int32_t count, const double* phi, double* out) {
+    PB200_TRY
+    if (!h || !phi || !out) fail(PB200_ERR_INVALID, "pb200_density_overlap: null argument");
+    Plan& P = h->p;
+    const DensityGeom G = density_geom(P, "pb200_density_overlap");
+    check_traj_range(P, traj0, count, "pb200_density_overlap");
+    CUDA_CHECK(cudaSetDevice(P.desc.device));
+    c2* d_phi = P.buf[(P.cur + 1) % 3].get();  // scratch of B D^2 >= D amplitudes
+    CUDA_CHECK(cudaMemcpyAsync(d_phi, phi, sizeof(c2) * (size_t)G.D, cudaMemcpyHostToDevice, P.stream));
+    DevBuf<double> d_acc(P, 2 * (size_t)count);
+    const long long blocks = std::min<long long>(G.D, (long long)P.sm_count * 8);
+    dim3 grid((unsigned)std::max<long long>(blocks, 1), (unsigned)count);
+    device_sum(P, d_acc.get(), d_acc.size(), out, [&] {
+        density_overlap_kernel<<<grid, 256, 0, P.stream>>>(d_phi, density_at(P, G, traj0), G.D, d_acc.get());
+    });
+    PB200_CATCH
+}
+
+int pb200_density_sample(pb200_plan* h, int32_t traj, int32_t one_digit, const double* uniforms, int32_t n_shots,
+                         int64_t* out) {
+    PB200_TRY
+    NvtxRange nvtx_range("pb200_density_sample");
+    if (!h || !uniforms || !out || n_shots < 1) fail(PB200_ERR_INVALID, "pb200_density_sample: bad argument");
+    Plan& P = h->p;
+    const DensityGeom G = density_geom(P, "pb200_density_sample");
+    if (traj < 0 || traj >= P.B) fail(PB200_ERR_INVALID, "pb200_density_sample: trajectory out of range");
+    if (one_digit < 0 || one_digit >= P.dim) fail(PB200_ERR_INVALID, "pb200_density_sample: one_digit out of range");
+    sample_bitstrings<true>(P, density_at(P, G, traj), G.D, G.n, G.n, one_digit, uniforms, n_shots, out);
     PB200_CATCH
 }
 
@@ -4104,7 +4276,7 @@ int pb200_shards_expect(pb200_plan** plans, int32_t count, const pb200_op_terms*
         X[r] = upload_exp(H, P);
         acc[r].reset(P, 2);
         src.shard = r;
-        sum_launch(P, acc[r].get(), 2, [&] { launch_expect(P, H, X[r].get(), src, nullptr, 1, acc[r].get()); });
+        sum_launch(P, acc[r].get(), 2, [&] { launch_expect<false>(P, P.D, H, X[r].get(), src, nullptr, 1, acc[r].get()); });
     }
     for (int r = 0; r < count; ++r) {
         double a[2];

@@ -126,3 +126,72 @@ class LindbladPlan:
     def get_rho(self) -> np.ndarray:
         """[n_traj, D, D]"""
         return self.plan.get_state().reshape(-1, self.D, self.D)
+
+    # --- reductions on the device (pb200_density_*): not divided by the trace --------------------------------------
+    @property
+    def n_traj(self) -> int:
+        return self.plan.n_traj
+
+    def _count(self, traj0: int, count: int | None) -> int:
+        return self.plan.n_traj - traj0 if count is None else count
+
+    def density_trace(self, traj0: int = 0, count: int | None = None) -> np.ndarray:
+        """``Re Tr rho_b``, ``[count]``."""
+        count = self._count(traj0, count)
+        out = np.empty(count, dtype=np.float64)
+        check(lib.pb200_density_trace(self.plan._handle, traj0, count, _p(out)))
+        return out
+
+    def density_occupation(self, digit: int, traj0: int = 0, count: int | None = None) -> np.ndarray:
+        """``Tr(|digit><digit|_k rho_b)``, ``[count, N]``."""
+        count = self._count(traj0, count)
+        out = np.empty((count, self.n), dtype=np.float64)
+        check(lib.pb200_density_occupation(self.plan._handle, traj0, count, int(digit), _p(out)))
+        return out
+
+    def density_correlation(self, digit: int, traj0: int = 0, count: int | None = None) -> np.ndarray:
+        """``Tr(n_i n_j rho_b)`` with ``n_k = |digit><digit|_k``, ``[count, N, N]``."""
+        count = self._count(traj0, count)
+        out = np.empty((count, self.n, self.n), dtype=np.float64)
+        check(lib.pb200_density_correlation(self.plan._handle, traj0, count, int(digit), _p(out)))
+        return out
+
+    def density_expect(self, terms, traj0: int = 0, count: int | None = None) -> np.ndarray:
+        """``Tr(O rho_b)`` (complex) of an operator given as monomial terms (``pulser_b200.opterms.OpTerms``)."""
+        count = self._count(traj0, count)
+        if (terms.n, terms.d) != (self.n, self.plan.dim):
+            raise ValueError(f"operator on {terms.n} qudits of dimension {terms.d}, the plan holds {self.n} of "
+                             f"{self.plan.dim}")
+        out = np.empty((count, 2), dtype=np.float64)
+        check(lib.pb200_density_expect(self.plan._handle, traj0, count, C.byref(terms.c_desc()), _p(out)))
+        return out[:, 0] + 1j * out[:, 1]
+
+    def density_energy(self, ham_plan: DevicePlan, t_us: float, traj0: int = 0,
+                       count: int | None = None) -> tuple[np.ndarray, np.ndarray]:
+        """``(Tr(H rho_b), Tr(H^2 rho_b))`` with ``H = H(t_us)`` of the single-state plan ``ham_plan``."""
+        count = self._count(traj0, count)
+        e = np.empty(count, dtype=np.float64)
+        e2 = np.empty(count, dtype=np.float64)
+        check(lib.pb200_density_energy(self.plan._handle, ham_plan._handle, float(t_us), traj0, count, _p(e), _p(e2)))
+        return e, e2
+
+    def density_overlap(self, phi: np.ndarray, traj0: int = 0, count: int | None = None) -> np.ndarray:
+        """``<phi|rho_b|phi>`` (complex) for a host ket ``phi`` of D amplitudes."""
+        count = self._count(traj0, count)
+        v = np.ascontiguousarray(np.asarray(phi, dtype=np.complex128).reshape(-1))
+        if v.shape[0] != self.D:
+            raise ValueError(f"state of length {v.shape[0]}, expected {self.D}")
+        out = np.empty((count, 2), dtype=np.float64)
+        check(lib.pb200_density_overlap(self.plan._handle, traj0, count, _p(v.view(np.float64)), _p(out)))
+        return out[:, 0] + 1j * out[:, 1]
+
+    def density_sample(self, n_samples: int, one_state: str, traj: int = 0) -> "Counter[str]":
+        """Bitstring shots from ``diag rho`` drawn on the device with the uniforms of the global ``np.random`` stream
+        (the recipe of ``DevicePlan.sample``)."""
+        from collections import Counter
+
+        u = np.ascontiguousarray(np.random.rand(n_samples), dtype=np.float64)
+        idx = np.empty(n_samples, dtype=np.int64)
+        check(lib.pb200_density_sample(self.plan._handle, traj, self.specs[0].eigenbasis.index(one_state), _p(u),
+                                       n_samples, idx.ctypes.data_as(C.POINTER(C.c_int64))))
+        return Counter(np.binary_repr(int(i), self.n) for i in idx)
