@@ -433,6 +433,13 @@ int pb200_host_taylor_shapes(const double* coef, const double* det,
  * |H_j| <= m[j] (j = 0..p): smallest K with remainder bound *tail_out <= tol. */
 int pb200_host_taylor_order(double h, const double* m, int32_t p, double tol,
                             int32_t* order_out, double* tail_out);
+/* First order k_lo of such a step of K orders whose outputs may be stored in
+ * single precision (g_stored: the step stores G_k = X chi_k as well): the
+ * smallest k_lo whose bound on the rounding's effect on psi(a+h),
+ * *bound_out, is <= tol (K when none is). */
+int pb200_host_taylor_lowprec(double h, const double* m, int32_t p, int32_t K,
+                              int32_t g_stored, double tol, int32_t* k_lo_out,
+                              double* bound_out);
 /* Chebyshev coefficients a_j of exp(-i*rho*x) on [-1,1], truncated at tol:
  * writes up to cap (re,im) pairs, returns the count through *count. */
 int pb200_host_chebyshev(double rho, double tol, double* out, int32_t cap,

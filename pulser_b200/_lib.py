@@ -161,6 +161,8 @@ def _load() -> C.CDLL:
             C.c_int, [dp, dp, C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.POINTER(C.c_int32), dp, dp, dp]),
         "pb200_host_taylor_order": (
             C.c_int, [C.c_double, dp, C.c_int32, C.c_double, C.POINTER(C.c_int32), dp]),
+        "pb200_host_taylor_lowprec": (
+            C.c_int, [C.c_double, dp, C.c_int32, C.c_int32, C.c_int32, C.c_double, C.POINTER(C.c_int32), dp]),
     }
     for name, (res, args) in sig.items():
         fn = getattr(lib, name)  # AttributeError if the symbol is missing
@@ -177,7 +179,8 @@ EXPORTED_SYMBOLS = [
     "pb200_state_get", "pb200_state_probabilities", "pb200_state_norm2",
     "pb200_state_occupation", "pb200_state_correlation", "pb200_state_energy", "pb200_state_overlap", "pb200_state_expect", "pb200_state_sample", "pb200_state_copy", "pb200_state_device_ptr", "pb200_propagate", "pb200_apply_h",
     "pb200_coefficients_at", "pb200_bench_apply", "pb200_host_interpolate",
-    "pb200_host_moments", "pb200_host_chebyshev", "pb200_host_taylor_fit", "pb200_host_taylor_order", "pb200_host_taylor_separable",
+    "pb200_host_moments", "pb200_host_chebyshev", "pb200_host_taylor_fit", "pb200_host_taylor_order", "pb200_host_taylor_lowprec",
+    "pb200_host_taylor_separable",
     "pb200_host_taylor_shapes",
     "pb200_plan_create_shard", "pb200_shards_link", "pb200_shards_propagate", "pb200_shards_apply_h", "pb200_shards_energy",
     "pb200_shards_expect",

@@ -104,6 +104,22 @@ __device__ __forceinline__ void st_c2_evict_last(c2* p, c2 v) {
     asm("createpolicy.fractional.L2::evict_last.b64 %0, 1.0;" : "=l"(pol));
     asm volatile("st.global.L2::cache_hint.v2.f64 [%0], {%1, %2}, %3;" ::"l"(p), "d"(v.x), "d"(v.y), "l"(pol) : "memory");
 }
+// single-precision copies of an amplitude (the tail orders of a Taylor step): 8-byte stores, rounded to nearest
+__device__ __forceinline__ void st_c2(float2* p, c2 v) { *p = make_float2((float)v.x, (float)v.y); }
+__device__ __forceinline__ void st_c2_evict_last(float2* p, c2 v) {
+    uint64_t pol;
+    asm("createpolicy.fractional.L2::evict_last.b64 %0, 1.0;" : "=l"(pol));
+    asm volatile("st.global.L2::cache_hint.v2.f32 [%0], {%1, %2}, %3;" ::"l"(p), "f"((float)v.x), "f"((float)v.y), "l"(pol)
+                 : "memory");
+}
+// an amplitude of a tile in shared memory or a gathered partner, in either precision, widened to fp64
+__device__ __forceinline__ c2 tile_c2(const c2& t) { return t; }
+__device__ __forceinline__ c2 tile_c2(const float2& t) { return {(double)t.x, (double)t.y}; }
+__device__ __forceinline__ double2 ld_partner(const c2* p) { return __ldg(reinterpret_cast<const double2*>(p)); }
+__device__ __forceinline__ double2 ld_partner(const float2* p) {
+    const float2 r = __ldg(p);
+    return make_double2((double)r.x, (double)r.y);
+}
 
 // Fused Lanczos step (StageArgs::lz set).  The gather source `v` holds the RAW vector r_j = G v_j - beta_{j-1} v_{j-1}
 // of the previous stage; alpha_j = Re<v_j, r_j> and |r_j|^2 were reduced by that stage into lz.acc_prev.  This stage
@@ -312,6 +328,10 @@ __device__ __forceinline__ c2 ld_own(const c2* p) {
     double2 r = __ldcs(reinterpret_cast<const double2*>(p));
     return {r.x, r.y};
 }
+__device__ __forceinline__ c2 ld_own(const float2* p) {
+    const float2 r = __ldcs(p);
+    return {(double)r.x, (double)r.y};
+}
 
 // one partner of a complex-drive Taylor stage: z = f chi (f = gx + i gy, the factor of the partner's transition),
 // p += z, q += sg z
@@ -326,9 +346,10 @@ __device__ __forceinline__ void taylor_signed_add(double gx, double gy, double s
 // register-block bits (tile bits TBITS-RB .. TBITS-1) are register moves, flips of the tile bits
 // [jstart, TBITS-RB) are independent LDS.128 from `tile`.
 // SIGNED (per-bit table only): q also receives the signed sum  sum_k sg_k f_k chi_k,  sg_k = +1 where the amplitude's bit
-// k is to_bit, with f_k the factor p receives (the complex-drive Taylor stage).
-template <bool UNIFORM, bool REAL_G, int TBITS, int RB, bool SIGNED = false>
-__device__ __forceinline__ void rb_tile_gather(const PassGeom& g, const c2* tile, const double* __restrict__ tab, int tid,
+// k is to_bit, with f_k the factor p receives (the complex-drive Taylor stage).  T: c2, or float2 for a single-precision
+// tile (LDS.64).
+template <bool UNIFORM, bool REAL_G, int TBITS, int RB, bool SIGNED = false, class T = c2>
+__device__ __forceinline__ void rb_tile_gather(const PassGeom& g, const T* tile, const double* __restrict__ tab, int tid,
                                                int to_bit, int jstart, bool skip_smem, const c2 (&v)[1 << RB],
                                                double (&pr)[1 << RB], double (&pi)[1 << RB], double (&qr)[1 << RB],
                                                double (&qi)[1 << RB]) {
@@ -378,7 +399,7 @@ __device__ __forceinline__ void rb_tile_gather(const PassGeom& g, const c2* tile
             const double sg = (bit == to_bit) ? 1.0 : -1.0;
 #pragma unroll
             for (int r = 0; r < R; ++r) {
-                const c2 pv = tile[ptid + r * NT];
+                const c2 pv = tile_c2(tile[ptid + r * NT]);
                 if (UNIFORM) {
                     pr[r] += pv.x; pi[r] += pv.y;
                     if (!REAL_G) { qr[r] = fma(sg, pv.x, qr[r]); qi[r] = fma(sg, pv.y, qi[r]); }
@@ -816,6 +837,10 @@ struct TaylorArgs {
     int acc_add_h;     // 1: chi_{k-1} (history term hchi[0]) joins the update as well
     int acc_on;        // 0: this order leaves the accumulator alone
     c2 acc_mul;        // factor of the whole accumulator (phase of the scalar centre on the last order, else 1)
+    // precision of the order (TaylorStep::k_lo): chi_k (v) is single precision (float2 in the slot), chi_{k+1} and G_k
+    // are stored so; bit j - 1 of hchi32 / hg32: chi_{k-j} / G_{k-j} is single precision
+    int src32, out32;
+    unsigned hchi32, hg32;
     // state-vector shards (stage_d2_taylor_kernel<..., SHARD = true>): the top shard_bits qubits of the global index
     // select the shard, every other operand is this shard's slice of 2^(N - shard_bits) amplitudes.  peer[q] = chi_k
     // of shard (shard ^ 1 << q): a flip of shard bit q leaves the local index unchanged
@@ -848,8 +873,9 @@ struct TaylorArgs {
 // dint(r) is the interaction diagonal of amplitude r.  v is consumed: with acc_add_h, chi_{k-1} is added into it once the
 // diagonal term no longer needs it, so the accumulator update reads no extra operand.
 // CPLX: (qx, qy) is G' of the complex-drive step.  DISS: (ex, ey) = i D chi_k, added to the sum that -i h / (k+1) scales.
-template <int R, int H = (R >= 4) ? R / 2 : R, bool SHARD = false, bool CPLX = false, bool DISS = false, class Off,
-          class Dint>
+// HIST32: a history operand may be single precision (TaylorArgs::hchi32, hg32); OUT32: chi_{k+1} and G_k are stored so.
+template <int R, int H = (R >= 4) ? R / 2 : R, bool SHARD = false, bool CPLX = false, bool DISS = false,
+          bool HIST32 = false, bool OUT32 = false, class Off, class Dint>
 __device__ __forceinline__ void taylor_epilogue(const TaylorArgs& a, const long long (&idx)[R], c2 (&v)[R],
                                                 const double (&gx)[R], const double (&gy)[R], const Off& off,
                                                 long long voff, const Dint& dint,
@@ -881,8 +907,14 @@ __device__ __forceinline__ void taylor_epilogue(const TaylorArgs& a, const long 
         for (int j = 0; j < a.nh; ++j) {
             if (a.hchi[j]) {
                 c2 c[H];
+                if (HIST32 && ((a.hchi32 >> j) & 1)) {
+                    const float2* src = reinterpret_cast<const float2*>(a.hchi[j]) + voff;
 #pragma unroll
-                for (int r = 0; r < H; ++r) c[r] = ld_own(a.hchi[j] + voff + idx[h0 + r]);
+                    for (int r = 0; r < H; ++r) c[r] = ld_own(src + idx[h0 + r]);
+                } else {
+#pragma unroll
+                    for (int r = 0; r < H; ++r) c[r] = ld_own(a.hchi[j] + voff + idx[h0 + r]);
+                }
 #pragma unroll
                 for (int r = 0; r < H; ++r) {
                     double d;
@@ -894,8 +926,14 @@ __device__ __forceinline__ void taylor_epilogue(const TaylorArgs& a, const long 
             }
             if (a.hg[j]) {
                 c2 c[H];
+                if (HIST32 && ((a.hg32 >> j) & 1)) {
+                    const float2* src = reinterpret_cast<const float2*>(a.hg[j]) + voff;
 #pragma unroll
-                for (int r = 0; r < H; ++r) c[r] = ld_own(a.hg[j] + voff + idx[h0 + r]);
+                    for (int r = 0; r < H; ++r) c[r] = ld_own(src + idx[h0 + r]);
+                } else {
+#pragma unroll
+                    for (int r = 0; r < H; ++r) c[r] = ld_own(a.hg[j] + voff + idx[h0 + r]);
+                }
 #pragma unroll
                 for (int r = 0; r < H; ++r) { sx[r] = fma(a.hom[j], c[r].x, sx[r]); sy[r] = fma(a.hom[j], c[r].y, sy[r]); }
             }
@@ -915,8 +953,13 @@ __device__ __forceinline__ void taylor_epilogue(const TaylorArgs& a, const long 
             res[r] = {a.scale.x * sx[r] - a.scale.y * sy[r], a.scale.x * sy[r] + a.scale.y * sx[r]};
             // chi_{k+1} is the next order's gather source: kept in L2 ahead of the ring buffers read once per order
             // (C2 on H100: the ring is twice the 50 MB L2; 42.9 against 44.1 us per order, DESIGN.md section 8)
-            st_c2_evict_last(a.out + voff + idx[h0 + r], res[r]);
-            if (a.g_out) st_c2(a.g_out + voff + idx[h0 + r], c2{gx[h0 + r], gy[h0 + r]});
+            if constexpr (OUT32) {
+                st_c2_evict_last(reinterpret_cast<float2*>(a.out) + voff + idx[h0 + r], res[r]);
+                if (a.g_out) st_c2(reinterpret_cast<float2*>(a.g_out) + voff + idx[h0 + r], c2{gx[h0 + r], gy[h0 + r]});
+            } else {
+                st_c2_evict_last(a.out + voff + idx[h0 + r], res[r]);
+                if (a.g_out) st_c2(a.g_out + voff + idx[h0 + r], c2{gx[h0 + r], gy[h0 + r]});
+            }
             if constexpr (CPLX) { if (a.g2_out) st_c2(a.g2_out + voff + idx[h0 + r], c2{qx[h0 + r], qy[h0 + r]}); }
         }
         if (a.acc_on) {
@@ -1056,8 +1099,11 @@ __device__ __forceinline__ void taylor_dint_setup(const TaylorArgs& a, long long
 // drive -conj(omega)).  The dissipator sum of a chunk is a second accumulator, which does not fit in 128 registers
 // either: the same launch shape as CPLX.  A pair whose row bit lies in the tile reads its both-flip partner from shared
 // memory, one above the tile costs one more coalesced load per atom.
+// SRC32 / OUT32: the tail orders of a step (TaylorStep::k_lo), uniform drives of one state (or its shards) only.  chi_k (tile and
+// partners) is read as float2, chi_{k+1} and G_k are stored as float2; the arithmetic, the partner sums and the
+// accumulator stay fp64.  The single-precision tile fills the first 64 KiB of the tile's 128.
 template <bool UNIFORM, bool REAL_G, int TBITS, int RB, bool SHARD = false, int NS = (UNIFORM ? 0 : 1), bool CPLX = false,
-          bool DISS = false>
+          bool DISS = false, bool SRC32 = false, bool OUT32 = false>
 __global__ void __launch_bounds__(1 << (TBITS - RB),
                                   (CPLX || DISS) ? 1 : (65536 / ((1 << (TBITS - RB)) * (RB >= 3 ? 128 : 64))))
 stage_d2_taylor_kernel(const __grid_constant__ TaylorArgs a) {
@@ -1066,6 +1112,9 @@ stage_d2_taylor_kernel(const __grid_constant__ TaylorArgs a) {
     static_assert(NS == (UNIFORM ? 0 : 1) || NS == PB200_TAYLOR_SMAX, "one-shape table, or PB200_TAYLOR_SMAX shapes");
     static_assert(!CPLX || !REAL_G, "a complex drive gathers through the per-bit table");
     static_assert(!DISS || (!UNIFORM && !SHARD && !CPLX), "a density matrix runs the batch gather, one device, one phase");
+    static_assert(!(SRC32 || OUT32) || (UNIFORM && NS == 0 && !CPLX && !DISS),
+                  "single-precision orders: one state, a uniform drive of one phase");
+    using TT = std::conditional_t<SRC32, float2, c2>;   // element of chi_k
     constexpr bool SHAPES = NS == PB200_TAYLOR_SMAX;
     constexpr int NT = 1 << (TBITS - RB);
     constexpr int TSIZE = 1 << TBITS;
@@ -1077,18 +1126,18 @@ stage_d2_taylor_kernel(const __grid_constant__ TaylorArgs a) {
     // accumulators per amplitude instead of the P and Q sums)
     constexpr bool TAB = !(UNIFORM && REAL_G);
     extern __shared__ __align__(128) unsigned char smem_raw[];
-    c2* tile = reinterpret_cast<c2*>(smem_raw);
+    TT* tile = reinterpret_cast<TT*>(smem_raw);
     __shared__ __align__(8) uint64_t mbar;
     const PassGeom& g = a.geo;
     const int tid = threadIdx.x;
     const long long traj = UNIFORM ? 0 : (long long)blockIdx.y;
     const long long voff = traj * a.D;
     const long long base = (long long)blockIdx.x << TBITS;
-    const c2* vsrc = a.v + voff;
+    const TT* vsrc = reinterpret_cast<const TT*>(a.v) + voff;
 
     if (tid == 0) mbar_init(&mbar, 1);
     __syncthreads();
-    double* dsm = reinterpret_cast<double*>(tile + TSIZE);   // taylor_dint_setup
+    double* dsm = reinterpret_cast<double*>(smem_raw + (size_t)TSIZE * sizeof(c2));   // taylor_dint_setup
     const double* ts = dsm + TBITS * TBITS + TBITS + 1;
     const double* xt = ts + (1 << RB);
     double* tab = dsm + taylor_dint_doubles(TBITS, RB) + g.n_bits * g.n_bits;
@@ -1101,8 +1150,8 @@ stage_d2_taylor_kernel(const __grid_constant__ TaylorArgs a) {
     pdl_wait();
     pdl_launch_dependents();
     if (tid == 0) {
-        mbar_arrive_expect_tx(&mbar, (uint32_t)TSIZE * 16u);
-        tma_load_1d(tile, vsrc + base, (uint32_t)TSIZE * 16u, &mbar);
+        mbar_arrive_expect_tx(&mbar, (uint32_t)(TSIZE * sizeof(TT)));
+        tma_load_1d(tile, vsrc + base, (uint32_t)(TSIZE * sizeof(TT)), &mbar);
     }
     // SHAPES, for J = 0 (order-0 coefficients m0) and J = 1 + history j (hm[s][j]) up to nh, behind the per-bit table:
     //   bl[J][i]   = sum_s m_{s,J} x (shape s's weights of the register bits i, relative to i = 0), the same for all
@@ -1179,10 +1228,10 @@ stage_d2_taylor_kernel(const __grid_constant__ TaylorArgs a) {
             const int bit = (int)((base >> p) & 1);
             double gx = 0.0, gy = 0.0;
             if (TAB) { gx = tab[2 * p]; gy = (bit == to_bit) ? tab[2 * p + 1] : -tab[2 * p + 1]; }
-            const c2* src = vsrc + (i0 ^ (1LL << p));
+            const TT* src = vsrc + (i0 ^ (1LL << p));
             double2 raw[RC];
 #pragma unroll
-            for (int r = 0; r < RC; ++r) raw[r] = __ldg(reinterpret_cast<const double2*>(src + r * NT));
+            for (int r = 0; r < RC; ++r) raw[r] = ld_partner(src + r * NT);
 #pragma unroll
             for (int r = 0; r < RC; ++r) {
                 if constexpr (CPLX) {
@@ -1205,10 +1254,13 @@ stage_d2_taylor_kernel(const __grid_constant__ TaylorArgs a) {
                     const int p = nb - a.shard_bits + q;
                     gx = tab[2 * p]; gy = (bit == to_bit) ? tab[2 * p + 1] : -tab[2 * p + 1];
                 }
-                const c2* src = a.peer[q] + i0;
+                const TT* src = reinterpret_cast<const TT*>(a.peer[q]) + i0;
                 double2 raw[RC];
 #pragma unroll
-                for (int r = 0; r < RC; ++r) raw[r] = *reinterpret_cast<const double2*>(src + r * NT);
+                for (int r = 0; r < RC; ++r) {
+                    if constexpr (SRC32) raw[r] = make_double2((double)src[r * NT].x, (double)src[r * NT].y);
+                    else raw[r] = *reinterpret_cast<const double2*>(src + r * NT);
+                }
 #pragma unroll
                 for (int r = 0; r < RC; ++r) {
                     if constexpr (CPLX) {
@@ -1232,11 +1284,11 @@ stage_d2_taylor_kernel(const __grid_constant__ TaylorArgs a) {
                 if ((m >> q) & 1) d += xt[(q + 1) * NT + tid];
             return d;
         };
-        const c2* sub = tile + (c << STB);
+        const TT* sub = tile + (c << STB);
         c2 v[RC];
         double qd[RC];   // the Q sums of rb_tile_gather: not used by the two instantiations below
 #pragma unroll
-        for (int r = 0; r < RC; ++r) v[r] = sub[tid + r * NT];
+        for (int r = 0; r < RC; ++r) v[r] = tile_c2(sub[tid + r * NT]);
         if constexpr (CPLX) rb_tile_gather<false, false, STB, 3, true>(g, sub, tab, tid, to_bit, 0, false, v, pr, pi, dr, di);
         else rb_tile_gather<!TAB, !TAB, STB, 3>(g, sub, tab, tid, to_bit, 0, false, v, pr, pi, qd, qd);
 #pragma unroll
@@ -1245,10 +1297,10 @@ stage_d2_taylor_kernel(const __grid_constant__ TaylorArgs a) {
             const int bit = (c >> q) & 1;
             double gx = 0.0, gy = 0.0;
             if (TAB) { gx = tab[2 * p]; gy = (bit == to_bit) ? tab[2 * p + 1] : -tab[2 * p + 1]; }
-            const c2* other = tile + ((c ^ (1 << q)) << STB);
+            const TT* other = tile + ((c ^ (1 << q)) << STB);
 #pragma unroll
             for (int r = 0; r < RC; ++r) {
-                const c2 pv = other[tid + r * NT];
+                const c2 pv = tile_c2(other[tid + r * NT]);
                 if constexpr (CPLX) {
                     taylor_signed_add(gx, gy, bit == to_bit ? 1.0 : -1.0, pv.x, pv.y, pr[r], pi[r], dr[r], di[r]);
                 } else if (!TAB) {
@@ -1293,12 +1345,12 @@ stage_d2_taylor_kernel(const __grid_constant__ TaylorArgs a) {
                     if (pr < TBITS) {
 #pragma unroll
                         for (int r = 0; r < RC; ++r) {
-                            const c2 t = tile[(tpos + r * NT) ^ (int)mask];
+                            const c2 t = tile_c2(tile[(tpos + r * NT) ^ (int)mask]);
                             pv[r] = make_double2(t.x, t.y);
                         }
                     } else {
 #pragma unroll
-                        for (int r = 0; r < RC; ++r) pv[r] = __ldg(reinterpret_cast<const double2*>(vsrc + (idx[r] ^ mask)));
+                        for (int r = 0; r < RC; ++r) pv[r] = ld_partner(vsrc + (idx[r] ^ mask));
                     }
 #pragma unroll
                     for (int r = 0; r < RC; ++r) taylor_diss_flip(a, idx[r], pr, pc, pv[r], dx[r], dy[r]);
@@ -1327,8 +1379,8 @@ stage_d2_taylor_kernel(const __grid_constant__ TaylorArgs a) {
                 a, idx, v, pr, pi, [&](int r, int J) { return lt[J * NT] + lc[(J << RB) + r]; }, voff, dint, nullptr,
                 nullptr, ex, ey);
         } else {
-            taylor_epilogue<RC, UNIFORM ? RC / 2 : RC / 4, SHARD, false, DISS>(a, idx, v, pr, pi, off, voff, dint, nullptr,
-                                                                             nullptr, ex, ey);
+            taylor_epilogue<RC, UNIFORM ? RC / 2 : RC / 4, SHARD, false, DISS, SRC32, OUT32>(a, idx, v, pr, pi, off, voff,
+                                                                                           dint, nullptr, nullptr, ex, ey);
         }
     }
 }

@@ -236,6 +236,7 @@ struct TaylorVariant {
     TaylorSmem smem;
     bool pdl;
     bool diss = false;   // master equation (TaylorArgs::n_pair > 0)
+    bool src32 = false, out32 = false;   // single-precision chi_k / chi_{k+1} and G_k (TaylorArgs::src32, out32)
 };
 
 static const std::vector<TaylorVariant>& taylor_variants() {
@@ -245,6 +246,15 @@ static const std::vector<TaylorVariant>& taylor_variants() {
         // one state, one drive coefficient (C2, C5)
         {true,  true,  false, 0,  false, stage_d2_taylor_kernel<true, true, TB, RB, false, 0, false>,     RB,  S::Tile,      true},
         {true,  false, false, 0,  false, stage_d2_taylor_kernel<true, false, TB, RB, false, 0, false>,    RB,  S::TileTable, true},
+        // ... the tail orders of their steps in single precision: the order at k_lo (fp64 -> fp32) and those after it
+        {true,  true,  false, 0,  false, stage_d2_taylor_kernel<true, true, TB, RB, false, 0, false, false, false, true>,
+         RB, S::Tile, true, false, false, true},
+        {true,  true,  false, 0,  false, stage_d2_taylor_kernel<true, true, TB, RB, false, 0, false, false, true, true>,
+         RB, S::Tile, true, false, true, true},
+        {true,  false, false, 0,  false, stage_d2_taylor_kernel<true, false, TB, RB, false, 0, false, false, false, true>,
+         RB, S::TileTable, true, false, false, true},
+        {true,  false, false, 0,  false, stage_d2_taylor_kernel<true, false, TB, RB, false, 0, false, false, true, true>,
+         RB, S::TileTable, true, false, true, true},
         // trajectory batch, per-qubit factors of one detuning shape (C4)
         {false, false, false, 1,  false, stage_d2_taylor_kernel<false, false, TB, RB, false, 1, false>,   RB,  S::TileTable, true},
         // several detuning shapes: one state (detuning maps), batches
@@ -254,6 +264,14 @@ static const std::vector<TaylorVariant>& taylor_variants() {
         // state-vector shards
         {true,  true,  true,  0,  false, stage_d2_taylor_kernel<true, true, TB, RB, true, 0, false>,      RB,  S::Tile,      false},
         {true,  false, true,  0,  false, stage_d2_taylor_kernel<true, false, TB, RB, true, 0, false>,     RB,  S::TileTable, false},
+        {true,  true,  true,  0,  false, stage_d2_taylor_kernel<true, true, TB, RB, true, 0, false, false, false, true>,
+         RB, S::Tile, false, false, false, true},
+        {true,  true,  true,  0,  false, stage_d2_taylor_kernel<true, true, TB, RB, true, 0, false, false, true, true>,
+         RB, S::Tile, false, false, true, true},
+        {true,  false, true,  0,  false, stage_d2_taylor_kernel<true, false, TB, RB, true, 0, false, false, false, true>,
+         RB, S::TileTable, false, false, false, true},
+        {true,  false, true,  0,  false, stage_d2_taylor_kernel<true, false, TB, RB, true, 0, false, false, true, true>,
+         RB, S::TileTable, false, false, true, true},
         {true,  true,  true,  SM, false, stage_d2_taylor_kernel<true, true, TB, RB, true, SM, false>,     RB,  S::Shapes,    false},
         {true,  false, true,  SM, false, stage_d2_taylor_kernel<true, false, TB, RB, true, SM, false>,    RB,  S::Shapes,    false},
         // complex drive: the phase moves inside the step
@@ -2423,6 +2441,49 @@ static int taylor_order(double h, const std::vector<double>& mj, double tol, dou
     return std::max(kk, 1);
 }
 
+// First order k_lo of a K-order step that stores its outputs (chi_{k+1}, and G_k with g_stored) in single precision:
+// the orders k >= k_lo.  A stored chi_j carries at most u32 |chi_j| <= u32 y_j of rounding, which reaches psi(1) once
+// through the accumulator and again through every later order: with S_j = sum_{k=j..K} z_k of the same majorant
+// recurrence started from a unit impulse at order j, at most u32 y_j S_j.  A stored G_j = X chi_j is only read by the
+// history terms om_i G_j of the later orders, whose coefficients |om_i| |X| are part of m_i, so its rounding costs at
+// most u32 y_j (S_j - 1).  Returns the smallest k_lo whose summed bound (*bound_out) is <= tol; K when none is.
+static int taylor_lowprec_order(double h, const std::vector<double>& mj, int K, bool g_stored, double tol,
+                                double& bound_out) {
+    constexpr double u32 = 5.9604644775390625e-08;   // 2^-24
+    const int p = (int)mj.size() - 1;
+    std::vector<double> y(K + 1, 0.0), S(K + 1, 0.0), z(K + 1);
+    y[0] = 1.0;
+    for (int k = 0; k < K; ++k) {
+        double s = 0.0;
+        for (int j = 0; j <= std::min(p, k); ++j) s += mj[j] * y[k - j];
+        y[k + 1] = h * s / (k + 1);
+    }
+    for (int j = 1; j <= K; ++j) {
+        std::fill(z.begin(), z.end(), 0.0);
+        z[j] = 1.0;
+        double sum = 1.0;
+        for (int k = j; k < K; ++k) {
+            double s = 0.0;
+            for (int i = 0; i <= std::min(p, k - j); ++i) s += mj[i] * z[k - i];
+            z[k + 1] = h * s / (k + 1);
+            sum += z[k + 1];
+        }
+        S[j] = sum;
+    }
+    // cost(L): chi_j for j = L+1 .. K, G_j for j = L .. K-2 (the last order stores no G)
+    double bound = 0.0;
+    int k_lo = K;
+    for (int L = K - 1; L >= 0; --L) {
+        double add = u32 * y[L + 1] * S[L + 1];
+        if (g_stored && L <= K - 2) add += u32 * y[L] * (S[L] - 1.0);
+        if (bound + add > tol) break;
+        bound += add;
+        k_lo = L;
+    }
+    bound_out = bound;
+    return k_lo;
+}
+
 // One order of a Taylor step: the tiled variant that the plan and the arguments select, or the plain kernel of small
 // registers (!tiled).  cplx: a step whose drive phase moves inside it
 static void launch_taylor_order(const Plan& P, bool tiled, const TaylorArgs& a, bool cplx) {
@@ -2442,14 +2503,14 @@ static void launch_taylor_order(const Plan& P, bool tiled, const TaylorArgs& a, 
     const int ns = a.tab_shapes ? PB200_TAYLOR_SMAX : uniform ? 0 : 1;
     for (const TaylorVariant& v : taylor_variants()) {
         if (v.uniform != uniform || v.real_g != real_g || v.shard != shard || v.ns != ns || v.cplx != cplx ||
-            v.diss != diss)
+            v.diss != diss || v.src32 != (a.src32 != 0) || v.out32 != (a.out32 != 0))
             continue;
         launch_k(v.kernel, dim3((unsigned)(P.D >> kTaylorTileBits), uniform ? 1u : (unsigned)P.B),
                  dim3(1u << (kTaylorTileBits - v.rb)), taylor_variant_smem(v, P.n), P.stream, v.pdl, a);
         return;
     }
-    fail(PB200_ERR_UNSUPPORTED, "no Taylor stage kernel for UNIFORM=%d REAL_G=%d SHARD=%d NS=%d CPLX=%d DISS=%d", uniform,
-         real_g, shard, ns, cplx, diss);
+    fail(PB200_ERR_UNSUPPORTED, "no Taylor stage kernel for UNIFORM=%d REAL_G=%d SHARD=%d NS=%d CPLX=%d DISS=%d SRC32=%d OUT32=%d",
+         uniform, real_g, shard, ns, cplx, diss, a.src32, a.out32);
 }
 
 // Geometry of the Taylor stage on the 2^L amplitudes a plan holds (L = N, or N - shard_bits on a shard): the
@@ -2475,6 +2536,7 @@ struct TaylorStep {
     int p_om = 0, p_th = 0, p = 0;
     std::vector<double> gam;         // centres of H_j
     int K = 0;
+    int k_lo = 0;                    // orders k >= k_lo store chi_{k+1} and G_k in single precision (K: none)
     double phi = 0.0;                // phase of the scalar centre over the step
     int n_chi = 0, n_g = 0;          // chi ring (slot 0 = the current state), G ring (and G' ring of a complex step)
     // drive of the step: 0 real along the plan's unit; 1 real along its own unit (one phase over the step, the existing
@@ -2495,6 +2557,7 @@ struct TaylorScheduler {
     double t, steps_len = 0.0, t_retry_len = 0.0, A_sum, C_sum[PB200_TAYLOR_SMAX], kRoundUnit = 0.05 * 1.1102230246251565e-16;
     int order, N, nt, ns;
     bool log_steps;
+    bool lowprec;   // the plan (or its shards) has single-precision stage kernels for its real-drive steps
     pb200_run_stats st{};
     struct Fit { TaylorPoly om, omi, th, m[PB200_TAYLOR_SMAX]; double om_allow = 0.0; bool ok; };
 
@@ -2527,6 +2590,9 @@ struct TaylorScheduler {
         // The fit error is budgeted over the call: 50 % of its share of the tolerance (10 % goes to the Taylor remainders).
         fit_total = 0.5 * rate * (t_stop - t_start);
         log_steps = env_int("PB200_TAYLOR_LOG", 0) != 0;
+        PassGeom geo;
+        bool tiled = false;
+        lowprec = taylor_geometry(P, geo, tiled) && tiled && C.uniform;
     }
 
     // fit of both coefficient functions on [a, a+h] with the smallest degrees that meet the residual budget.
@@ -2692,18 +2758,20 @@ struct TaylorScheduler {
 
     // the order of step s, its log line and its share of the error estimate; rho = h sum_j m_j / (j + 1)
     void record(TaylorStep& s, const Fit& F, const std::vector<double>& mj, int p_m, double om_resid, double rho) {
-        double trunc_bound = 0.0;
+        double trunc_bound = 0.0, round32 = 0.0;
         s.K = taylor_order(s.h, mj, std::max(1e-15, 0.1 * rate * s.h), trunc_bound);
+        // the tail orders in single precision: another 10 % of the step's share of the tolerance
+        s.k_lo = (lowprec && s.drive != 2) ? taylor_lowprec_order(s.h, mj, s.K, s.n_g > 0, 0.1 * rate * s.h, round32) : s.K;
         st.n_applies += s.K; st.n_exponentials += 1; ++st.n_steps;
         if (log_steps)
-            fprintf(stderr, "taylor step t=%.6f h_ns=%.3f p_om=%d p_th=%d p_m=%d K=%d ring=%d rho=%.3f resid=%.2e/%.2e/%.2e drive=%s\n",
+            fprintf(stderr, "taylor step t=%.6f h_ns=%.3f p_om=%d p_th=%d p_m=%d K=%d ring=%d rho=%.3f resid=%.2e/%.2e/%.2e drive=%s k_lo=%d\n",
                     s.t, s.h * 1e3, s.p_om, s.p_th, p_m, s.K, s.ring() + 1, mj[0] * s.h, om_resid, F.th.resid, F.m[0].resid,
-                    s.drive == 2 ? "cplx" : s.drive == 1 ? "rot" : "real");
+                    s.drive == 2 ? "cplx" : s.drive == 1 ? "rot" : "real", s.k_lo);
         st.max_rho = std::max(st.max_rho, rho);
         double fit_m = 0.0;
         for (int q = 0; q < ns; ++q) fit_m += C_sum[q] * F.m[q].resid;
         const double fit_err = s.h * (A_sum * om_resid + N * F.th.resid + fit_m);
-        st.err_estimate += trunc_bound + fit_err;
+        st.err_estimate += trunc_bound + round32 + fit_err;
         fit_spent += fit_err;
         { const double r = kRoundUnit * std::exp(std::min(rho, 40.0)); round2 += r * r; }
         steps_len += s.h;
@@ -2834,6 +2902,8 @@ static TaylorArgs taylor_args(const Plan& P, const PassGeom& geo, const TaylorSt
     a.th0 = s.th[0]; a.gam0 = s.gam[0]; a.om0 = s.om[0];
     for (int q = 0; q < PB200_TAYLOR_SMAX; ++q) a.m0[q] = m_c(q, 0);
     a.scale = {0.0, -s.h / (k + 1)};
+    a.src32 = k > s.k_lo;
+    a.out32 = k >= s.k_lo;
     a.nh = std::min(s.p, k);
     for (int j = 1; j <= a.nh; ++j) {
         const double thj = th_c(j), omj = j < (int)s.om.size() ? s.om[j] : 0.0;
@@ -2842,6 +2912,9 @@ static TaylorArgs taylor_args(const Plan& P, const PassGeom& geo, const TaylorSt
         a.hth[j - 1] = thj; a.hgam[j - 1] = s.gam[j]; a.hom[j - 1] = omj;
         a.hchi[j - 1] = (thj != 0.0 || any_m || s.gam[j] != 0.0) ? R.chi[(k - j) % s.n_chi] : nullptr;
         a.hg[j - 1] = (omj != 0.0) ? R.gr[(k - j) % s.n_g] : nullptr;
+        // chi_{k-j} was written by order k-j-1, G_{k-j} by order k-j
+        if (k - j - 1 >= s.k_lo) a.hchi32 |= 1u << (j - 1);
+        if (k - j >= s.k_lo) a.hg32 |= 1u << (j - 1);
         if (s.drive == 2) {
             const double omij = j < (int)s.omi.size() ? s.omi[j] : 0.0;
             a.homi[j - 1] = omij;
@@ -4375,6 +4448,16 @@ int pb200_host_taylor_order(double h, const double* m, int32_t p, double tol, in
     double tail = 0.0;
     *order_out = taylor_order(h, std::vector<double>(m, m + p + 1), tol, tail);
     if (tail_out) *tail_out = tail;
+    PB200_CATCH
+}
+
+int pb200_host_taylor_lowprec(double h, const double* m, int32_t p, int32_t K, int32_t g_stored, double tol,
+                              int32_t* k_lo_out, double* bound_out) {
+    PB200_TRY
+    if (!m || !k_lo_out || p < 0 || p > PB200_TAYLOR_PMAX || K < 1) fail(PB200_ERR_INVALID, "bad argument");
+    double bound = 0.0;
+    *k_lo_out = taylor_lowprec_order(h, std::vector<double>(m, m + p + 1), K, g_stored != 0, tol, bound);
+    if (bound_out) *bound_out = bound;
     PB200_CATCH
 }
 
