@@ -185,7 +185,11 @@ int pb200_plan_set_drive(pb200_plan* plan, int32_t drive, int32_t traj0,
  * row-major, interleaved complex, acting on the (row digit, column digit) pair
  * (k, k + N).  Afterwards pb200_propagate integrates  rho' = -i[H,rho] + D(rho)
  * by symmetric splitting  exp(h/2 D) U(h) exp(h/2 D)  with Richardson
- * extrapolation and the same step controller (order 2 -> 4).  d <= 3. */
+ * extrapolation and the same step controller (order 2 -> 4).  d <= 3.
+ * On a shard of vec(rho) (pb200_plan_create_shard of the 2N-qudit description:
+ * the shard bits are the top row bits) every shard takes the same generators
+ * before pb200_shards_link; pb200_shards_propagate then runs the Taylor
+ * propagator with the dissipator inside the series. */
 int pb200_plan_set_dissipator(pb200_plan* plan, int32_t n_pairs,
                               const double* generators);
 
@@ -286,7 +290,11 @@ int pb200_state_device_ptr(pb200_plan* plan, void** dptr);
  * a master-equation run (default_observables.py:184-561 on a density matrix)
  * without copying rho to the host.  Values are NOT divided by the trace; the
  * caller normalises.  A plan without a dissipator is refused
- * (PB200_ERR_UNSUPPORTED). */
+ * (PB200_ERR_UNSUPPORTED).  On a shard of vec(rho) (one trajectory, holding the
+ * rows [r0, r0 + D / G) of rho) each reduction returns the share of those rows,
+ * read from the shard's own slice: the sum over the G shards is the value of the
+ * whole matrix (pb200_density_sample: the shots of the shard's block of 2^N / G
+ * bitstrings, out = their low N - shard_bits bits, as pb200_state_sample). */
 /* trace[c] = Re Tr rho_{traj0+c} */
 int pb200_density_trace(pb200_plan* plan, int32_t traj0, int32_t count,
                         double* trace);
@@ -297,7 +305,8 @@ int pb200_density_occupation(pb200_plan* plan, int32_t traj0, int32_t count,
 int pb200_density_correlation(pb200_plan* plan, int32_t traj0, int32_t count,
                               int32_t digit, double* corr);
 /* out[c] = Tr(op rho_{traj0+c}) as (re, im), op as in pb200_state_expect;
- * term t reads rho[shift_t(r), r], one element per (term, r). */
+ * term t reads rho[shift_t(r), r], one element per (term, r) (on a shard:
+ * rho[r, shift_t(r)] of its own rows r). */
 int pb200_density_expect(pb200_plan* plan, int32_t traj0, int32_t count,
                          const pb200_op_terms* op, double* out);
 /* energy[c] = Re Tr(H rho_{traj0+c}), h2[c] = Re Tr(H^2 rho_{traj0+c}) with
@@ -305,7 +314,8 @@ int pb200_density_expect(pb200_plan* plan, int32_t traj0, int32_t count,
  * register and basis on the same device (the noiseless Hamiltonian handed to the
  * observables).  Reads the diagonal, the drive transitions and the interaction
  * diagonal of H: O(D (1 + N n_drives)^2) loads, never the whole matrix.  XY
- * registers are refused (PB200_ERR_UNSUPPORTED). */
+ * registers are refused (PB200_ERR_UNSUPPORTED).  A shard sums Tr(rho H) and
+ * Tr(rho H^2) over its own rows, with a `ham` plan on its own device. */
 int pb200_density_energy(pb200_plan* plan, pb200_plan* ham, double t_us,
                          int32_t traj0, int32_t count, double* energy,
                          double* h2);
@@ -358,10 +368,11 @@ int pb200_bench_apply(pb200_plan* plan, double t_us, int32_t reps,
 int pb200_plan_create_shard(pb200_plan** out, const pb200_plan_desc* desc,
                             int32_t shard_bits, int32_t shard_index);
 /* Link the G shards plans[i] = shard i (after their uploads): checks N, sampling
- * times and the Taylor structure (one global drive, of any phase), merges the
- * interaction bounds so that every shard schedules exactly like the unsharded
- * plan, enables peer access between distinct devices (PB200_ERR_UNSUPPORTED
- * where it is impossible). */
+ * times and the Taylor structure (one global drive, of any phase; vec(rho):
+ * one phase, the same dissipator on every shard), merges the interaction bounds
+ * so that every shard schedules exactly like the unsharded plan, enables peer
+ * access between distinct devices (PB200_ERR_UNSUPPORTED where it is
+ * impossible). */
 int pb200_shards_link(pb200_plan** plans, int32_t count);
 /* pb200_propagate of the whole state with the Taylor propagator (integrator 0
  * or 3; options steering the Magnus controller are refused): the schedule is

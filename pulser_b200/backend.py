@@ -624,9 +624,11 @@ class DeviceHamiltonian(B200Operator):
 class B200Config(EmulationConfig[B200State]):
     """``QutipConfig`` mirror (``qutip_config.py:28-192``): same options, plus
 
-    ``devices``: CUDA ordinals of the shards of the state vector (2, 4 or 8 entries; the same ordinal may repeat).
+    ``devices``: CUDA ordinals of the shards of the state (2, 4 or 8 entries; the same ordinal may repeat).
     A noiseless single-state run is then split over ``len(devices)`` plans (``pulser_b200.sharded.ShardedPlan``), so
-    registers larger than one GPU's memory can run.  Default ``None``: one plan on one device.
+    registers larger than one GPU's memory can run; so is the density matrix of a master equation whose noise is
+    dephasing, relaxation, depolarizing or eff_noise only (``pulser_b200.lindblad.ShardedLindbladPlan``), exact where
+    one device would need Monte-Carlo trajectories.  Default ``None``: one plan on one device.
     """
 
     _enforce_expected_kwargs = True
@@ -875,12 +877,13 @@ class B200Backend(EmulatorBackend):
         return (sim._has_collapse_ops() and not sim._use_mcwf() and hasattr(lindblad.LindbladPlan, "density_trace")
                 and sim._hamiltonian_data.basis_data.interaction_type != "XY")
 
-    def _stream_density(self, hplan: Any, atom_order: tuple) -> list[Results]:
+    def _stream_density(self, hplan: Any, atom_order: tuple, devices: list[int] | None = None) -> list[Results]:
         """Master equation: the density matrices of the trajectories (one without stochastic noise) are evolved in
         device batches through the evaluation times, and every observable sees a ``DeviceDensityView`` of its
         trajectory, so no density matrix is stored per evaluation time.  The Hamiltonian handed over is the noiseless
         one (``qutip_backend.py:258-264``).  One ``Results`` per trajectory repetition, like the replay path; within a
-        batch the observables are visited time-major, as in ``_stream_noisy``."""
+        batch the observables are visited time-major, as in ``_stream_noisy``.  ``devices``: the one density matrix
+        is split over these shards (``lindblad.ShardedLindbladPlan``) instead of one ``LindbladPlan``."""
         from . import lindblad
 
         sim, config = self._sim_obj, self._config
@@ -908,7 +911,12 @@ class B200Backend(EmulatorBackend):
             per_traj = [[Results(atom_order=atom_order, total_duration=sim.total_duration_ns) for _ in range(reps)]
                         for _, reps in chunk]
             stats: dict = {}
-            with lindblad.LindbladPlan([s for s, _ in chunk], sim._interp_order, sim._gpu) as plan:
+            specs = [s for s, _ in chunk]
+            if devices is None:
+                plan = lindblad.LindbladPlan(specs, sim._interp_order, sim._gpu)
+            else:
+                plan = lindblad.ShardedLindbladPlan(specs, devices, sim._interp_order)
+            with plan:
                 plan.set_state(sim._initial_state.full().reshape(-1))
                 prev = float(times[0])
                 for t_us in times:
@@ -935,24 +943,27 @@ class B200Backend(EmulatorBackend):
         return out
 
     def _run_sharded(self, devices: list[int]) -> Results:
-        """Noiseless sequence on a state vector split over ``devices`` (``B200Config(devices=...)``), streamed through
-        the evaluation times like the single-plan run."""
+        """A state split over ``devices`` (``B200Config(devices=...)``), streamed through the evaluation times like the
+        single-plan runs: the state vector of a noiseless sequence, or the density matrix of a master equation whose
+        noise is collapse operators only (``_sharded_master_equation``)."""
         from . import engine, sharded
         from ._lib import PB200Error
 
         sim = self._sim_obj
-        if sim.noise_model.noise_types:
-            raise NotImplementedError(
-                "a state vector split over `devices` runs noiseless sequences only; this one has the noise types "
-                f"{sorted(sim.noise_model.noise_types)}"
-            )
+        master = _sharded_master_equation(sim.noise_model)
         sim._validate_options({})
-        sim._check_supported()
+        if not master:
+            # the master equation runs exactly at any size here: no Monte-Carlo fallback needs a trajectory count
+            sim._check_supported()
         n_dev = engine.device_count()
         missing = sorted({d for d in devices if d >= n_dev})
         if missing:
             raise ValueError(f"`devices` names CUDA device(s) {missing}, but {n_dev} are visible")
-        res = Results(atom_order=tuple(sim._register.qubit_ids), total_duration=sim.total_duration_ns)
+        atom_order = tuple(sim._register.qubit_ids)
+        if master:
+            with engine.DevicePlan(sim._noiseless_spec(), sim._interp_order, devices[0]) as hplan:
+                return self._stream_density(hplan, atom_order, devices)[0]
+        res = Results(atom_order=atom_order, total_duration=sim.total_duration_ns)
         try:
             plan = sharded.ShardedPlan(sim._noiseless_spec(), devices, sim._interp_order)
         except PB200Error as e:
@@ -1009,6 +1020,28 @@ class B200Backend(EmulatorBackend):
                     self._replay(hplan, cleanres, res)
                     results.append(res)
             return Results.aggregate(results, **_state_aggregators(results))
+
+
+# noise types that are collapse operators of the master equation, with no stochastic part
+_COLLAPSE_NOISE = frozenset({"dephasing", "relaxation", "depolarizing", "eff_noise"})
+
+
+def _sharded_master_equation(noise_model: Any) -> bool:
+    """Does a run with ``devices`` split a density matrix (True) or a state vector (False, no noise)?  Raises
+    ``NotImplementedError`` with the reason for any noise model that neither covers."""
+    types = set(noise_model.noise_types)
+    if not types:
+        return False
+    if "leakage" in types:
+        raise NotImplementedError(
+            "a density matrix split over `devices` needs a d = 2 register; leakage (d = 3) is not sharded"
+        )
+    if not types <= _COLLAPSE_NOISE or _has_stochastic_noise(noise_model):
+        raise NotImplementedError(
+            "a state split over `devices` runs noiseless sequences and master equations without stochastic noise "
+            f"(dephasing, relaxation, depolarizing, eff_noise); this one has the noise types {sorted(types)}"
+        )
+    return True
 
 
 class B200LegacyBackend(pulser.backend.abc.Backend):

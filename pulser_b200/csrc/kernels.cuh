@@ -1098,7 +1098,9 @@ __device__ __forceinline__ void taylor_dint_setup(const TaylorArgs& a, long long
 // DISS: the master equation on vec(rho) (TaylorArgs::dw, df; the batch gather, whose per-bit table carries the column
 // drive -conj(omega)).  The dissipator sum of a chunk is a second accumulator, which does not fit in 128 registers
 // either: the same launch shape as CPLX.  A pair whose row bit lies in the tile reads its both-flip partner from shared
-// memory, one above the tile costs one more coalesced load per atom.
+// memory, one above the tile costs one more coalesced load per atom.  DISS with SHARD: vec(rho) split by its top row
+// bits (one trajectory); the per-bit table's entries of the shard bits drive the peer loads, and a pair whose row bit
+// is a shard bit reads its both-flip partner from that peer.
 // SRC32 / OUT32: the tail orders of a step (TaylorStep::k_lo), uniform drives of one state (or its shards) only.  chi_k (tile and
 // partners) is read as float2, chi_{k+1} and G_k are stored as float2; the arithmetic, the partner sums and the
 // accumulator stay fp64.  The single-precision tile fills the first 64 KiB of the tile's 128.
@@ -1108,10 +1110,10 @@ __global__ void __launch_bounds__(1 << (TBITS - RB),
                                   (CPLX || DISS) ? 1 : (65536 / ((1 << (TBITS - RB)) * (RB >= 3 ? 128 : 64))))
 stage_d2_taylor_kernel(const __grid_constant__ TaylorArgs a) {
     static_assert(RB >= 3, "chunks of 8 amplitudes per thread");
-    static_assert(UNIFORM || !SHARD, "shards carry one state with a uniform drive");
+    static_assert(UNIFORM || !SHARD || DISS, "shards carry one state with a uniform drive, or one density matrix");
     static_assert(NS == (UNIFORM ? 0 : 1) || NS == PB200_TAYLOR_SMAX, "one-shape table, or PB200_TAYLOR_SMAX shapes");
     static_assert(!CPLX || !REAL_G, "a complex drive gathers through the per-bit table");
-    static_assert(!DISS || (!UNIFORM && !SHARD && !CPLX), "a density matrix runs the batch gather, one device, one phase");
+    static_assert(!DISS || (!UNIFORM && !CPLX), "a density matrix runs the batch gather, one phase");
     static_assert(!(SRC32 || OUT32) || (UNIFORM && NS == 0 && !CPLX && !DISS),
                   "single-precision orders: one state, a uniform drive of one phase");
     using TT = std::conditional_t<SRC32, float2, c2>;   // element of chi_k
@@ -1190,9 +1192,10 @@ stage_d2_taylor_kernel(const __grid_constant__ TaylorArgs a) {
     const int nb = g.n_bits;
     // static per-qubit detuning weights: sum over (bits of base) + (bits of tid) + (register bits)
     double common = 0.0;
-    if (!UNIFORM && !SHAPES) {
+    if (!UNIFORM && !SHAPES) {   // a shard's global bits N - shard_bits + q are the bits of the shard index
         for (int p = 0; p < nb; ++p) {
-            const int bit = (int)(((base + tid) >> p) & 1);
+            int bit = (int)(((base + tid) >> p) & 1);
+            if (SHARD && p >= nb - a.shard_bits) bit = (a.shard >> (p - (nb - a.shard_bits))) & 1;
             common += (bit == a.from_is_one) ? tab[2 * nb + p] : 0.0;
         }
     }
@@ -1330,10 +1333,13 @@ stage_d2_taylor_kernel(const __grid_constant__ TaylorArgs a) {
         }
         double ex[RC], ey[RC];   // DISS: i D chi_k
         if constexpr (DISS) {
+            // SHARD: the dissipator reads the row and column bits of the global index (the shard index holds the top
+            // row bits)
+            const long long goff = SHARD ? (long long)a.shard << (nb - a.shard_bits) : 0LL;
             double dx[RC], dy[RC];
 #pragma unroll
             for (int r = 0; r < RC; ++r) {
-                const c2 w = taylor_diss_diag(a, idx[r], v[r]);
+                const c2 w = taylor_diss_diag(a, goff | idx[r], v[r]);
                 dx[r] = w.x; dy[r] = w.y;
             }
             if (a.diss_flip) {
@@ -1348,12 +1354,18 @@ stage_d2_taylor_kernel(const __grid_constant__ TaylorArgs a) {
                             const c2 t = tile_c2(tile[(tpos + r * NT) ^ (int)mask]);
                             pv[r] = make_double2(t.x, t.y);
                         }
+                    } else if (SHARD && pr >= nb - a.shard_bits) {
+                        // the row bit is shard bit q: the partner is the peer's, at the local index with the column
+                        // bit flipped (the column bits are all local)
+                        const TT* src = reinterpret_cast<const TT*>(a.peer[pr - (nb - a.shard_bits)]);
+#pragma unroll
+                        for (int r = 0; r < RC; ++r) pv[r] = ld_partner(src + (idx[r] ^ (1LL << pc)));
                     } else {
 #pragma unroll
                         for (int r = 0; r < RC; ++r) pv[r] = ld_partner(vsrc + (idx[r] ^ mask));
                     }
 #pragma unroll
-                    for (int r = 0; r < RC; ++r) taylor_diss_flip(a, idx[r], pr, pc, pv[r], dx[r], dy[r]);
+                    for (int r = 0; r < RC; ++r) taylor_diss_flip(a, goff | idx[r], pr, pc, pv[r], dx[r], dy[r]);
                 }
             }
 #pragma unroll
@@ -1847,12 +1859,13 @@ __global__ void dint_bounds_kernel(const double* dint, int n, int dim, int rstat
 
 // ---- measurement: bitstring weights, occupations, sampling ---------------------------------------------------
 // The weight of basis state s in trajectory traj: |psi_s|^2 of a ket (RHO = false: D amplitudes per trajectory), or
-// the diagonal element Re rho_ss of a density matrix (RHO = true: vec(rho)[r D + c] = rho_rc, D^2 entries per
-// trajectory, D = the dimension of the physical register).
+// the diagonal element Re rho_ss of a density matrix (RHO = true: vec(rho)[r D + c] = rho_rc, D = the dimension of
+// the physical register, `rows` rows of D entries per trajectory).  A density-matrix shard holds the rows
+// [r0, r0 + rows) of one matrix: p = its slice + r0 points at rho[r0, r0], and s counts from r0.
 template <bool RHO>
-__device__ __forceinline__ double basis_weight(const c2* p, long long traj, long long D, long long s) {
+__device__ __forceinline__ double basis_weight(const c2* p, long long traj, long long D, long long rows, long long s) {
     if constexpr (RHO) {
-        return p[traj * D * D + s * (D + 1)].x;
+        return p[traj * rows * D + s * (D + 1)].x;
     } else {
         const c2 v = p[traj * D + s];
         return v.x * v.x + v.y * v.y;
@@ -1861,35 +1874,38 @@ __device__ __forceinline__ double basis_weight(const c2* p, long long traj, long
 
 // weights[b(s)] += |psi_s|^2 (or rho_ss) with bit k of b = [digit_k(s) == one_digit], qudit 0 = most significant bit
 // (QutipResult._weights, qutip_result.py:101-158: reversal for ground-rydberg and the 3/4-level
-// marginalisation are both this rule).  A shard (d = 2) covers an aligned block of 2^L = D bitstrings: weights[b mod D].
+// marginalisation are both this rule).  A shard (d = 2) covers an aligned block of 2^L = rows bitstrings:
+// weights[b mod rows].  `rows` basis states from `off` on (rows = D but on a density-matrix shard, basis_weight).
 // A density matrix's diagonal may carry rounding noise below zero: it is clipped so the cumulative sum stays monotone.
 template <bool RHO>
-__global__ void bitstring_weights_kernel(const c2* psi, double* weights, long long D, int n, int dim, int one_digit,
-                                         long long off) {
-    for (long long s = blockIdx.x * (long long)blockDim.x + threadIdx.x; s < D;
+__global__ void bitstring_weights_kernel(const c2* psi, double* weights, long long D, long long rows, int n, int dim,
+                                         int one_digit, long long off) {
+    for (long long s = blockIdx.x * (long long)blockDim.x + threadIdx.x; s < rows;
          s += (long long)gridDim.x * blockDim.x) {
-        double p = basis_weight<RHO>(psi, 0, D, s);
+        double p = basis_weight<RHO>(psi, 0, D, rows, s);
         if constexpr (RHO) p = fmax(p, 0.0);
         long long rem = off + s, b = 0;
         for (int k = n - 1; k >= 0; --k) {  // qudit k <-> bit n-1-k
             if ((int)(rem % dim) == one_digit) b |= 1LL << (n - 1 - k);
             rem /= dim;
         }
-        if (dim == 2) weights[b & (D - 1)] = p;  // a permutation: no atomics needed
+        if (dim == 2) weights[b & (rows - 1)] = p;  // a permutation: no atomics needed
         else atomicAdd(weights + b, p);
     }
 }
 
-// occ[k] += sum_s |psi_s|^2 [digit_k(s) == digit]   (Occupation observable / <n_k>; rho_ss for RHO)
+// occ[k] += sum_s |psi_s|^2 [digit_k(s) == digit]   (Occupation observable / <n_k>; rho_ss for RHO; `rows` as in
+// bitstring_weights_kernel)
 template <bool RHO>
-__global__ void occupation_kernel(const c2* psi, double* occ, long long D, int n, int dim, int digit, long long off) {
+__global__ void occupation_kernel(const c2* psi, double* occ, long long D, long long rows, int n, int dim, int digit,
+                                  long long off) {
     extern __shared__ double socc[];
     for (int i = threadIdx.x; i < n; i += blockDim.x) socc[i] = 0.0;
     __syncthreads();
     const long long traj = blockIdx.y;
-    for (long long s = blockIdx.x * (long long)blockDim.x + threadIdx.x; s < D;
+    for (long long s = blockIdx.x * (long long)blockDim.x + threadIdx.x; s < rows;
          s += (long long)gridDim.x * blockDim.x) {
-        const double p = basis_weight<RHO>(psi, traj, D, s);
+        const double p = basis_weight<RHO>(psi, traj, D, rows, s);
         if (p == 0.0) continue;
         long long rem = off + s;
         for (int k = n - 1; k >= 0; --k) {
@@ -1904,23 +1920,23 @@ __global__ void occupation_kernel(const c2* psi, double* occ, long long D, int n
 // corr[traj][i*n+j] (i <= j) += sum_s |psi_s|^2 [digit_i(s) == digit][digit_j(s) == digit]
 // (CorrelationMatrix observable <n_i n_j>; the diagonal is the occupation).  A block stages 2048 probabilities and
 // their per-qudit match masks in shared memory; each warp then reduces a subset of the n(n+1)/2 pairs over them.
-// RHO: the weights are the diagonal rho_ss.
+// RHO: the weights are the diagonal rho_ss.  `rows` as in bitstring_weights_kernel.
 template <bool RHO>
-__global__ void __launch_bounds__(256) correlation_kernel(const c2* psi, double* corr, long long D, int n, int dim, int digit,
-                                                          long long off) {
+__global__ void __launch_bounds__(256) correlation_kernel(const c2* psi, double* corr, long long D, long long rows, int n,
+                                                          int dim, int digit, long long off) {
     constexpr int CH = 2048;
     __shared__ double sp[CH];
     __shared__ unsigned long long sm[CH];
     const long long traj = blockIdx.y;
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31, nw = blockDim.x >> 5;
     const int npairs = n * (n + 1) / 2;
-    for (long long base = blockIdx.x * (long long)CH; base < D; base += (long long)gridDim.x * CH) {
+    for (long long base = blockIdx.x * (long long)CH; base < rows; base += (long long)gridDim.x * CH) {
         for (int e = threadIdx.x; e < CH; e += blockDim.x) {
             const long long s = base + e;
             double p = 0.0;
             unsigned long long m = 0ull;
-            if (s < D) {
-                p = basis_weight<RHO>(psi, traj, D, s);
+            if (s < rows) {
+                p = basis_weight<RHO>(psi, traj, D, rows, s);
                 long long rem = off + s;
                 for (int k = n - 1; k >= 0; --k) {
                     if ((int)(rem % dim) == digit) m |= 1ull << k;
@@ -1987,8 +2003,9 @@ struct ExpD2Term {
 };
 struct ExpGenSite { c2 r; unsigned long long bit; };
 // where the partners live: src[shard ^ (f >> local_bits)] holds the slice of index bits above local_bits (one
-// pointer and shard 0 for a whole state; a shard group passes every shard's state, peers through peer access)
-struct ExpSrc { const c2* p[8]; int shard; int local_bits; };
+// pointer and shard 0 for a whole state; a shard group passes every shard's state, peers through peer access).
+// row_len > 0: RHO on the rows a density-matrix shard holds (expect_terms_d2_kernel), rows of row_len entries
+struct ExpSrc { const c2* p[8]; int shard; int local_bits; long long row_len; };
 
 __device__ __forceinline__ void exp_reduce(double re, double im, double* acc) {
     for (int o = 16; o > 0; o >>= 1) {
@@ -2008,7 +2025,9 @@ __device__ __forceinline__ void exp_reduce(double re, double im, double* acc) {
 
 // acc[traj] += sum_terms (blockIdx.y = trajectory; D = 2^local_bits amplitudes per trajectory; 256 threads).
 // RHO: src.p[0] holds density matrices of D^2 entries (no shards) and the term reads Tr(term rho) =
-// sum_g term[g, g ^ f] rho[g ^ f, g]: one element per (mask, g), never the whole matrix.
+// sum_g term[g, g ^ f] rho[g ^ f, g]: one element per (mask, g), never the whole matrix.  With src.row_len, the plan
+// holds the D rows g = (shard << local_bits) | s of one matrix (a shard), and the same trace is summed over the stored
+// rows instead: sum_g term[g ^ f, g] rho[g, g ^ f], the term's factors read at x = g ^ f.
 template <bool RHO>
 __global__ void __launch_bounds__(256) expect_terms_d2_kernel(const __grid_constant__ ExpSrc src, long long D,
                                                               const ExpD2Term* terms, const ExpGenSite* gens,
@@ -2016,7 +2035,7 @@ __global__ void __launch_bounds__(256) expect_terms_d2_kernel(const __grid_const
                                                               double* acc) {
     __shared__ ExpD2Term st[kExpChunkTerms];
     __shared__ ExpGenSite sg[kExpChunkSites];
-    const long long traj_off = (long long)blockIdx.y * (RHO ? D * D : D);
+    const long long traj_off = (long long)blockIdx.y * (RHO ? D * (src.row_len ? src.row_len : D) : D);
     const c2* own = src.p[src.shard] + traj_off;
     const unsigned long long off = (unsigned long long)src.shard << src.local_bits;
     const unsigned long long lmask = (unsigned long long)D - 1ull;
@@ -2037,18 +2056,20 @@ __global__ void __launch_bounds__(256) expect_terms_d2_kernel(const __grid_const
                 if (T.f != fcur) {  // uniform across the block: the loads of a warp are coalesced
                     fcur = T.f;
                     if constexpr (RHO) {
-                        q = own[(long long)((unsigned long long)s ^ fcur) * D + s];
+                        q = src.row_len ? own[s * src.row_len + (long long)(g ^ fcur)]
+                                        : own[(long long)((unsigned long long)s ^ fcur) * D + s];
                     } else {
                         c2 p = v;
                         if (fcur) p = src.p[src.shard ^ (int)(fcur >> src.local_bits)][traj_off + (long long)((unsigned long long)s ^ (fcur & lmask))];
                         q = {v.x * p.x + v.y * p.y, v.x * p.y - v.y * p.x};
                     }
                 }
-                if ((g & T.care) != T.val) continue;
+                const unsigned long long x = (RHO && src.row_len) ? g ^ fcur : g;   // the row of the term's element
+                if ((x & T.care) != T.val) continue;
                 c2 c = T.c;
                 for (int j = 0; j < T.sn; ++j)
-                    if (g & sg[T.s0 + j].bit) c = cmul(c, sg[T.s0 + j].r);
-                if (__popcll(g & T.z) & 1) c = {-c.x, -c.y};
+                    if (x & sg[T.s0 + j].bit) c = cmul(c, sg[T.s0 + j].r);
+                if (__popcll(x & T.z) & 1) c = {-c.x, -c.y};
                 re = fma(c.x, q.x, re); re = fma(-c.y, q.y, re);
                 im = fma(c.x, q.y, im); im = fma(c.y, q.x, im);
             }
@@ -2107,26 +2128,29 @@ __global__ void __launch_bounds__(256) expect_terms_kernel(const c2* psi, long l
 }
 
 // ---- reductions of density matrices vec(rho)[r D + c] = rho[r, c] (D^2 entries per trajectory, blockIdx.y) -------
-// acc[2 traj] += Re Tr rho
-__global__ void __launch_bounds__(256) density_trace_kernel(const c2* rho, long long D, double* acc) {
+// A density-matrix shard holds the rows [r0, r0 + rows) of one matrix (rows = D, r0 = 0 for whole matrices): the sums
+// below run over the rows a plan holds, so a shard's value is its share of the whole matrix's.
+// acc[2 traj] += Re Tr rho  (rho: the slice + r0, basis_weight)
+__global__ void __launch_bounds__(256) density_trace_kernel(const c2* rho, long long D, long long rows, double* acc) {
     double tr = 0.0;
-    for (long long r = blockIdx.x * (long long)blockDim.x + threadIdx.x; r < D; r += (long long)gridDim.x * blockDim.x)
-        tr += basis_weight<true>(rho, blockIdx.y, D, r);
+    for (long long r = blockIdx.x * (long long)blockDim.x + threadIdx.x; r < rows; r += (long long)gridDim.x * blockDim.x)
+        tr += basis_weight<true>(rho, blockIdx.y, D, rows, r);
     exp_reduce(tr, 0.0, acc);
 }
 
 // acc[traj] += <phi| rho |phi> = sum_{r,c} conj(phi_r) rho[r, c] phi_c (complex): a block per row at a time
-__global__ void __launch_bounds__(256) density_overlap_kernel(const c2* phi, const c2* rho, long long D, double* acc) {
-    const c2* m = rho + (long long)blockIdx.y * D * D;
+__global__ void __launch_bounds__(256) density_overlap_kernel(const c2* phi, const c2* rho, long long D, long long rows,
+                                                              long long r0, double* acc) {
+    const c2* m = rho + (long long)blockIdx.y * rows * D;
     double re = 0.0, im = 0.0;
-    for (long long r = blockIdx.x; r < D; r += gridDim.x) {
+    for (long long r = blockIdx.x; r < rows; r += gridDim.x) {
         double sr = 0.0, si = 0.0;  // sum_c rho[r, c] phi_c
         for (long long c = threadIdx.x; c < D; c += blockDim.x) {
             const c2 a = m[r * D + c], b = phi[c];
             sr = fma(a.x, b.x, sr); sr = fma(-a.y, b.y, sr);
             si = fma(a.x, b.y, si); si = fma(a.y, b.x, si);
         }
-        const c2 p = phi[r];  // conj(p) (sr + i si)
+        const c2 p = phi[r0 + r];  // conj(p) (sr + i si)
         re = fma(p.x, sr, re); re = fma(p.y, si, re);
         im = fma(p.x, si, im); im = fma(-p.y, sr, im);
     }
@@ -2195,6 +2219,66 @@ __global__ void __launch_bounds__(256) density_energy_kernel(const c2* rho, long
                 else if (digit == h.from[q]) { a = r + (long long)(h.to[q] - h.from[q]) * st; g.y = -g.y; }
                 else continue;
                 const c2 ya = density_h_row(h, m, D, a, r, unused);
+                e2 = fma(g.x, ya.x, e2); e2 = fma(-g.y, ya.y, e2);
+            }
+            st *= h.dim;
+        }
+    }
+    exp_reduce(e1, e2, acc);
+}
+
+// (rho H)[b, a] = sum_c rho[b, c] H[c, a] over c = a and the drive transitions of a, from row b of rho alone (m + b D:
+// the row as the plan stores it); diag = H[a, a].  H[c, a] = conj(H[a, c]): the elements density_h_row reads, conjugated
+__device__ __forceinline__ c2 density_row_h(const DensityH& h, const c2* row, long long a, double& diag) {
+    diag = h.dint ? h.dint[a] : 0.0;
+    double yr = 0.0, yi = 0.0;
+    long long rem = a, st = 1;
+    for (int k = h.n - 1; k >= 0; --k) {
+        const int digit = (int)(rem % h.dim);
+        rem /= h.dim;
+        for (int q = 0; q < h.n_drives; ++q) {
+            const c2 g = h.g[q][k];
+            if (digit == h.to[q]) {   // H[c, a] = H[.. from .., .. to ..] = conj(g)
+                const c2 v = row[a + (long long)(h.from[q] - h.to[q]) * st];
+                yr = fma(g.x, v.x, yr); yr = fma(g.y, v.y, yr);
+                yi = fma(g.x, v.y, yi); yi = fma(-g.y, v.x, yi);
+            } else if (digit == h.from[q]) {   // H[c, a] = g
+                const c2 v = row[a + (long long)(h.to[q] - h.from[q]) * st];
+                yr = fma(g.x, v.x, yr); yr = fma(-g.y, v.y, yr);
+                yi = fma(g.x, v.y, yi); yi = fma(g.y, v.x, yi);
+                diag -= h.th[q][k];
+            }
+        }
+        st *= h.dim;
+    }
+    const c2 v = row[a];
+    return {fma(diag, v.x, yr), fma(diag, v.y, yi)};
+}
+
+// The rows [r0, r0 + rows) of one density matrix (a shard's): acc[0] += Re sum_b (rho H)[b, b], acc[1] += Re sum_b
+// sum_a (rho H)[b, a] H[a, b] over a = b and the drive partners of b.  Tr(H rho) = Tr(rho H) and Tr(H^2 rho) =
+// Tr(rho H^2): the same sums as density_energy_kernel's, ordered so that every element read lies in a stored row.
+__global__ void __launch_bounds__(256) density_energy_rows_kernel(const c2* rho, long long D, long long rows, long long r0,
+                                                                  const __grid_constant__ DensityH h, double* acc) {
+    double e1 = 0.0, e2 = 0.0;
+    for (long long bl = blockIdx.x * (long long)blockDim.x + threadIdx.x; bl < rows; bl += (long long)gridDim.x * blockDim.x) {
+        const long long b = r0 + bl;
+        const c2* row = rho + bl * D;
+        double diag, unused;
+        const c2 y = density_row_h(h, row, b, diag);
+        e1 += y.x;
+        e2 = fma(diag, y.x, e2);
+        long long rem = b, st = 1;
+        for (int k = h.n - 1; k >= 0; --k) {
+            const int digit = (int)(rem % h.dim);
+            rem /= h.dim;
+            for (int q = 0; q < h.n_drives; ++q) {
+                c2 g = h.g[q][k];  // H[a, b]
+                long long a;
+                if (digit == h.to[q]) { a = b + (long long)(h.from[q] - h.to[q]) * st; g.y = -g.y; }
+                else if (digit == h.from[q]) a = b + (long long)(h.to[q] - h.from[q]) * st;
+                else continue;
+                const c2 ya = density_row_h(h, row, a, unused);
                 e2 = fma(g.x, ya.x, e2); e2 = fma(-g.y, ya.y, e2);
             }
             st *= h.dim;

@@ -284,6 +284,9 @@ static const std::vector<TaylorVariant>& taylor_variants() {
         // master equation on vec(rho): the batch gather (the column drive is -conj(omega)), one or several shapes
         {false, false, false, 1,  false, stage_d2_taylor_kernel<false, false, TB, RBC, false, 1, false, true>,  RBC, S::TileTable, true, true},
         {false, false, false, SM, false, stage_d2_taylor_kernel<false, false, TB, RBC, false, SM, false, true>, RBC, S::Shapes,    true, true},
+        // ... split over state-vector shards by its top row bits
+        {false, false, true,  1,  false, stage_d2_taylor_kernel<false, false, TB, RBC, true, 1, false, true>,   RBC, S::TileTable, false, true},
+        {false, false, true,  SM, false, stage_d2_taylor_kernel<false, false, TB, RBC, true, SM, false, true>,  RBC, S::Shapes,    false, true},
     };
     return v;
 }
@@ -1589,7 +1592,7 @@ static void propagate_mcwf(Plan& P, double t_start, double t_stop, const pb200_r
                 device_sum(P, d_occ.get(), occ.size(), occ.data(), [&] {
                     for (int dgt = 0; dgt < P.dim; ++dgt)
                         occupation_kernel<false><<<(unsigned)std::max<long long>(nb, 1), 256, sizeof(double) * P.n, P.stream>>>(
-                            psi, d_occ.get() + (size_t)dgt * P.n, P.D, P.n, P.dim, dgt, 0LL);
+                            psi, d_occ.get() + (size_t)dgt * P.n, P.D, P.D, P.n, P.dim, dgt, 0LL);
                 });
             }
             // channel (op, qudit) with probability <L^+L>
@@ -3305,40 +3308,43 @@ static void launch_expect(const Plan& P, long long D, const ExpHost& H, const ch
                                                         H.n_chunks, d_acc);
 }
 
-// occ[count][n] of `count` trajectories at src (RHO: density matrices of D^2 entries) of D basis states
+// occ[count][n] of `count` trajectories at src (RHO: density matrices of D^2 entries) of D basis states: the `rows`
+// of them from basis state `off` on (rows = D, off = the shard offset, but on a density-matrix shard; basis_weight)
 template <bool RHO>
-static void reduce_occupation(const Plan& P, const c2* src, long long D, int n, int count, int digit, double* occ) {
+static void reduce_occupation(const Plan& P, const c2* src, long long D, long long rows, long long off, int n, int count,
+                              int digit, double* occ) {
     CUDA_CHECK(cudaSetDevice(P.desc.device));
     DevBuf<double> d_occ(P, (size_t)count * n);
-    const long long blocks = std::min<long long>((D + 255) / 256, (long long)P.sm_count * 4);
+    const long long blocks = std::min<long long>((rows + 255) / 256, (long long)P.sm_count * 4);
     dim3 grid((unsigned)std::max<long long>(blocks, 1), (unsigned)count);
     device_sum(P, d_occ.get(), d_occ.size(), occ, [&] {
-        occupation_kernel<RHO><<<grid, 256, sizeof(double) * n, P.stream>>>(src, d_occ.get(), D, n, P.dim, digit,
-                                                                          P.shard_offset());
+        occupation_kernel<RHO><<<grid, 256, sizeof(double) * n, P.stream>>>(src, d_occ.get(), D, rows, n, P.dim, digit, off);
     });
 }
 
 // corr[count][n][n] (symmetric) of `count` trajectories at src, as reduce_occupation
 template <bool RHO>
-static void reduce_correlation(const Plan& P, const c2* src, long long D, int n, int count, int digit, double* corr) {
+static void reduce_correlation(const Plan& P, const c2* src, long long D, long long rows, long long off, int n, int count,
+                               int digit, double* corr) {
     CUDA_CHECK(cudaSetDevice(P.desc.device));
     const size_t nn = (size_t)n * n;
     DevBuf<double> d_c(P, count * nn);
-    const long long blocks = std::min<long long>((D + 2047) / 2048, (long long)P.sm_count * 4);
+    const long long blocks = std::min<long long>((rows + 2047) / 2048, (long long)P.sm_count * 4);
     dim3 grid((unsigned)std::max<long long>(blocks, 1), (unsigned)count);
     device_sum(P, d_c.get(), d_c.size(), corr, [&] {
-        correlation_kernel<RHO><<<grid, 256, 0, P.stream>>>(src, d_c.get(), D, n, P.dim, digit, P.shard_offset());
+        correlation_kernel<RHO><<<grid, 256, 0, P.stream>>>(src, d_c.get(), D, rows, n, P.dim, digit, off);
     });
     for (int c = 0; c < count; ++c)  // the kernel fills i <= j
         for (int i = 0; i < n; ++i)
             for (int j = 0; j < i; ++j) corr[c * nn + (size_t)i * n + j] = corr[c * nn + (size_t)j * n + i];
 }
 
-// Bitstring shots of one state (RHO: of one density matrix's diagonal) of D basis states on n qudits: the weights of
-// the 2^nbits bitstrings, their inclusive prefix sum and one binary search per uniform (pb200_state_sample).
+// Bitstring shots of one state (RHO: of one density matrix's diagonal) of D basis states on n qudits, `rows` of them from
+// basis state `off` on (reduce_occupation): the weights of the 2^nbits bitstrings, their inclusive prefix sum and one
+// binary search per uniform (pb200_state_sample).
 template <bool RHO>
-static void sample_bitstrings(const Plan& P, const c2* src, long long D, int n, int nbits, int one_digit,
-                              const double* uniforms, int n_shots, int64_t* out) {
+static void sample_bitstrings(const Plan& P, const c2* src, long long D, long long rows, long long off, int n, int nbits,
+                              int one_digit, const double* uniforms, int n_shots, int64_t* out) {
     if (nbits > 30) fail(PB200_ERR_UNSUPPORTED, "bitstring sampling: at most 30 qudits (32-bit item count of the prefix scan)");
     CUDA_CHECK(cudaSetDevice(P.desc.device));
     const long long M = 1LL << nbits;
@@ -3346,9 +3352,9 @@ static void sample_bitstrings(const Plan& P, const c2* src, long long D, int n, 
     DevBuf<long long> d_idx(P, (size_t)n_shots);
     CUDA_CHECK(cudaMemsetAsync(d_w.get(), 0, sizeof(double) * (size_t)M, P.stream));
     CUDA_CHECK(cudaMemcpyAsync(d_u.get(), uniforms, sizeof(double) * (size_t)n_shots, cudaMemcpyHostToDevice, P.stream));
-    const long long blocks = std::min<long long>((D + 255) / 256, (long long)P.sm_count * 8);
+    const long long blocks = std::min<long long>((rows + 255) / 256, (long long)P.sm_count * 8);
     bitstring_weights_kernel<RHO><<<(unsigned)std::max<long long>(blocks, 1), 256, 0, P.stream>>>(
-        src, d_w.get(), D, n, P.dim, one_digit, P.shard_offset());
+        src, d_w.get(), D, rows, n, P.dim, one_digit, off);
     CUDA_CHECK(cudaGetLastError());
     size_t tmp_bytes = 0;
     CUDA_CHECK(cub::DeviceScan::InclusiveSum(nullptr, tmp_bytes, d_w.get(), d_w.get(), (int)M, P.stream));
@@ -3671,7 +3677,6 @@ int pb200_plan_set_dissipator(pb200_plan* h, int32_t n_pairs, const double* gene
     if (!h || !generators) fail(PB200_ERR_INVALID, "null argument");
     Plan& P = h->p;
     if (P.dim > 3) fail(PB200_ERR_UNSUPPORTED, "dissipator: d <= 3 only");
-    if (P.shard_bits) fail(PB200_ERR_UNSUPPORTED, "dissipator: not on state-vector shards");
     if (n_pairs < 1 || 2 * n_pairs != P.n) fail(PB200_ERR_INVALID, "dissipator: the plan must hold 2*n_pairs qudits");
     const int dd = P.dim * P.dim;
     P.diss_gen.assign(n_pairs, std::vector<cplx>((size_t)dd * dd));
@@ -3807,7 +3812,8 @@ int pb200_state_occupation(pb200_plan* h, int32_t traj0, int32_t count, int32_t 
     Plan& P = h->p;
     check_traj_range(P, traj0, count, "pb200_state_occupation");
     if (digit < 0 || digit >= P.dim) fail(PB200_ERR_INVALID, "digit out of range");
-    reduce_occupation<false>(P, P.buf[P.cur].get() + (size_t)traj0 * P.D, P.D, P.n, count, digit, occ);
+    reduce_occupation<false>(P, P.buf[P.cur].get() + (size_t)traj0 * P.D, P.D, P.D, P.shard_offset(), P.n, count, digit,
+                             occ);
     PB200_CATCH
 }
 
@@ -3818,7 +3824,8 @@ int pb200_state_correlation(pb200_plan* h, int32_t traj0, int32_t count, int32_t
     check_traj_range(P, traj0, count, "pb200_state_correlation");
     if (digit < 0 || digit >= P.dim) fail(PB200_ERR_INVALID, "digit out of range");
     if (P.n > 40) fail(PB200_ERR_UNSUPPORTED, "too many qudits for the correlation matrix");
-    reduce_correlation<false>(P, P.buf[P.cur].get() + (size_t)traj0 * P.D, P.D, P.n, count, digit, corr);
+    reduce_correlation<false>(P, P.buf[P.cur].get() + (size_t)traj0 * P.D, P.D, P.D, P.shard_offset(), P.n, count, digit,
+                              corr);
     PB200_CATCH
 }
 
@@ -3894,8 +3901,8 @@ int pb200_state_sample(pb200_plan* h, int32_t traj, int32_t one_digit, const dou
     if (traj < 0 || traj >= P.B) fail(PB200_ERR_INVALID, "trajectory out of range");
     if (one_digit < 0 || one_digit >= P.dim) fail(PB200_ERR_INVALID, "one_digit out of range");
     // a shard samples its own slice: M = its 2^L bitstrings, out[i] = the low L bits of the global bitstring
-    sample_bitstrings<false>(P, P.buf[P.cur].get() + (size_t)traj * P.D, P.D, P.n, P.n - P.shard_bits, one_digit,
-                             uniforms, n_shots, out);
+    sample_bitstrings<false>(P, P.buf[P.cur].get() + (size_t)traj * P.D, P.D, P.D, P.shard_offset(), P.n, P.n - P.shard_bits,
+                             one_digit, uniforms, n_shots, out);
     PB200_CATCH
 }
 
@@ -3927,20 +3934,24 @@ int pb200_state_device_ptr(pb200_plan* h, void** dptr) {
 }
 
 // ---- reductions of density matrices (plans with a dissipator) ------------------------------------------------------
-// The plan holds vec(rho) of N = n / 2 physical qudits: D = dim^N, trajectory b at buf + b D^2.
-struct DensityGeom { int n; long long D; };
+// The plan holds vec(rho) of N = n / 2 physical qudits: D = dim^N, trajectory b at buf + b D^2.  A shard of vec(rho)
+// (one trajectory) holds the rows [r0, r0 + rows) of rho, rows = D / 2^shard_bits: each reduction returns the share of
+// those rows, which the caller sums over the shards (the kernels never read a peer's rows).
+struct DensityGeom { int n; long long D, rows, r0; };
 
 static DensityGeom density_geom(const Plan& P, const char* who) {
     if (!P.has_diss)
         fail(PB200_ERR_UNSUPPORTED, "%s: the plan holds state vectors, not a density matrix (no dissipator)", who);
     if (!P.state_set) fail(PB200_ERR_STATE, "%s: no state set", who);
-    DensityGeom G{P.n / 2, 1};
+    DensityGeom G{P.n / 2, 1, 0, 0};
     for (int k = 0; k < G.n; ++k) G.D *= P.dim;
+    G.rows = G.D >> P.shard_bits;
+    G.r0 = (long long)P.shard * G.rows;
     return G;
 }
 
 static const c2* density_at(const Plan& P, const DensityGeom& G, int traj) {
-    return P.buf[P.cur].get() + (size_t)traj * G.D * G.D;
+    return P.buf[P.cur].get() + (size_t)traj * G.rows * G.D;
 }
 
 int pb200_density_trace(pb200_plan* h, int32_t traj0, int32_t count, double* trace) {
@@ -3952,10 +3963,10 @@ int pb200_density_trace(pb200_plan* h, int32_t traj0, int32_t count, double* tra
     CUDA_CHECK(cudaSetDevice(P.desc.device));
     DevBuf<double> d_acc(P, 2 * (size_t)count);
     std::vector<double> acc(2 * (size_t)count);
-    const long long blocks = std::min<long long>((G.D + 255) / 256, (long long)P.sm_count * 4);
+    const long long blocks = std::min<long long>((G.rows + 255) / 256, (long long)P.sm_count * 4);
     dim3 grid((unsigned)std::max<long long>(blocks, 1), (unsigned)count);
     device_sum(P, d_acc.get(), acc.size(), acc.data(), [&] {
-        density_trace_kernel<<<grid, 256, 0, P.stream>>>(density_at(P, G, traj0), G.D, d_acc.get());
+        density_trace_kernel<<<grid, 256, 0, P.stream>>>(density_at(P, G, traj0) + G.r0, G.D, G.rows, d_acc.get());
     });
     for (int c = 0; c < count; ++c) trace[c] = acc[2 * (size_t)c];
     PB200_CATCH
@@ -3968,7 +3979,7 @@ int pb200_density_occupation(pb200_plan* h, int32_t traj0, int32_t count, int32_
     const DensityGeom G = density_geom(P, "pb200_density_occupation");
     check_traj_range(P, traj0, count, "pb200_density_occupation");
     if (digit < 0 || digit >= P.dim) fail(PB200_ERR_INVALID, "pb200_density_occupation: digit out of range");
-    reduce_occupation<true>(P, density_at(P, G, traj0), G.D, G.n, count, digit, occ);
+    reduce_occupation<true>(P, density_at(P, G, traj0) + G.r0, G.D, G.rows, G.r0, G.n, count, digit, occ);
     PB200_CATCH
 }
 
@@ -3979,7 +3990,7 @@ int pb200_density_correlation(pb200_plan* h, int32_t traj0, int32_t count, int32
     const DensityGeom G = density_geom(P, "pb200_density_correlation");
     check_traj_range(P, traj0, count, "pb200_density_correlation");
     if (digit < 0 || digit >= P.dim) fail(PB200_ERR_INVALID, "pb200_density_correlation: digit out of range");
-    reduce_correlation<true>(P, density_at(P, G, traj0), G.D, G.n, count, digit, corr);
+    reduce_correlation<true>(P, density_at(P, G, traj0) + G.r0, G.D, G.rows, G.r0, G.n, count, digit, corr);
     PB200_CATCH
 }
 
@@ -3992,15 +4003,20 @@ int pb200_density_expect(pb200_plan* h, int32_t traj0, int32_t count, const pb20
     check_traj_range(P, traj0, count, "pb200_density_expect");
     check_op_terms(op, G.n, P.dim, "pb200_density_expect");
     std::fill(out, out + 2 * (size_t)count, 0.0);
-    const ExpHost H = exp_host(op, G.n, P.dim, G.n);
+    const int local_bits = G.n - P.shard_bits;
+    const ExpHost H = exp_host(op, G.n, P.dim, local_bits);
     if (H.n_chunks == 0) return PB200_OK;
     CUDA_CHECK(cudaSetDevice(P.desc.device));
     const DevBuf<char> X = upload_exp(H, P);
     DevBuf<double> d_acc(P, 2 * (size_t)count);
     const c2* rho = density_at(P, G, traj0);
     ExpSrc src{};
-    src.p[0] = rho; src.shard = 0; src.local_bits = G.n;
-    device_sum(P, d_acc.get(), d_acc.size(), out, [&] { launch_expect<true>(P, G.D, H, X.get(), src, rho, count, d_acc.get()); });
+    src.p[0] = rho; src.shard = 0; src.local_bits = local_bits;
+    if (P.shard_bits) {   // the stored rows of a shard (d = 2): rows (shard << local_bits) | s of D entries
+        src.p[P.shard] = rho; src.shard = P.shard; src.row_len = G.D;
+    }
+    device_sum(P, d_acc.get(), d_acc.size(), out,
+               [&] { launch_expect<true>(P, G.rows, H, X.get(), src, rho, count, d_acc.get()); });
     PB200_CATCH
 }
 
@@ -4020,7 +4036,9 @@ int pb200_density_energy(pb200_plan* h, pb200_plan* ham, double t_us, int32_t tr
     if (Q.n != G.n || Q.dim != P.dim)
         fail(PB200_ERR_INVALID, "pb200_density_energy: the Hamiltonian plan has %d qudits of dimension %d, the density "
              "matrix %d of dimension %d", Q.n, Q.dim, G.n, P.dim);
-    if (Q.desc.device != P.desc.device) fail(PB200_ERR_UNSUPPORTED, "pb200_density_energy: plans on different devices");
+    if (Q.desc.device != P.desc.device)
+        fail(PB200_ERR_UNSUPPORTED, "pb200_density_energy: plans on different devices (a shard on device %d needs a "
+             "Hamiltonian plan of its own there)", P.desc.device);
     if (G.n > kDensityMaxQudits) fail(PB200_ERR_UNSUPPORTED, "pb200_density_energy: at most %d qudits", kDensityMaxQudits);
     check_drives_set(Q, "pb200_density_energy");
     const ExpParams E = params_at(Q, t_us);
@@ -4039,10 +4057,15 @@ int pb200_density_energy(pb200_plan* h, pb200_plan* ham, double t_us, int32_t tr
     CUDA_CHECK(cudaSetDevice(P.desc.device));
     DevBuf<double> d_acc(P, 2 * (size_t)count);
     std::vector<double> acc(2 * (size_t)count);
-    const long long blocks = (G.D + 255) / 256;
+    const long long blocks = (G.rows + 255) / 256;
     dim3 grid((unsigned)std::max<long long>(blocks, 1), (unsigned)count);
     device_sum(P, d_acc.get(), acc.size(), acc.data(), [&] {
-        density_energy_kernel<<<grid, 256, 0, P.stream>>>(density_at(P, G, traj0), G.D, dh, d_acc.get());
+        // a shard sums over the rows it stores (Tr(rho H), Tr(rho H^2)): (H rho)[a, r] would read the rows of its peers
+        if (P.shard_bits)
+            density_energy_rows_kernel<<<grid, 256, 0, P.stream>>>(density_at(P, G, traj0), G.D, G.rows, G.r0, dh,
+                                                                   d_acc.get());
+        else
+            density_energy_kernel<<<grid, 256, 0, P.stream>>>(density_at(P, G, traj0), G.D, dh, d_acc.get());
     });
     for (int c = 0; c < count; ++c) { energy[c] = acc[2 * (size_t)c]; h2[c] = acc[2 * (size_t)c + 1]; }
     PB200_CATCH
@@ -4058,10 +4081,10 @@ int pb200_density_overlap(pb200_plan* h, int32_t traj0, int32_t count, const dou
     c2* d_phi = P.buf[(P.cur + 1) % 3].get();  // scratch of B D^2 >= D amplitudes
     CUDA_CHECK(cudaMemcpyAsync(d_phi, phi, sizeof(c2) * (size_t)G.D, cudaMemcpyHostToDevice, P.stream));
     DevBuf<double> d_acc(P, 2 * (size_t)count);
-    const long long blocks = std::min<long long>(G.D, (long long)P.sm_count * 8);
+    const long long blocks = std::min<long long>(G.rows, (long long)P.sm_count * 8);
     dim3 grid((unsigned)std::max<long long>(blocks, 1), (unsigned)count);
     device_sum(P, d_acc.get(), d_acc.size(), out, [&] {
-        density_overlap_kernel<<<grid, 256, 0, P.stream>>>(d_phi, density_at(P, G, traj0), G.D, d_acc.get());
+        density_overlap_kernel<<<grid, 256, 0, P.stream>>>(d_phi, density_at(P, G, traj0), G.D, G.rows, G.r0, d_acc.get());
     });
     PB200_CATCH
 }
@@ -4075,7 +4098,8 @@ int pb200_density_sample(pb200_plan* h, int32_t traj, int32_t one_digit, const d
     const DensityGeom G = density_geom(P, "pb200_density_sample");
     if (traj < 0 || traj >= P.B) fail(PB200_ERR_INVALID, "pb200_density_sample: trajectory out of range");
     if (one_digit < 0 || one_digit >= P.dim) fail(PB200_ERR_INVALID, "pb200_density_sample: one_digit out of range");
-    sample_bitstrings<true>(P, density_at(P, G, traj), G.D, G.n, G.n, one_digit, uniforms, n_shots, out);
+    sample_bitstrings<true>(P, density_at(P, G, traj) + G.r0, G.D, G.rows, G.r0, G.n, G.n - P.shard_bits, one_digit,
+                            uniforms, n_shots, out);
     PB200_CATCH
 }
 
@@ -4165,8 +4189,13 @@ int pb200_shards_link(pb200_plan** plans, int32_t count) {
         if (P.has_interaction != G[0]->has_interaction || (P.has_interaction && !P.dint_shared))
             fail(PB200_ERR_INVALID, "pb200_shards_link: every shard needs the same (shared) interaction");
         if (!P.tabs_set[0][0]) fail(PB200_ERR_STATE, "pb200_shards_link: the drive of shard %d is not set", i);
+        // a master equation: every shard carries the same dissipator, so that each one's a-priori bound (w_knot, m_0)
+        // and with it the group's schedule are those of the unsharded plan
+        if (P.has_diss != G[0]->has_diss || P.diss_gen != G[0]->diss_gen)
+            fail(PB200_ERR_INVALID, "pb200_shards_link: the shards carry different dissipators");
         if (!taylor_prepare(P)) fail(PB200_ERR_UNSUPPORTED, "pb200_shards_link: no Taylor propagator for this sequence: %s", g_taylor_why);
-        if (!P.tay.drive_uniform)
+        // vec(rho) runs the batch gather, whose per-bit table holds the column drive -conj(omega)
+        if (!P.tay.drive_uniform && !P.has_diss)
             fail(PB200_ERR_UNSUPPORTED, "pb200_shards_link: shards need one drive coefficient for every qubit (per-qubit drive "
                                         "amplitudes are not sharded; per-qubit detuning is)");
     }

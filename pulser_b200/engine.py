@@ -113,6 +113,7 @@ class DevicePlan:
         self.shard = None if shard is None else (int(shard[0]), int(shard[1]))
         self.D = s0.hilbert_dim if shard is None else s0.hilbert_dim >> self.shard[0]
         self.interp_order = interp_order
+        self.device = device
         self._handle = C.c_void_p()
         times = np.ascontiguousarray(s0.sampling_times, dtype=np.float64)
         desc = PlanDesc()
