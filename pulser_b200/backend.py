@@ -628,7 +628,8 @@ class B200Config(EmulationConfig[B200State]):
     A noiseless single-state run is then split over ``len(devices)`` plans (``pulser_b200.sharded.ShardedPlan``), so
     registers larger than one GPU's memory can run; so is the density matrix of a master equation whose noise is
     dephasing, relaxation, depolarizing or eff_noise only (``pulser_b200.lindblad.ShardedLindbladPlan``), exact where
-    one device would need Monte-Carlo trajectories.  Default ``None``: one plan on one device.
+    one device would need Monte-Carlo trajectories, under a drive of one phase (a master equation whose drive phase
+    moves runs on one device, on the Taylor propagator as well).  Default ``None``: one plan on one device.
     """
 
     _enforce_expected_kwargs = True

@@ -346,14 +346,16 @@ __device__ __forceinline__ void taylor_signed_add(double gx, double gy, double s
 // register-block bits (tile bits TBITS-RB .. TBITS-1) are register moves, flips of the tile bits
 // [jstart, TBITS-RB) are independent LDS.128 from `tile`.
 // SIGNED (per-bit table only): q also receives the signed sum  sum_k sg_k f_k chi_k,  sg_k = +1 where the amplitude's bit
-// k is to_bit, with f_k the factor p receives (the complex-drive Taylor stage).  T: c2, or float2 for a single-precision
-// tile (LDS.64).
-template <bool UNIFORM, bool REAL_G, int TBITS, int RB, bool SIGNED = false, class T = c2>
+// k is to_bit, with f_k the factor p receives (the complex-drive Taylor stage).  COLSIGN: vec(rho) with a complex drive,
+// sg_k is negated on the column bits (bit positions below ncol), whose y-factor is i conj(unit) rather than i unit.
+// T: c2, or float2 for a single-precision tile (LDS.64).
+template <bool UNIFORM, bool REAL_G, int TBITS, int RB, bool SIGNED = false, bool COLSIGN = false, class T = c2>
 __device__ __forceinline__ void rb_tile_gather(const PassGeom& g, const T* tile, const double* __restrict__ tab, int tid,
                                                int to_bit, int jstart, bool skip_smem, const c2 (&v)[1 << RB],
                                                double (&pr)[1 << RB], double (&pi)[1 << RB], double (&qr)[1 << RB],
-                                               double (&qi)[1 << RB]) {
+                                               double (&qi)[1 << RB], int ncol = 0) {
     static_assert(!SIGNED || !UNIFORM, "signed sums of the per-bit table gather");
+    static_assert(!COLSIGN || SIGNED, "the column sign belongs to the signed sums");
     constexpr int R = 1 << RB;
     constexpr int NT = 1 << (TBITS - RB);
     // --- flips inside the register block (tile bits TBITS-RB .. TBITS-1) ---
@@ -361,9 +363,11 @@ __device__ __forceinline__ void rb_tile_gather(const PassGeom& g, const T* tile,
     for (int q = 0; q < RB; ++q) {
         const int j = TBITS - RB + q;
         double gx = 0.0, gyt = 0.0;
+        bool col = false;
         if (!UNIFORM) {
             const int p = (j < g.lo_bits) ? j : (j - g.lo_bits + g.hi_shift);
             gx = tab[2 * p]; gyt = tab[2 * p + 1];
+            col = COLSIGN && p < ncol;
         }
 #pragma unroll
         for (int r = 0; r < R; ++r) {
@@ -376,7 +380,7 @@ __device__ __forceinline__ void rb_tile_gather(const PassGeom& g, const T* tile,
                 }
             } else if constexpr (SIGNED) {
                 const double gy = (bit == to_bit) ? gyt : -gyt;
-                taylor_signed_add(gx, gy, bit == to_bit ? 1.0 : -1.0, pv.x, pv.y, pr[r], pi[r], qr[r], qi[r]);
+                taylor_signed_add(gx, gy, ((bit == to_bit) != col) ? 1.0 : -1.0, pv.x, pv.y, pr[r], pi[r], qr[r], qi[r]);
             } else {
                 const double gy = (bit == to_bit) ? gyt : -gyt;
                 pr[r] = fma(gx, pv.x, pr[r]); pr[r] = fma(-gy, pv.y, pr[r]);
@@ -391,12 +395,14 @@ __device__ __forceinline__ void rb_tile_gather(const PassGeom& g, const T* tile,
             const int bit = (tid >> j) & 1;
             const int ptid = tid ^ (1 << j);
             double gx = 0.0, gy = 0.0;
+            bool col = false;
             if (!UNIFORM) {
                 const int p = (j < g.lo_bits) ? j : (j - g.lo_bits + g.hi_shift);
                 gx = tab[2 * p];
                 gy = (bit == to_bit) ? tab[2 * p + 1] : -tab[2 * p + 1];
+                col = COLSIGN && p < ncol;
             }
-            const double sg = (bit == to_bit) ? 1.0 : -1.0;
+            const double sg = ((bit == to_bit) != col) ? 1.0 : -1.0;
 #pragma unroll
             for (int r = 0; r < R; ++r) {
                 const c2 pv = tile_c2(tile[ptid + r * NT]);
@@ -1101,6 +1107,10 @@ __device__ __forceinline__ void taylor_dint_setup(const TaylorArgs& a, long long
 // memory, one above the tile costs one more coalesced load per atom.  DISS with SHARD: vec(rho) split by its top row
 // bits (one trajectory); the per-bit table's entries of the shard bits drive the peer loads, and a pair whose row bit
 // is a shard bit reads its both-flip partner from that peer.
+// CPLX with DISS: vec(rho) under a drive whose phase moves.  Row bit k sees unit omega, column bit k -conj(unit)
+// conj(omega) (the table holds f = unit on row bits and -conj(unit) on column bits), so the drive part of H_j is
+// om_j G + omi_j G' where G' is the CPLX signed sum with the sign of every column bit (position < n_pair) negated: the
+// column's y-factor is i conj(unit) = -i f.  The dissipator acts on chi_k alone, as without CPLX.  One state only.
 // SRC32 / OUT32: the tail orders of a step (TaylorStep::k_lo), uniform drives of one state (or its shards) only.  chi_k (tile and
 // partners) is read as float2, chi_{k+1} and G_k are stored as float2; the arithmetic, the partner sums and the
 // accumulator stay fp64.  The single-precision tile fills the first 64 KiB of the tile's 128.
@@ -1113,7 +1123,8 @@ stage_d2_taylor_kernel(const __grid_constant__ TaylorArgs a) {
     static_assert(UNIFORM || !SHARD || DISS, "shards carry one state with a uniform drive, or one density matrix");
     static_assert(NS == (UNIFORM ? 0 : 1) || NS == PB200_TAYLOR_SMAX, "one-shape table, or PB200_TAYLOR_SMAX shapes");
     static_assert(!CPLX || !REAL_G, "a complex drive gathers through the per-bit table");
-    static_assert(!DISS || (!UNIFORM && !CPLX), "a density matrix runs the batch gather, one phase");
+    static_assert(!DISS || (!UNIFORM && !(CPLX && SHARD)),
+                  "a density matrix runs the batch gather; a moving phase on whole density matrices only");
     static_assert(!(SRC32 || OUT32) || (UNIFORM && NS == 0 && !CPLX && !DISS),
                   "single-precision orders: one state, a uniform drive of one phase");
     using TT = std::conditional_t<SRC32, float2, c2>;   // element of chi_k
@@ -1127,6 +1138,7 @@ stage_d2_taylor_kernel(const __grid_constant__ TaylorArgs a) {
     // drive of non-zero phase (G = sum_k (unit |to><from|_k + h.c.): one complex factor per partner and two
     // accumulators per amplitude instead of the P and Q sums)
     constexpr bool TAB = !(UNIFORM && REAL_G);
+    constexpr bool COLSIGN = CPLX && DISS;   // the signed sums change sign on the column bits of vec(rho)
     extern __shared__ __align__(128) unsigned char smem_raw[];
     TT* tile = reinterpret_cast<TT*>(smem_raw);
     __shared__ __align__(8) uint64_t mbar;
@@ -1232,13 +1244,15 @@ stage_d2_taylor_kernel(const __grid_constant__ TaylorArgs a) {
             double gx = 0.0, gy = 0.0;
             if (TAB) { gx = tab[2 * p]; gy = (bit == to_bit) ? tab[2 * p + 1] : -tab[2 * p + 1]; }
             const TT* src = vsrc + (i0 ^ (1LL << p));
+            const bool col = COLSIGN && p < a.n_pair;
             double2 raw[RC];
 #pragma unroll
             for (int r = 0; r < RC; ++r) raw[r] = ld_partner(src + r * NT);
 #pragma unroll
             for (int r = 0; r < RC; ++r) {
                 if constexpr (CPLX) {
-                    taylor_signed_add(gx, gy, bit == to_bit ? 1.0 : -1.0, raw[r].x, raw[r].y, pr[r], pi[r], dr[r], di[r]);
+                    taylor_signed_add(gx, gy, ((bit == to_bit) != col) ? 1.0 : -1.0, raw[r].x, raw[r].y, pr[r], pi[r], dr[r],
+                                      di[r]);
                 } else if (!TAB) {
                     pr[r] += raw[r].x; pi[r] += raw[r].y;
                 } else {
@@ -1292,12 +1306,14 @@ stage_d2_taylor_kernel(const __grid_constant__ TaylorArgs a) {
         double qd[RC];   // the Q sums of rb_tile_gather: not used by the two instantiations below
 #pragma unroll
         for (int r = 0; r < RC; ++r) v[r] = tile_c2(sub[tid + r * NT]);
-        if constexpr (CPLX) rb_tile_gather<false, false, STB, 3, true>(g, sub, tab, tid, to_bit, 0, false, v, pr, pi, dr, di);
+        if constexpr (CPLX)
+            rb_tile_gather<false, false, STB, 3, true, COLSIGN>(g, sub, tab, tid, to_bit, 0, false, v, pr, pi, dr, di, a.n_pair);
         else rb_tile_gather<!TAB, !TAB, STB, 3>(g, sub, tab, tid, to_bit, 0, false, v, pr, pi, qd, qd);
 #pragma unroll
         for (int q = 0; q < CB; ++q) {   // flips of the chunk bits
             const int p = STB + q;
             const int bit = (c >> q) & 1;
+            const bool col = COLSIGN && p < a.n_pair;
             double gx = 0.0, gy = 0.0;
             if (TAB) { gx = tab[2 * p]; gy = (bit == to_bit) ? tab[2 * p + 1] : -tab[2 * p + 1]; }
             const TT* other = tile + ((c ^ (1 << q)) << STB);
@@ -1305,7 +1321,7 @@ stage_d2_taylor_kernel(const __grid_constant__ TaylorArgs a) {
             for (int r = 0; r < RC; ++r) {
                 const c2 pv = tile_c2(other[tid + r * NT]);
                 if constexpr (CPLX) {
-                    taylor_signed_add(gx, gy, bit == to_bit ? 1.0 : -1.0, pv.x, pv.y, pr[r], pi[r], dr[r], di[r]);
+                    taylor_signed_add(gx, gy, ((bit == to_bit) != col) ? 1.0 : -1.0, pv.x, pv.y, pr[r], pi[r], dr[r], di[r]);
                 } else if (!TAB) {
                     pr[r] += pv.x; pi[r] += pv.y;
                 } else {
@@ -1379,10 +1395,11 @@ stage_d2_taylor_kernel(const __grid_constant__ TaylorArgs a) {
             if constexpr (SHAPES) {
                 const double* lc = bl + c * RC;
                 const double* lt = at + tid;
-                taylor_epilogue<RC, RC / 4, SHARD, true>(
-                    a, idx, v, pr, pi, [&](int r, int J) { return lt[J * NT] + lc[(J << RB) + r]; }, voff, dint, qx, qy);
+                taylor_epilogue<RC, RC / 4, SHARD, true, DISS>(
+                    a, idx, v, pr, pi, [&](int r, int J) { return lt[J * NT] + lc[(J << RB) + r]; }, voff, dint, qx, qy,
+                    ex, ey);
             } else {
-                taylor_epilogue<RC, RC / 4, SHARD, true>(a, idx, v, pr, pi, off, voff, dint, qx, qy);
+                taylor_epilogue<RC, RC / 4, SHARD, true, DISS>(a, idx, v, pr, pi, off, voff, dint, qx, qy, ex, ey);
             }
         } else if constexpr (SHAPES) {
             const double* lc = bl + c * RC;
@@ -1399,7 +1416,7 @@ stage_d2_taylor_kernel(const __grid_constant__ TaylorArgs a) {
 
 // any register size (N < 13 in particular): one thread per amplitude, partners through global loads.  CPLX: the
 // complex-drive step, G' = i (P - Q) as well (stage_d2_taylor_kernel).  DISS: the master equation on vec(rho), the
-// both-flip partners through global loads too.
+// both-flip partners through global loads too.  Both: the signed sum changes sign on the column bits.
 template <bool CPLX = false, bool DISS = false>
 __global__ void __launch_bounds__(256) stage_d2_taylor_small_kernel(const __grid_constant__ TaylorArgs a) {
     const long long s = (long long)blockIdx.x * blockDim.x + threadIdx.x;
@@ -1420,7 +1437,8 @@ __global__ void __launch_bounds__(256) stage_d2_taylor_small_kernel(const __grid
             const int bit = (int)((s >> p) & 1);
             const double gx = tab[2 * p], gy = (bit == a.to_bit) ? tab[2 * p + 1] : -tab[2 * p + 1];
             if constexpr (CPLX) {
-                taylor_signed_add(gx, gy, bit == a.to_bit ? 1.0 : -1.0, raw.x, raw.y, gxs, gys, dx, dy);
+                const bool col = DISS && p < a.n_pair;   // vec(rho): the column bits' signed sum changes sign
+                taylor_signed_add(gx, gy, ((bit == a.to_bit) != col) ? 1.0 : -1.0, raw.x, raw.y, gxs, gys, dx, dy);
             } else {
                 gxs = fma(gx, raw.x, gxs); gxs = fma(-gy, raw.y, gxs);
                 gys = fma(gx, raw.y, gys); gys = fma(gy, raw.x, gys);

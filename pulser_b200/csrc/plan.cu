@@ -284,6 +284,9 @@ static const std::vector<TaylorVariant>& taylor_variants() {
         // master equation on vec(rho): the batch gather (the column drive is -conj(omega)), one or several shapes
         {false, false, false, 1,  false, stage_d2_taylor_kernel<false, false, TB, RBC, false, 1, false, true>,  RBC, S::TileTable, true, true},
         {false, false, false, SM, false, stage_d2_taylor_kernel<false, false, TB, RBC, false, SM, false, true>, RBC, S::Shapes,    true, true},
+        // ... under a drive whose phase moves inside the step (column bits: the signed sum changes sign)
+        {false, false, false, 1,  true,  stage_d2_taylor_kernel<false, false, TB, RBC, false, 1, true, true>,   RBC, S::TileTable, true, true},
+        {false, false, false, SM, true,  stage_d2_taylor_kernel<false, false, TB, RBC, false, SM, true, true>,  RBC, S::Shapes,    true, true},
         // ... split over state-vector shards by its top row bits
         {false, false, true,  1,  false, stage_d2_taylor_kernel<false, false, TB, RBC, true, 1, false, true>,   RBC, S::TileTable, false, true},
         {false, false, true,  SM, false, stage_d2_taylor_kernel<false, false, TB, RBC, true, SM, false, true>,  RBC, S::Shapes,    false, true},
@@ -430,6 +433,10 @@ struct Plan {
         int ns = 0;                        // detuning shapes, <= PB200_TAYLOR_SMAX
         PiecewiseCubic<double> shape[PB200_TAYLOR_SMAX];   // M_s(t)
         std::vector<cplx> a;               // [B][N] per qubit
+        // vec(rho) under a moving phase (taylor_prepare): the column qudits' factors are their rows' a, and the table
+        // holds -conj(a unit) on the column bits, the drive -conj(unit omega) of any unit.  A constant phase keeps the
+        // column factors of the fit (a_col unit = -conj(a_row unit) for the reference unit only)
+        bool conj_cols = false;
         std::vector<double> c;             // [B][N][ns]
         double a_sum_max = 0.0;            // max over trajectories of sum_k |a|
         double c_sum_max[PB200_TAYLOR_SMAX] = {};   // max over trajectories of sum_k |c_s|
@@ -2113,7 +2120,8 @@ static std::vector<double> taylor_table(const Plan& P, cplx unit) {
         double* t = tab.data() + (size_t)b * stride;
         for (int k = 0; k < N; ++k) {
             const int p = N - 1 - k;
-            const cplx g = C.a[(size_t)b * N + k] * unit;
+            const cplx au = C.a[(size_t)b * N + k] * unit;
+            const cplx g = (C.conj_cols && k >= N / 2) ? -std::conj(au) : au;   // column qudit k of vec(rho)
             t[2 * p] = g.real(); t[2 * p + 1] = g.imag();
             for (int s = 0; s < C.ns; ++s) t[2 * N + s * N + p] = C.c[((size_t)b * N + k) * C.ns + s];
         }
@@ -2160,7 +2168,10 @@ static Plan::DissTaylor diss_taylor_analyse(const std::vector<std::vector<cplx>>
 }
 
 static const char* const kWhyMovingPhaseRho =
-    "the drive phase moves: on a density matrix the column drive -conj(omega(t)) is not a multiple of omega(t)";
+    "the drive phase moves and the drive rows are not multiples of one row: on a density matrix a moving phase needs "
+    "one global drive shape (per-qubit static factors allowed), whose columns drive -conj(omega(t))";
+static const char* const kWhyMovingPhaseShards =
+    "the drive phase moves: vec(rho) shards take a drive of one phase (a moving phase runs on whole density matrices)";
 
 // the drive relative to the phase of its largest sample (real and imaginary parts), per-(trajectory, qubit) static
 // factors, device table
@@ -2183,13 +2194,40 @@ static bool taylor_prepare(Plan& P) {
     for (int b = 0; b < B; ++b)
         for (int k = 0; k < N; ++k) { crow[(size_t)b * N + k] = &coef_pc(b, k); drow[(size_t)b * N + k] = &det_pc(b, k); }
     const int npc = nt - 1;   // pieces of every interpolant; sample i = c0[i], the last one = y_last
-    const SeparableFit F = taylor_separable(
-        B, N, nt,
-        [&](int b, int k, int i) { const PiecewiseCubic<cplx>* pc = crow[(size_t)b * N + k]; return i < npc ? pc->c0[i] : pc->y_last; },
-        [&](int b, int k, int i) { const PiecewiseCubic<double>* pc = drow[(size_t)b * N + k]; return i < npc ? pc->c0[i] : pc->y_last; },
-        PB200_TAYLOR_SMAX);
+    auto cs = [&](int b, int k, int i) { const PiecewiseCubic<cplx>* pc = crow[(size_t)b * N + k]; return i < npc ? pc->c0[i] : pc->y_last; };
+    auto ds = [&](int b, int k, int i) { const PiecewiseCubic<double>* pc = drow[(size_t)b * N + k]; return i < npc ? pc->c0[i] : pc->y_last; };
+    SeparableFit F = taylor_separable(B, N, nt, cs, ds, PB200_TAYLOR_SMAX);
+    // vec(rho) (lindblad.doubled_spec): column qudit k + N/2 drives -conj(row k).  Under a moving phase that is no
+    // multiple of the row's drive, so the drive is fitted on the row half (each column qudit reads its row's samples, and
+    // gets the row's factor a) and the table conjugates on the column bits (TaylorCache::conj_cols).  The detuning rows
+    // are fitted whole, as with a constant phase
+    const int n2 = N / 2;
+    auto doubled_fit = [&](SeparableFit& out) {
+        double scale = 0.0;
+        for (int b = 0; b < B; ++b)
+            for (int k = 0; k < N; ++k)
+                for (int i = 0; i < nt; ++i) scale = std::max(scale, std::abs(cs(b, k, i)));
+        for (int b = 0; b < B; ++b)
+            for (int k = 0; k < n2; ++k)
+                for (int i = 0; i < nt; ++i)
+                    if (std::abs(cs(b, k + n2, i) + std::conj(cs(b, k, i))) > 2e-13 * std::max(scale, 1e-300)) {
+                        out.why = kWhyMovingPhaseRho;
+                        return false;
+                    }
+        out = taylor_separable(B, N, nt, [&](int b, int k, int i) { return cs(b, k < n2 ? k : k - n2, i); }, ds,
+                               PB200_TAYLOR_SMAX);
+        if (out.why == kWhyDriveRows) out.why = kWhyMovingPhaseRho;
+        return out.ok;
+    };
+    bool conj_cols = false;
+    if (!F.ok && P.has_diss && F.why == kWhyDriveRows) {
+        SeparableFit Fd;
+        if (!doubled_fit(Fd)) { g_taylor_why = C.why = Fd.why; return false; }
+        F = Fd;
+        conj_cols = true;
+    }
     if (!F.ok) {
-        g_taylor_why = C.why = (P.has_diss && F.why == kWhyDriveRows) ? kWhyMovingPhaseRho : F.why;
+        g_taylor_why = C.why = F.why;
         return false;
     }
     const double scale = F.scale;
@@ -2213,7 +2251,21 @@ static bool taylor_prepare(Plan& P) {
     C.om.y_last = (ref.y_last * cu).real();
     C.om_im.y_last = (ref.y_last * cu).imag();
     if (!C.phase_moves) C.om_im = PiecewiseCubic<double>();   // constant phase: the real drive of before, exactly
-    else if (P.has_diss) { g_taylor_why = C.why = kWhyMovingPhaseRho; return false; }
+    if (P.has_diss && C.phase_moves) {
+        if (P.shard_bits) { g_taylor_why = C.why = kWhyMovingPhaseShards; return false; }
+        // a phase that moves within the whole fit's tolerance: the row-half fit all the same (the reference row, and with
+        // it unit and omega, is the same one: a column sample is never larger than its row's)
+        if (!conj_cols) {
+            SeparableFit Fd;
+            if (!doubled_fit(Fd) || Fd.ref_b != F.ref_b || Fd.ref_k != F.ref_k || Fd.big != F.big) {
+                g_taylor_why = C.why = kWhyMovingPhaseRho;
+                return false;
+            }
+            F = Fd;
+            conj_cols = true;
+        }
+    }
+    C.conj_cols = conj_cols;
     C.unit = {unit.real(), unit.imag()};
     C.a = F.a; C.c = F.c; C.ns = F.ns;
     for (int s = 0; s < C.ns; ++s) C.shape[s] = make_interpolant<double>(P.times.data(), F.m[s].data(), nt, P.desc.interp_order);
@@ -2352,8 +2404,8 @@ static bool taylor_worthwhile(Plan& P, double gtol) {
     int cnt = 0;
     for (char c : rough) cnt += c;
     if (4 * cnt > nt) { g_taylor_why = "splines too rough for multi-interval polynomial steps"; return false; }
-    // (iii) a master equation: the alternative is the splitting path, not Krylov; measured faster at every size it runs
-    // (experiments/lindblad_cost.py, DESIGN.md section 3a)
+    // (iii) a master equation: the alternative is the splitting path, not Krylov; measured faster at every size it runs,
+    // under a moving drive phase too (experiments/lindblad_cost.py, lindblad_phase_cost.py, DESIGN.md section 3a)
     if (P.has_diss) return true;
     taylor_knot_widths(P);
     double wsum = 0.0;
@@ -2493,8 +2545,8 @@ static void launch_taylor_order(const Plan& P, bool tiled, const TaylorArgs& a, 
     const bool diss = a.n_pair > 0;
     if (!tiled) {
         const dim3 grid((unsigned)((P.D + 255) / 256), (unsigned)P.B);
-        if (diss && !cplx) stage_d2_taylor_small_kernel<false, true><<<grid, 256, 0, P.stream>>>(a);
-        else if (diss) fail(PB200_ERR_UNSUPPORTED, "no Taylor stage kernel for a dissipator with a complex drive");
+        if (diss && cplx) stage_d2_taylor_small_kernel<true, true><<<grid, 256, 0, P.stream>>>(a);
+        else if (diss) stage_d2_taylor_small_kernel<false, true><<<grid, 256, 0, P.stream>>>(a);
         else if (cplx) stage_d2_taylor_small_kernel<true><<<grid, 256, 0, P.stream>>>(a);
         else stage_d2_taylor_small_kernel<false><<<grid, 256, 0, P.stream>>>(a);
         return;

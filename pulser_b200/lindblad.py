@@ -15,11 +15,14 @@ the dissipator of single-qudit collapse operators factorises into one
 ``d^2 x d^2`` matrix per (row digit, column digit) pair (``pair_op_kernel``).
 Where every atom's generator is the same and has no entry that flips exactly
 one bit of the (row, column) pair -- dephasing, relaxation, depolarizing, any
-set of collapse operators each diagonal or off-diagonal -- and the drive keeps
-one phase, ``pb200_propagate`` runs the time-dependent Taylor propagator with
-the dissipator inside the series (no splitting error; default tolerance 1e-10).
-Otherwise, or with ``integrator=1 / 2``, the two are combined by symmetric
-splitting + Richardson extrapolation (see include/pulser_b200.h).
+set of collapse operators each diagonal or off-diagonal -- and the drive is one
+global shape (per-qubit static factors allowed) whose phase may move in time
+(phase shifts, phase jumps between pulses, Ramsey pairs, EOM drift correction:
+the column qudits then drive ``-conj(omega(t))``, which the stage forms from the
+same partner loads), ``pb200_propagate`` runs the time-dependent Taylor
+propagator with the dissipator inside the series (no splitting error; default
+tolerance 1e-10).  Otherwise, or with ``integrator=1 / 2``, the two are combined
+by symmetric splitting + Richardson extrapolation (see include/pulser_b200.h).
 
 ``ShardedLindbladPlan`` splits vec(rho) of one sequence over 2, 4 or 8 state-vector shards
 (``pulser_b200.sharded``): the top bits of the 2N-qubit index are the top row bits, so a shard
@@ -222,8 +225,9 @@ class ShardedLindbladPlan:
     The reductions are the ``pb200_density_*`` of each shard, i.e. its rows' share, summed here.  The methods mirror
     those of ``LindbladPlan`` that ``B200Backend._stream_density`` and ``DeviceDensityView`` call (one trajectory).
 
-    Scope: d = 2, one phase of the drive, a dissipator without single-bit-flip entries, Ising interaction, no SLM mask;
-    anything else raises ``NotImplementedError`` with its reason.
+    Scope: d = 2, a drive of one phase (a phase that moves in time runs on an unsharded ``LindbladPlan``), a dissipator
+    without single-bit-flip entries, Ising interaction, no SLM mask; anything else raises ``NotImplementedError`` with
+    its reason.
     """
 
     def __init__(self, specs: HamiltonianSpec | Sequence[HamiltonianSpec], devices: Sequence[int],

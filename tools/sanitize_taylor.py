@@ -31,3 +31,13 @@ for n in (3, 7):
         lp.set_state(np.eye(1, 2**n, 2**n - 1)[0])
         st = lp.propagate(0.0, spec.sampling_times[-1], integrator=3)
         print("lindblad n", n, "launches", st["n_launches"], "trace", np.trace(lp.get_rho()[0]).real)
+# master equation under a moving drive phase (CPLX + DISS kernels): a phase jump of pi/2 mid-sweep, N = 3 (small kernel)
+# and N = 7 (tiled)
+ph = np.where(np.arange(len(amp)) < len(amp) // 2, 0.0, np.pi / 2)
+for n in (3, 7):
+    spec = W.ising_global_spec(W.disc_register(n, 16.0, 5.0, 3), W.C6_LEVEL_60, amp, det, phase=ph)
+    spec.collapse_ops = ops
+    with LindbladPlan(spec) as lp:
+        lp.set_state(np.eye(1, 2**n, 2**n - 1)[0])
+        st = lp.propagate(0.0, spec.sampling_times[-1], integrator=3)
+        print("lindblad phase jump n", n, "launches", st["n_launches"], "trace", np.trace(lp.get_rho()[0]).real)
